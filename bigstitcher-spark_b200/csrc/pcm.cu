@@ -6,10 +6,11 @@
 // to 16 so every row is 128 B aligned):
 //
 //   k_fft_x_r2c      uint16/float crop -> blended mirrored extension + zero pad -> R2C along x
-//   k_fft_strided    (mode 0) forward FFT along y, in place, both spectra in one launch
-//   k_fft_strided    (mode 1) forward z FFT of A and B, unit-magnitude normalisation,
+//   k_fft_col540     forward FFT along y, in place, both spectra in one launch
+//   k_fft_xpower_col540  forward z FFT of A and B, unit-magnitude normalisation,
 //                    conj(A)*B, forward z FFT of the product      [reads 2S, writes S]
-//   k_fft_strided    (mode 0) forward y FFT of the product
+//   k_fft_col540     forward y FFT of the product
+//                    (other padded y / z sizes than 540: k_fft_strided_pipe / k_fft_xpower_pipe / k_fft_strided)
 //   k_fft_x_c2r      conj + C2R along x, in place -> real PCM (row pitch 2*pitch floats)
 //   k_peaks          periodic 6-neighbour local maxima, per-CTA top-K
 //   k_gather27       3x3x3 neighbourhoods of the K peaks (sub-pixel fit runs on the host)
@@ -801,6 +802,101 @@ __global__ void __launch_bounds__(PCM_THREADS, 2) k_fft_xpower_pipe(const __grid
 }
 
 // ------------------------------------------------------------------------------------------
+// Strided passes of the static 540-point plan (540 = 20 x 27, RegFft2): tiles of 540 rows x TC columns, data in
+// registers from the global load to the global store, one shared-memory exchange and one block barrier per
+// transform.  Persistent CTAs; the next tile's loads go out into the stage-1 registers as soon as the current
+// tile's stage 1 has written them to the exchange buffer, so they are in flight under stage 2 and the stores (a
+// register double buffer would need twice the stage-1 registers; a cp.async staging tile would add two
+// shared-memory passes per element and cost the occupancy a second 69 KB buffer allows).
+//
+// TC = 16 (128 B row segments), NT = 320: stage 1 has 27 x 16 = 432 items of 20 points (threads 0..111 take two),
+// stage 2 has 20 x 16 = 320 items of 27 points (one per thread).  One CTA per SM (a 69 KB exchange buffer each for
+// A, B and the product in the z pass).
+#define COL540_TC 16
+#define COL540_NT 320
+typedef RegFft2<20, 27, COL540_TC, COL540_NT> Col540;      // forward: 20 first, then 27
+typedef RegFft2<27, 20, COL540_TC, COL540_NT> Col540Q;     // cross-power product: starts on Col540's output
+static_assert(Col540Q::IT1 == Col540::IT2 && Col540Q::I1 == Col540::I2, "product transform must start in registers");
+
+__device__ __forceinline__ void col540_tw(float2* tw, const float2* __restrict__ g) {
+    for (int i = threadIdx.x; i < Col540::N; i += blockDim.x) tw[i] = g[i];
+}
+
+// forward y FFT in place, tiles of both spectra (p.n_tiles = tiles_x * n_other * n_img)
+__global__ void __launch_bounds__(COL540_NT, 1) k_fft_col540(const __grid_constant__ StridedPipeArgs p) {
+    const StridedArgs& a = p.s;
+    float2* tw = bs_sm;
+    auto tile_ptr = [&](int t) -> float2* {
+        const int tx = t % p.tiles_x, r = t / p.tiles_x;
+        const int o = r % p.n_other, im = r / p.n_other;
+        return (im ? a.b : a.a) + (size_t)o * a.ostride + (size_t)tx * COL540_TC;
+    };
+    Col540::In v;
+    int t = blockIdx.x;
+    if (t < p.n_tiles) Col540::load(v, tile_ptr(t), a.estride);
+    col540_tw(tw, a.tw);
+    __syncthreads();
+    for (int it = 0; t < p.n_tiles; t += gridDim.x, ++it) {
+        float2* x = bs_sm + Col540::N + (it & 1) * Col540::XSIZE;   // two exchange buffers: one barrier per tile
+        Col540::stage1(v, x, tw);
+        const int tn = t + gridDim.x;
+        if (tn < p.n_tiles) Col540::load(v, tile_ptr(tn), a.estride);
+        __syncthreads();
+        Col540::stage2(x, [&](const float2 (&w)[27], int, int k1, int c) { Col540::store(w, tile_ptr(t), a.estride, k1, c); });
+    }
+}
+
+// z cross-power: forward z FFT of A and B, unit-magnitude normalisation and conj(A) * B, then the forward FFT of
+// the product as RegFft2<27, 20>, which starts on the registers holding the product.  A's spectrum stays in its
+// exchange buffer (each stage-2 item writes its 27 outputs back to the 27 slots it read), so B's loads can be in
+// flight under A's stage 2 without the 54 registers of A's column on top.  Three exchange buffers (A, B, product),
+// three barriers per tile.  B(t) loads under A's stage 2, A(t+1) under the product's stage 2 and the stores.
+__global__ void __launch_bounds__(COL540_NT, 1) k_fft_xpower_col540(const __grid_constant__ StridedPipeArgs p) {
+    const StridedArgs& a = p.s;
+    float2* tw = bs_sm;
+    float2* XA = bs_sm + Col540::N;
+    float2* XB = XA + Col540::XSIZE;
+    float2* XQ = XB + Col540::XSIZE;
+    auto tile_off = [&](int t) -> size_t {
+        return (size_t)(t / p.tiles_x) * a.ostride + (size_t)(t % p.tiles_x) * COL540_TC;
+    };
+    Col540::In v;
+    Col540Q::In q;   // q[u] = product column of Col540's stage-2 item u
+    int t = blockIdx.x;
+    if (t < p.n_tiles) Col540::load(v, a.a + tile_off(t), a.estride);
+    col540_tw(tw, a.tw);
+    __syncthreads();
+    for (; t < p.n_tiles; t += gridDim.x) {
+        const size_t off = tile_off(t);
+        Col540::stage1(v, XA, tw);
+        Col540::load(v, a.b + off, a.estride);
+        __syncthreads();
+        Col540::stage2(XA, [&](const float2 (&w)[27], int, int k1, int c) {
+            float2* s = Col540::slot(XA, k1, c);
+#pragma unroll
+            for (int k2 = 0; k2 < 27; ++k2) s[k2 * COL540_TC] = w[k2];
+        });
+        Col540::stage1(v, XB, tw);
+        __syncthreads();
+        Col540::stage2(XB, [&](const float2 (&w)[27], int u, int k1, int c) {
+            const float2* s = Col540::slot(XA, k1, c);
+#pragma unroll
+            for (int k2 = 0; k2 < 27; ++k2) {
+                const float2 x = unit_or_zero(s[k2 * COL540_TC], a.thresh);
+                const float2 y = unit_or_zero(w[k2], a.thresh);
+                q[u][k2] = make_float2(x.x * y.x + x.y * y.y, x.x * y.y - x.y * y.x);  // conj(x) * y
+            }
+        });
+        Col540Q::stage1(q, XQ, tw);
+        const int tn = t + gridDim.x;
+        if (tn < p.n_tiles) Col540::load(v, a.a + tile_off(tn), a.estride);
+        __syncthreads();
+        float2* g = a.a + off;
+        Col540Q::stage2(XQ, [&](const float2 (&w)[20], int, int k1, int c) { Col540Q::store(w, g, a.estride, k1, c); });
+    }
+}
+
+// ------------------------------------------------------------------------------------------
 // x pass, complex -> real, in place
 
 template <class F>
@@ -995,9 +1091,6 @@ __global__ void __launch_bounds__(PCM_THREADS) k_peaks(const __grid_constant__ P
 // compile-time specialisations: padded 512^3 overlaps -> 540^3 (x half-length 270)
 typedef FftStatic<270, 4, 17, 2, PCM_THREADS, 9, 6, 5> FftX270;
 typedef FftStatic<270, 3, 9, 2, PCM_THREADS, 9, 6, 5> FftX270L8;
-typedef FftStatic<540, 3, 8, 1, PCM_THREADS, 9, 10, 6> FftS540;
-typedef FftStatic<540, 2, 4, 1, PCM_THREADS, 9, 10, 6> FftS540T4;
-typedef FftStatic<540, 3, 8, 1, PCM_THREADS, 27, 20> FftS540R2;   // two-stage variant (radix 27 x 20)
 
 // ------------------------------------------------------------------------------------------
 // Pearson sums for all candidate shifts in one launch
@@ -1481,8 +1574,9 @@ static int pcm_geometry(bs_ctx* ctx, const long long dims[3], const int ext[3], 
     const bool allow_static = env_int("BS_FFT_STATIC", 1) != 0;
     g->static_x = allow_static && g->M == FftX270::N && (g->lshift_x == FftX270::LSHIFT || g->lshift_x == FftX270L8::LSHIFT) &&
                   (g->lshift_r2c == 3 || g->lshift_r2c == 4);
-    g->static_y = allow_static && g->P[1] == FftS540::N && g->tshift_y == FftS540::LSHIFT;
-    g->static_z = allow_static && g->P[2] == FftS540::N && (g->tshift_z == FftS540::LSHIFT || g->tshift_z == FftS540T4::LSHIFT);
+    // k_fft_col540 / k_fft_xpower_col540: the pitch (a multiple of 16) always divides into 16-column tiles
+    g->static_y = allow_static && g->P[1] == Col540::N;
+    g->static_z = allow_static && g->P[2] == Col540::N;
     return BS_OK;
 }
 
@@ -1545,6 +1639,19 @@ static int set_smem(bs_ctx* ctx, const void* fn, size_t bytes) {
     return BS_OK;
 }
 
+// n_img: 1 or 2 spectra through k_fft_col540 (y), 0 for the cross-power k_fft_xpower_col540 (z)
+static void launch_col540(bs_ctx* ctx, const StridedArgs& a, int tiles_x, int n_other, int n_img) {
+    StridedPipeArgs pp;
+    pp.s = a;
+    pp.tiles_x = tiles_x;
+    pp.n_other = n_other;
+    pp.n_tiles = tiles_x * n_other * (n_img ? n_img : 1);
+    const int nctas = std::min(pp.n_tiles, ctx->sm_count);   // one CTA per SM (shared memory, registers)
+    const size_t smem = (Col540::N + (n_img ? 2 : 3) * (size_t)Col540::XSIZE) * sizeof(float2);
+    if (n_img) k_fft_col540<<<nctas, COL540_NT, smem, ctx->stream>>>(pp);
+    else k_fft_xpower_col540<<<nctas, COL540_NT, smem, ctx->stream>>>(pp);
+}
+
 // forward pipeline up to the real PCM in ws.spec_a (row pitch 2*pitch floats)
 static int pcm_compute_pcm(bs_ctx* ctx, const void* d1, const void* d2, int dtype, const PcmGeometry& g,
                            PcmDeviceTables* t) {
@@ -1563,15 +1670,10 @@ static int pcm_compute_pcm(bs_ctx* ctx, const void* d1, const void* d2, int dtyp
         if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_tma<FftX270>, 0))) return rc;
         if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_tma<FftGeneric>, 0))) return rc;
         if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r<FftX270L8>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_strided<FftS540>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_strided<FftS540T4>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_strided<FftS540R2>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_strided_pipe<FftS540>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_strided_pipe<FftS540R2>, 0))) return rc;
         if ((rc = set_smem(ctx, (const void*)k_fft_strided_pipe<FftGeneric>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_xpower_pipe<FftS540R2>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_xpower_pipe<FftS540>, 0))) return rc;
         if ((rc = set_smem(ctx, (const void*)k_fft_xpower_pipe<FftGeneric>, 0))) return rc;
+        if ((rc = set_smem(ctx, (const void*)k_fft_col540, 0))) return rc;
+        if ((rc = set_smem(ctx, (const void*)k_fft_xpower_col540, 0))) return rc;
         if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r<FftX270>, 0))) return rc;
         ctx->pcm_attr_done = true;
     }
@@ -1644,7 +1746,9 @@ static int pcm_compute_pcm(bs_ctx* ctx, const void* d1, const void* d2, int dtyp
         dim3 grid(g.pitch >> g.tshift_y, g.P[2], 2);
         bs_launch_scope sc(ctx, "fft_y");
         const size_t smem_pipe = ((size_t)((g.P[1] + 1) & ~1) + 3 * (size_t)g.P[1] * (1 << g.tshift_y)) * sizeof(float2);
-        if (env_int("BS_FFT_Y_PIPE", 1) && smem_pipe <= PCM_SMEM_MAX) {
+        if (g.static_y) {
+            launch_col540(ctx, a, g.pitch / COL540_TC, g.P[2], 2);
+        } else if (smem_pipe <= PCM_SMEM_MAX) {
             StridedPipeArgs pp;
             pp.s = a;
             pp.tiles_x = g.pitch >> g.tshift_y;
@@ -1652,11 +1756,8 @@ static int pcm_compute_pcm(bs_ctx* ctx, const void* d1, const void* d2, int dtyp
             pp.n_tiles = pp.tiles_x * pp.n_other * 2;
             const int per_sm = std::max(1, std::min(2, (int)(PCM_SMEM_MAX / (smem_pipe + 1024))));
             const int nctas = std::min(pp.n_tiles, ctx->sm_count * per_sm);
-            if (g.static_y && env_int("BS_FFT_Y_R2", 1)) k_fft_strided_pipe<FftS540R2><<<nctas, PCM_THREADS, smem_pipe, ctx->stream>>>(pp);
-            else if (g.static_y) k_fft_strided_pipe<FftS540><<<nctas, PCM_THREADS, smem_pipe, ctx->stream>>>(pp);
-            else k_fft_strided_pipe<FftGeneric><<<nctas, PCM_THREADS, smem_pipe, ctx->stream>>>(pp);
-        } else if (g.static_y) k_fft_strided<FftS540><<<grid, PCM_THREADS, g.smem_y, ctx->stream>>>(a);
-        else k_fft_strided<FftGeneric><<<grid, PCM_THREADS, g.smem_y, ctx->stream>>>(a);
+            k_fft_strided_pipe<FftGeneric><<<nctas, PCM_THREADS, smem_pipe, ctx->stream>>>(pp);
+        } else k_fft_strided<FftGeneric><<<grid, PCM_THREADS, g.smem_y, ctx->stream>>>(a);
     }
     BS_CUDA(ctx, cudaGetLastError());
     {
@@ -1671,7 +1772,9 @@ static int pcm_compute_pcm(bs_ctx* ctx, const void* d1, const void* d2, int dtyp
         a.thresh = 1e-5f;  // PhaseCorrelation2Util.normalizeInterval threshold
         dim3 grid(g.pitch >> g.tshift_z, g.P[1], 1);
         bs_launch_scope sc(ctx, "fft_z_xpower");
-        if (env_int("BS_FFT_Z_PIPE", 1) && g.tshift_z >= 1 && !(g.static_z && g.tshift_z == 2)) {
+        if (g.static_z) {
+            launch_col540(ctx, a, g.pitch / COL540_TC, g.P[1], 0);
+        } else if (g.tshift_z >= 1) {
             StridedPipeArgs pp;
             pp.s = a;
             pp.tiles_x = g.pitch >> g.tshift_z;
@@ -1679,13 +1782,8 @@ static int pcm_compute_pcm(bs_ctx* ctx, const void* d1, const void* d2, int dtyp
             pp.n_tiles = pp.tiles_x * pp.n_other;
             const int per_sm = std::max(1, std::min(2, (int)(PCM_SMEM_MAX / (g.smem_z + 1024))));
             const int nctas = std::min(pp.n_tiles, ctx->sm_count * per_sm);
-            if (g.static_z && g.tshift_z == 3 && env_int("BS_FFT_Z_R2", 1)) k_fft_xpower_pipe<FftS540R2><<<nctas, PCM_THREADS, g.smem_z, ctx->stream>>>(pp);
-            else if (g.static_z && g.tshift_z == 3) k_fft_xpower_pipe<FftS540><<<nctas, PCM_THREADS, g.smem_z, ctx->stream>>>(pp);
-            else k_fft_xpower_pipe<FftGeneric><<<nctas, PCM_THREADS, g.smem_z, ctx->stream>>>(pp);
-        } else if (g.static_z && g.tshift_z == 3 && env_int("BS_FFT_Z_R2", 1)) k_fft_strided<FftS540R2><<<grid, PCM_THREADS, g.smem_z, ctx->stream>>>(a);
-        else if (g.static_z && g.tshift_z == 2) k_fft_strided<FftS540T4><<<grid, PCM_THREADS, g.smem_z, ctx->stream>>>(a);
-        else if (g.static_z) k_fft_strided<FftS540><<<grid, PCM_THREADS, g.smem_z, ctx->stream>>>(a);
-        else k_fft_strided<FftGeneric><<<grid, PCM_THREADS, g.smem_z, ctx->stream>>>(a);
+            k_fft_xpower_pipe<FftGeneric><<<nctas, PCM_THREADS, g.smem_z, ctx->stream>>>(pp);
+        } else k_fft_strided<FftGeneric><<<grid, PCM_THREADS, g.smem_z, ctx->stream>>>(a);
     }
     BS_CUDA(ctx, cudaGetLastError());
     {
@@ -1701,7 +1799,9 @@ static int pcm_compute_pcm(bs_ctx* ctx, const void* d1, const void* d2, int dtyp
         dim3 grid(g.pitch >> g.tshift_y, g.P[2], 1);
         bs_launch_scope sc(ctx, "fft_y_inv");
         const size_t smem_pipe = ((size_t)((g.P[1] + 1) & ~1) + 3 * (size_t)g.P[1] * (1 << g.tshift_y)) * sizeof(float2);
-        if (env_int("BS_FFT_Y_PIPE", 1) && smem_pipe <= PCM_SMEM_MAX) {
+        if (g.static_y) {
+            launch_col540(ctx, a, g.pitch / COL540_TC, g.P[2], 1);
+        } else if (smem_pipe <= PCM_SMEM_MAX) {
             StridedPipeArgs pp;
             pp.s = a;
             pp.tiles_x = g.pitch >> g.tshift_y;
@@ -1709,11 +1809,8 @@ static int pcm_compute_pcm(bs_ctx* ctx, const void* d1, const void* d2, int dtyp
             pp.n_tiles = pp.tiles_x * pp.n_other * 1;
             const int per_sm = std::max(1, std::min(2, (int)(PCM_SMEM_MAX / (smem_pipe + 1024))));
             const int nctas = std::min(pp.n_tiles, ctx->sm_count * per_sm);
-            if (g.static_y && env_int("BS_FFT_Y_R2", 1)) k_fft_strided_pipe<FftS540R2><<<nctas, PCM_THREADS, smem_pipe, ctx->stream>>>(pp);
-            else if (g.static_y) k_fft_strided_pipe<FftS540><<<nctas, PCM_THREADS, smem_pipe, ctx->stream>>>(pp);
-            else k_fft_strided_pipe<FftGeneric><<<nctas, PCM_THREADS, smem_pipe, ctx->stream>>>(pp);
-        } else if (g.static_y) k_fft_strided<FftS540><<<grid, PCM_THREADS, g.smem_y, ctx->stream>>>(a);
-        else k_fft_strided<FftGeneric><<<grid, PCM_THREADS, g.smem_y, ctx->stream>>>(a);
+            k_fft_strided_pipe<FftGeneric><<<nctas, PCM_THREADS, smem_pipe, ctx->stream>>>(pp);
+        } else k_fft_strided<FftGeneric><<<grid, PCM_THREADS, g.smem_y, ctx->stream>>>(a);
     }
     BS_CUDA(ctx, cudaGetLastError());
     {

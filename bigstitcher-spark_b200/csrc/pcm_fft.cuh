@@ -319,7 +319,83 @@ struct FftStatic {
 
 
 // ------------------------------------------------------------------------------------------
-// Warp-private line FFT: ONE warp transforms ONE contiguous line (buf[e]) with only
+// Register-resident two-stage transform of a column tile: TC columns of N = RA * RB points, element n of column
+// c at g[n * estride + c].  Cooley-Tukey with n = RB n1 + n2 and k = k1 + RA k2:
+//   stage 1  item (n2, c) holds x[RB n1 + n2], n1 < RA, in registers: dft<RA>, times W_N^(n2 k1), and ONE write
+//            per element to the exchange buffer X[(k1 RB + n2) TC + c]
+//   (one __syncthreads)
+//   stage 2  item (k1, c) reads X[(k1 RB + n2) TC + c], n2 < RB, once: dft<RB> leaves X[k1 + RA k2] in register k2
+// Items of a stage are i = threadIdx.x + u NT, with (n2 | k1) = i / TC and c = i % TC, so a warp touches 32 / TC
+// consecutive row segments of TC columns: the global accesses are whole segments, the exchange writes are
+// contiguous, and the exchange reads of one n2 are 32 / TC segments of TC float2 (the 2-wavefront minimum).
+// Two-element twiddles n2 k1 < N index the table tw[e] = e^{-2 pi i e / N} (shared memory) directly.
+//
+// Stage 2 of RegFft2<RA, RB> leaves item (k1, c) holding x[k1 + RA k2] for k2 < RB, which is exactly the stage-1
+// item (n2' = k1, c) of RegFft2<RB, RA> (input n = RA n1' + n2', n1' = k2): a second transform of the result
+// starts on the registers the threads already hold, with no exchange in between.
+template <int RA, int RB, int TC, int NT>
+struct RegFft2 {
+    static constexpr int N = RA * RB;
+    static constexpr int I1 = RB * TC, IT1 = (I1 + NT - 1) / NT;   // stage-1 items, per thread
+    static constexpr int I2 = RA * TC, IT2 = (I2 + NT - 1) / NT;   // stage-2 items, per thread
+    static constexpr int XSIZE = N * TC;                           // exchange buffer, float2
+    typedef float2 In[IT1][RA];
+
+    static __device__ __forceinline__ bool live1(int u) { return I1 % NT == 0 || (int)threadIdx.x + u * NT < I1; }
+    static __device__ __forceinline__ bool live2(int u) { return I2 % NT == 0 || (int)threadIdx.x + u * NT < I2; }
+
+    static __device__ __forceinline__ void load(In& v, const float2* __restrict__ g, long long estride) {
+#pragma unroll
+        for (int u = 0; u < IT1; ++u) {
+            if (!live1(u)) continue;
+            const int i = threadIdx.x + u * NT;
+            const float2* p = g + (long long)(i / TC) * estride + (i % TC);
+#pragma unroll
+            for (int n1 = 0; n1 < RA; ++n1) v[u][n1] = __ldcg(p + (long long)(RB * n1) * estride);
+        }
+    }
+    static __device__ __forceinline__ void stage1(In& v, float2* __restrict__ X, const float2* __restrict__ tw) {
+#pragma unroll
+        for (int u = 0; u < IT1; ++u) {
+            if (!live1(u)) continue;
+            const int i = threadIdx.x + u * NT;
+            const int n2 = i / TC, c = i % TC;
+            dft<RA>(v[u]);
+            X[n2 * TC + c] = v[u][0];
+#pragma unroll
+            for (int k1 = 1; k1 < RA; ++k1) X[(k1 * RB + n2) * TC + c] = cmulf(v[u][k1], tw[n2 * k1]);
+        }
+    }
+    // stage 2, one item at a time (its RB outputs are live only until emit returns):
+    // emit(w, u, k1, c) receives w[k2] = X[k1 + RA k2] of column c
+    template <class Emit>
+    static __device__ __forceinline__ void stage2(const float2* __restrict__ X, Emit&& emit) {
+#pragma unroll
+        for (int u = 0; u < IT2; ++u) {
+            if (!live2(u)) continue;
+            const int i = threadIdx.x + u * NT;
+            const int k1 = i / TC, c = i % TC;
+            const float2* p = X + k1 * RB * TC + c;
+            float2 w[RB];
+#pragma unroll
+            for (int n2 = 0; n2 < RB; ++n2) w[n2] = p[n2 * TC];
+            dft<RB>(w);
+            emit(w, u, k1, c);
+        }
+    }
+    static __device__ __forceinline__ void store(const float2 (&w)[RB], float2* __restrict__ g, long long estride, int k1,
+                                                 int c) {
+        float2* p = g + (long long)k1 * estride + c;
+#pragma unroll
+        for (int k2 = 0; k2 < RB; ++k2) __stcg(p + (long long)(RA * k2) * estride, w[k2]);
+    }
+    // the item's own exchange slots: X[(k1 RB + k2) TC + c] (write-back of a stage-2 result for the same thread)
+    static __device__ __forceinline__ float2* slot(float2* X, int k1, int c) { return X + k1 * RB * TC + c; }
+};
+
+
+// ------------------------------------------------------------------------------------------
+// Warp-private line FFT:ONE warp transforms ONE contiguous line (buf[e]) with only
 // __syncwarp() between stages, so the x passes need no block-wide barriers at all and the 8
 // warps of a CTA drift freely (one warp's loads overlap another's butterflies).
 template <int R>
