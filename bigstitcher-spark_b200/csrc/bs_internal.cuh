@@ -93,6 +93,9 @@ struct bs_ctx {
     std::multimap<size_t, bs_pool_entry> vol_pool;
     int sm_count = 132;
     bool pcm_attr_done = false;       // cudaFuncSetAttribute(max dynamic smem) done on this device
+    bool pearson_attr_done = false;   // the same for k_pearson_u16 (set from its first launch)
+    size_t pearson_smem = 0;          // dynamic smem of k_pearson_u16's last launch on this context ...
+    int pearson_occ = 0;              // ... and its resident CTAs per SM
 };
 
 int bs_set_error(bs_ctx* ctx, int code, const char* fmt, ...);

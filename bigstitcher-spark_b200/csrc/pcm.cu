@@ -14,7 +14,8 @@
 //   k_fft_x_c2r      conj + C2R along x, in place -> real PCM (row pitch 2*pitch floats)
 //   k_peaks          periodic 6-neighbour local maxima, per-CTA top-K
 //   k_gather27       3x3x3 neighbourhoods of the K peaks (sub-pixel fit runs on the host)
-//   k_pearson        exact integer sums (uint64 atomics) for all surviving wrap candidates
+//   k_pearson_u16    exact integer sums (uint64 atomics) for all surviving wrap candidates, slab-staged image 1
+//                    (k_pearson: uint8 / float32 and unaligned uint16 crops)
 //
 // Inverse transforms are forward transforms of conjugated data (conj(F(conj X)) = N F^-1 X);
 // the two conjugations between consecutive passes cancel, so only the product step and the
@@ -1109,116 +1110,251 @@ struct PearsonArgs {
     double* sums_d;              // same for float input
 };
 
-// Row-chunk-major traversal: a warp owns PR_ROWS consecutive rows of image 1 and evaluates EVERY
-// candidate on them before moving on, so all candidates stream through the volumes in lockstep and
-// the second..K-th read of a row is an L1/L2 hit (DRAM traffic ~ one sweep instead of K sweeps).
+// Generic path (uint8, float32, uint16 without 16-byte aligned bases): a warp owns PR_ROWS consecutive image-1 rows
+// and evaluates every candidate on them, re-reading both images' rows from global memory per candidate.
 #define PR_ROWS 16
-#define PR_MLP 8
 
-__device__ __forceinline__ void pr_acc(unsigned int va, unsigned int vb, unsigned int& ra, unsigned int& rb,
-                                       unsigned long long& saa, unsigned long long& sbb, unsigned long long& sab) {
-    ra += va;
-    rb += vb;
-    saa += (unsigned long long)va * va;   // one IMAD.WIDE.U32 with 64-bit accumulate each
-    sbb += (unsigned long long)vb * vb;
-    sab += (unsigned long long)va * vb;
+// ------------------------------------------------------------------------------------------
+// uint16 Pearson sums.  Work unit: a slab of up to PRS_ROWS consecutive image-1 rows, staged once into shared memory
+// by a 1-D bulk copy (evict-first in L2) while the previous slab is consumed.  Persistent CTAs take slabs from a
+// global counter in row (z-major) order, so all CTAs work inside a narrow z band and candidates with nearby (y, z)
+// shifts share image-2 lines in L2.  For every candidate whose box meets the slab, a warp streams the matching
+// image-2 row segments in 16-byte chunks aligned on the flat element index (so any row pitch works) and pairs them
+// with the image-1 elements realigned from two 16-byte shared-memory reads.  Image 1 crosses DRAM once per pair,
+// image 2 about once per candidate box.
+#define PRS_ROWS 32
+#define PRS_STAGE_ELEMS 16384     // bound on the staged rows per slab: 32 KB of uint16
+#define PRS_PAD 8                 // elements in front of a staged slab (a chunk's realignment may start before it)
+
+struct PearsonU16Args {
+    const unsigned short* img1;   // both 16-byte aligned
+    const unsigned short* img2;
+    int dx, dy, dz;
+    int slab_rows;                // image-1 rows per slab (<= PRS_ROWS, slab_rows * dx <= PRS_STAGE_ELEMS unless dx is larger)
+    int stage_elems;              // uint16 elements per stage buffer, multiple of 8
+    int nslabs;
+    const PearsonCand* cands;
+    unsigned long long* sums;     // 5 per candidate: sa, sb, saa, sbb, sab
+    const int* ncand;
+    int* counter;                 // slab counter, zero at launch
+};
+
+__device__ __forceinline__ unsigned long long l2_evict_first_policy() {
+    unsigned long long p;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ void tma_bulk_g2s_hint(void* dst, const void* src, unsigned int bytes, unsigned long long* bar,
+                                                  unsigned long long policy) {
+    asm volatile(
+        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+            smem_u32(dst)),
+        "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
+        : "memory");
+}
+__device__ __forceinline__ uint4 ldg_stream16(const void* p) {
+    uint4 v;
+    asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+                 : "l"(p));
+    return v;
 }
 
-__device__ __forceinline__ void pearson_u16(const PearsonArgs& a, int ncand, unsigned long long* s_acc) {
-    const unsigned short* __restrict__ i1 = (const unsigned short*)a.img1;
-    const unsigned short* __restrict__ i2 = (const unsigned short*)a.img2;
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    const long long nrows = (long long)a.dy * a.dz;
-    const long long nchunks = (nrows + PR_ROWS - 1) / PR_ROWS;
-    const bool even_rows = !(a.dx & 1) && !((size_t)i1 & 3) && !((size_t)i2 & 3);
-    for (long long ch = (long long)blockIdx.x * nw + wid; ch < nchunks; ch += (long long)gridDim.x * nw) {
-        const long long r0 = ch * PR_ROWS;
-        const int z0 = (int)(r0 / a.dy), y0 = (int)(r0 - (long long)z0 * a.dy);
-        for (int c = 0; c < ncand; ++c) {
-            const PearsonCand cd = a.cands[c];
-            unsigned long long sa = 0, sb = 0, saa = 0, sbb = 0, sab = 0;
-            bool any = false;
-            // both x offsets even -> aligned ushort2 loads on both images
-            const bool vec = even_rows && !((cd.o1[0] | cd.o2[0]) & 1);
-            for (int rr = 0; rr < PR_ROWS; ++rr) {
-                const long long r = r0 + rr;
-                if (r >= nrows) break;
-                int z = z0, y = y0 + rr;          // (z, y) of row r0 + rr without a 64-bit division per row
-                while (y >= a.dy) { y -= a.dy; ++z; }
-                const int yy = y - cd.o1[1], zz = z - cd.o1[2];
-                if (yy < 0 || yy >= cd.sz[1] || zz < 0 || zz >= cd.sz[2]) continue;
-                any = true;
-                const unsigned short* p1 = i1 + (size_t)r * a.dx + cd.o1[0];
-                const unsigned short* p2 = i2 + ((size_t)(zz + cd.o2[2]) * a.dy + (yy + cd.o2[1])) * a.dx + cd.o2[0];
-                unsigned int ra = 0, rb = 0;
-                const int n = cd.sz[0];
-                if (vec) {
-                    const unsigned int* q1 = reinterpret_cast<const unsigned int*>(p1);
-                    const unsigned int* q2 = reinterpret_cast<const unsigned int*>(p2);
-                    const int nv = n >> 1;
-                    for (int x0 = lane; x0 < nv; x0 += 32 * PR_MLP) {   // PR_MLP words per image in flight per lane
-                        unsigned int w1[PR_MLP], w2[PR_MLP];
+// warp 0: stage slab s (flat image-1 elements [e0, e1)) into buf, where buf[PRS_PAD + e - (e0 & ~7)] = img1[e].
+// Lane 0 issues the bulk copy of the 16-byte aligned middle; lanes 0-7 / 8-15 load the unaligned head / tail
+// (< 8 elements each).
+__device__ __forceinline__ void prs_stage(const PearsonU16Args& a, int s, long long nrows, unsigned short* buf,
+                                          unsigned long long* bar, unsigned long long policy, int lane) {
+    const long long r0 = (long long)s * a.slab_rows, r1 = min(r0 + a.slab_rows, nrows);
+    const long long e0 = r0 * a.dx, e1 = r1 * a.dx, a0 = e0 & ~7LL;
+    const long long b0 = (e0 + 7) & ~7LL, b1 = e1 & ~7LL;
+    if (lane == 0) {
+        const unsigned int bytes = b1 > b0 ? (unsigned int)((b1 - b0) * 2) : 0u;
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the generic reads of the previous use came first
+        mbar_expect_tx(bar, bytes);
+        if (bytes) tma_bulk_g2s_hint(buf + PRS_PAD + (b0 - a0), a.img1 + b0, bytes, bar, policy);
+    }
+    const long long e = lane < 8 ? e0 + lane : max(b0, b1) + (lane - 8);
+    if (lane < 16 && e < (lane < 8 ? min(b0, e1) : e1)) buf[PRS_PAD + (e - a0)] = a.img1[e];
+}
+
+__device__ __forceinline__ void prs_acc(const unsigned int A[4], const unsigned int B[4], unsigned int& sa, unsigned int& sb,
+                                        unsigned long long& saa, unsigned long long& sbb, unsigned long long& sab) {
 #pragma unroll
-                        for (int u = 0; u < PR_MLP; ++u) {
-                            const int x = x0 + 32 * u;
-                            w1[u] = x < nv ? __ldg(q1 + x) : 0u;
-                            w2[u] = x < nv ? __ldg(q2 + x) : 0u;
-                        }
+    for (int m = 0; m < 4; ++m) {
+        const unsigned int a0 = A[m] & 0xffffu, a1 = A[m] >> 16, b0 = B[m] & 0xffffu, b1 = B[m] >> 16;
+        sa += a0 + a1;
+        sb += b0 + b1;
+        saa += (unsigned long long)a0 * a0;   // IMAD.WIDE.U32 with 64-bit accumulate each
+        saa += (unsigned long long)a1 * a1;
+        sbb += (unsigned long long)b0 * b0;
+        sbb += (unsigned long long)b1 * b1;
+        sab += (unsigned long long)a0 * b0;
+        sab += (unsigned long long)a1 * b1;
+    }
+}
+
+// One image-2 row segment of one candidate, owned by a warp.  Chunk k covers image-2 elements g + 8k .. g + 8k + 7
+// (g 16-byte aligned); elements lo .. hi - 1 of the chunk sequence belong to the segment.  s1 points at the staged
+// image-1 element paired with chunk 0's first element, rounded down to 16 bytes; SH is the rounding (0..7).
+// Chunks k >= kvec reach past the end of image 2 and are loaded element by element.
+template <int SH>
+__device__ __forceinline__ void prs_row(const unsigned short* __restrict__ g, const unsigned short* s1, int lo, int hi,
+                                        int nch, int kvec, int lane, unsigned int& sa, unsigned int& sb,
+                                        unsigned long long& saa, unsigned long long& sbb, unsigned long long& sab) {
+    for (int k0 = lane; k0 < nch; k0 += 64) {
+        uint4 v[2];
 #pragma unroll
-                        for (int u = 0; u < PR_MLP; ++u) {
-                            pr_acc(w1[u] & 0xffffu, w2[u] & 0xffffu, ra, rb, saa, sbb, sab);
-                            pr_acc(w1[u] >> 16, w2[u] >> 16, ra, rb, saa, sbb, sab);
-                        }
-                    }
-                    if ((n & 1) && lane == 0) pr_acc(__ldg(p1 + n - 1), __ldg(p2 + n - 1), ra, rb, saa, sbb, sab);
-                } else if (even_rows && n >= 4) {
-                    // exactly one x offset is odd: aligned words on one side, funnel-shifted pairs of
-                    // aligned words on the other (element -1 and the following words stay inside the row)
-                    // the aligned side is accumulated as "a", the funnel-shifted side as "b"; the
-                    // a/b statistics are swapped once per row when image 1 is the shifted side
-                    const bool odd1 = cd.o1[0] & 1;
-                    const unsigned int* qa = reinterpret_cast<const unsigned int*>(odd1 ? p2 : p1);
-                    const unsigned int* qm = reinterpret_cast<const unsigned int*>((odd1 ? p1 : p2) - 1);
-                    const int nv = (n >> 1) - 1;  // last pair(s) handled below: qm[x + 1] must not leave the row
-                    unsigned int ta = 0, tb = 0;
-                    unsigned long long taa = 0, tbb = 0;
-                    for (int x0 = lane; x0 < nv; x0 += 32 * PR_MLP) {
-                        unsigned int wa[PR_MLP], m0[PR_MLP], m1[PR_MLP];
-#pragma unroll
-                        for (int u = 0; u < PR_MLP; ++u) {
-                            const int x = x0 + 32 * u;
-                            wa[u] = x < nv ? __ldg(qa + x) : 0u;
-                            m0[u] = x < nv ? __ldg(qm + x) : 0u;
-                            m1[u] = x < nv ? __ldg(qm + x + 1) : 0u;
-                        }
-#pragma unroll
-                        for (int u = 0; u < PR_MLP; ++u) {
-                            const unsigned int wm = __funnelshift_r(m0[u], m1[u], 16);
-                            pr_acc(wa[u] & 0xffffu, wm & 0xffffu, ta, tb, taa, tbb, sab);
-                            pr_acc(wa[u] >> 16, wm >> 16, ta, tb, taa, tbb, sab);
-                        }
-                    }
-                    if (odd1) { ra += tb; rb += ta; saa += tbb; sbb += taa; }
-                    else { ra += ta; rb += tb; saa += taa; sbb += tbb; }
-                    for (int x = 2 * nv + lane; x < n; x += 32) pr_acc(__ldg(p1 + x), __ldg(p2 + x), ra, rb, saa, sbb, sab);
-                } else {
-#pragma unroll 4
-                    for (int x = lane; x < n; x += 32) pr_acc(__ldg(p1 + x), __ldg(p2 + x), ra, rb, saa, sbb, sab);
+        for (int u = 0; u < 2; ++u) {        // both chunks' loads in flight before any arithmetic
+            const int k = k0 + 32 * u;
+            v[u] = make_uint4(0u, 0u, 0u, 0u);
+            if (k < kvec) {
+                v[u] = ldg_stream16(g + 8 * k);
+            } else if (k < nch) {
+                unsigned long long w0 = 0ull, w1 = 0ull;
+                for (int j = max(lo - 8 * k, 0); j < min(hi - 8 * k, 8); ++j) {
+                    const unsigned long long e = g[8 * k + j];
+                    if (j < 4) w0 |= e << (16 * j);
+                    else w1 |= e << (16 * (j - 4));
                 }
-                sa += ra;
-                sb += rb;
-            }
-            if (!any) continue;  // warp-uniform
-            unsigned long long v[5] = {sa, sb, saa, sbb, sab};
-#pragma unroll
-            for (int k = 0; k < 5; ++k) {
-                unsigned long long t = v[k];
-#pragma unroll
-                for (int off = 16; off > 0; off >>= 1) t += __shfl_down_sync(0xffffffffu, t, off);
-                if (lane == 0 && t) atomicAdd(&s_acc[5 * c + k], t);
+                v[u] = make_uint4((unsigned int)w0, (unsigned int)(w0 >> 32), (unsigned int)w1, (unsigned int)(w1 >> 32));
             }
         }
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+            const int k = k0 + 32 * u;
+            if (k >= nch) break;
+            const uint4 p = *reinterpret_cast<const uint4*>(s1 + 8 * k);
+            const uint4 q = *reinterpret_cast<const uint4*>(s1 + 8 * k + 8);
+            const unsigned int w[8] = {p.x, p.y, p.z, p.w, q.x, q.y, q.z, q.w};
+            unsigned int A[4], B[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
+#pragma unroll
+            for (int m = 0; m < 4; ++m)
+                A[m] = (SH & 1) ? __funnelshift_r(w[SH / 2 + m], w[SH / 2 + m + 1], 16) : w[SH / 2 + m];
+            const int l = lo - 8 * k, h = hi - 8 * k;
+            if (l > 0 || h < 8) {            // first / last chunk of the segment: zero both sides outside it
+#pragma unroll
+                for (int m = 0; m < 4; ++m) {
+                    const unsigned int mk = ((2 * m >= l && 2 * m < h) ? 0x0000ffffu : 0u) |
+                                            ((2 * m + 1 >= l && 2 * m + 1 < h) ? 0xffff0000u : 0u);
+                    A[m] &= mk;
+                    B[m] &= mk;
+                }
+            }
+            prs_acc(A, B, sa, sb, saa, sbb, sab);
+        }
     }
+}
+
+// dynamic smem: 2 stage buffers, the candidate list, 5 accumulators per candidate
+__global__ void __launch_bounds__(PCM_THREADS, 3) k_pearson_u16(const __grid_constant__ PearsonU16Args a) {
+    const int ncand = *a.ncand;   // written by k_pcm_select (no host round trip between peaks and Pearson)
+    if (ncand <= 0) return;
+    constexpr int NW = PCM_THREADS / 32, RPW = PRS_ROWS / NW;
+    unsigned short* stage = reinterpret_cast<unsigned short*>(bs_sm);
+    PearsonCand* s_cand = reinterpret_cast<PearsonCand*>(stage + 2 * (size_t)a.stage_elems);
+    unsigned long long* s_acc = reinterpret_cast<unsigned long long*>(s_cand + ncand);
+    __shared__ unsigned long long bars[2];
+    __shared__ int s_slab[2];
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const long long nrows = (long long)a.dy * a.dz, nel = nrows * a.dx;
+    const unsigned long long policy = l2_evict_first_policy();
+    for (int i = tid; i < 10 * ncand; i += blockDim.x) reinterpret_cast<int*>(s_cand)[i] = reinterpret_cast<const int*>(a.cands)[i];
+    for (int i = tid; i < 5 * ncand; i += blockDim.x) s_acc[i] = 0ull;
+    if (tid == 0) {
+        mbar_init(&bars[0], 1);
+        mbar_init(&bars[1], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    if (wid == 0) {
+        const int s = __shfl_sync(0xffffffffu, lane == 0 ? atomicAdd(a.counter, 1) : 0, 0);
+        if (lane == 0) s_slab[0] = s;
+        if (s < a.nslabs) prs_stage(a, s, nrows, stage, &bars[0], policy, lane);
+    }
+    __syncthreads();
+    for (int it = 0;; ++it) {
+        const int buf = it & 1;
+        const int s = s_slab[buf];
+        if (s >= a.nslabs) break;
+        if (wid == 0) {   // next slab's copy is in flight while this one is consumed
+            const int sn = __shfl_sync(0xffffffffu, lane == 0 ? atomicAdd(a.counter, 1) : 0, 0);
+            if (lane == 0) s_slab[buf ^ 1] = sn;
+            if (sn < a.nslabs) prs_stage(a, sn, nrows, stage + (size_t)(buf ^ 1) * a.stage_elems, &bars[buf ^ 1], policy, lane);
+        }
+        const long long r0 = (long long)s * a.slab_rows;
+        const int nr = (int)min((long long)a.slab_rows, nrows - r0);
+        const int z0 = (int)(r0 / a.dy), y0 = (int)(r0 - (long long)z0 * a.dy);
+        const int zl = (int)((r0 + nr - 1) / a.dy);
+        // (y, z) of this warp's rows wid, wid + NW, ...
+        int ry[RPW], rz[RPW];
+#pragma unroll
+        for (int j = 0; j < RPW; ++j) {
+            int y = y0 + wid + j * NW, z = z0;
+            while (y >= a.dy) { y -= a.dy; ++z; }
+            ry[j] = y;
+            rz[j] = z;
+        }
+        // staged image-1 element e0 + i (e0 = r0 * dx, the slab's first) sits at sbuf[soff + i]
+        const unsigned short* sbuf = stage + (size_t)buf * a.stage_elems;
+        const int soff = PRS_PAD + (int)((r0 * a.dx) & 7);
+        mbar_wait(&bars[buf], (it >> 1) & 1);
+        for (int c = 0; c < ncand; ++c) {
+            const PearsonCand cd = s_cand[c];
+            if (zl < cd.o1[2] || z0 >= cd.o1[2] + cd.sz[2]) continue;   // block-uniform
+            unsigned int sa = 0, sb = 0;
+            unsigned long long saa = 0, sbb = 0, sab = 0;
+            bool any = false;
+#pragma unroll
+            for (int j = 0; j < RPW; ++j) {
+                const int rr = wid + j * NW;
+                const int yy = ry[j] - cd.o1[1], zz = rz[j] - cd.o1[2];
+                if (rr >= nr || yy < 0 || yy >= cd.sz[1] || zz < 0 || zz >= cd.sz[2]) continue;
+                any = true;
+                const long long g2 = ((long long)(zz + cd.o2[2]) * a.dy + (yy + cd.o2[1])) * a.dx + cd.o2[0];
+                const long long c2 = g2 & ~7LL;
+                const int lo = (int)(g2 - c2), hi = lo + cd.sz[0];
+                const int nch = (hi + 7) >> 3;
+                const int kvec = (int)min((long long)nch, (nel - c2) >> 3);
+                // staged index of the image-1 element paired with image-2 element c2 (>= soff - 7 >= 1)
+                const int t = soff + rr * a.dx + cd.o1[0] - lo;
+                const unsigned short* s1 = sbuf + (t & ~7);
+                const unsigned short* g = a.img2 + c2;
+                switch (t & 7) {
+                    case 0: prs_row<0>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
+                    case 1: prs_row<1>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
+                    case 2: prs_row<2>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
+                    case 3: prs_row<3>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
+                    case 4: prs_row<4>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
+                    case 5: prs_row<5>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
+                    case 6: prs_row<6>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
+                    default: prs_row<7>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
+                }
+            }
+            if (!any) continue;  // warp-uniform
+            // per-warp partials: sa, sb < slab elements * 65535 < 2^32
+#pragma unroll
+            for (int off = 16; off > 0; off >>= 1) {
+                sa += __shfl_xor_sync(0xffffffffu, sa, off);
+                sb += __shfl_xor_sync(0xffffffffu, sb, off);
+                saa += __shfl_xor_sync(0xffffffffu, saa, off);
+                sbb += __shfl_xor_sync(0xffffffffu, sbb, off);
+                sab += __shfl_xor_sync(0xffffffffu, sab, off);
+            }
+            if (lane == 0) {
+                unsigned long long* acc = s_acc + 5 * c;
+                if (sa) atomicAdd(acc + 0, (unsigned long long)sa);
+                if (sb) atomicAdd(acc + 1, (unsigned long long)sb);
+                if (saa) atomicAdd(acc + 2, saa);
+                if (sbb) atomicAdd(acc + 3, sbb);
+                if (sab) atomicAdd(acc + 4, sab);
+            }
+        }
+        __syncthreads();   // every warp is done with this buffer before it is refilled
+    }
+    __syncthreads();
+    for (int i = tid; i < 5 * ncand; i += blockDim.x)
+        if (s_acc[i]) atomicAdd(a.sums + i, s_acc[i]);
 }
 
 template <typename T, typename ACC>
@@ -1268,7 +1404,7 @@ __global__ void __launch_bounds__(PCM_THREADS) k_pearson(const __grid_constant__
     double* s_d = reinterpret_cast<double*>(bs_sm);
     for (int i = threadIdx.x; i < 5 * ncand; i += blockDim.x) s_u[i] = 0ull;  // 0.0 has the same bit pattern
     __syncthreads();
-    if (a.dtype == BS_DTYPE_U16) pearson_u16(a, ncand, s_u);
+    if (a.dtype == BS_DTYPE_U16) pearson_generic<unsigned short, unsigned long long>(a, ncand, s_u);
     else if (a.dtype == BS_DTYPE_U8) pearson_generic<unsigned char, unsigned long long>(a, ncand, s_u);
     else pearson_generic<float, double>(a, ncand, s_d);
     __syncthreads();
@@ -1328,7 +1464,7 @@ struct SelectArgs {
     PcmSelect* sel;
     PearsonCand* cands;           // 8 * K
     unsigned long long* sums;     // 5 * 8 * K, zeroed here
-    int* ncand;
+    int* ncand;                   // [0]: candidate count, [1]: Pearson slab counter (zeroed here)
 };
 
 __global__ void __launch_bounds__(256) k_pcm_select(const __grid_constant__ SelectArgs a) {
@@ -1386,7 +1522,8 @@ __global__ void __launch_bounds__(256) k_pcm_select(const __grid_constant__ Sele
         }
         a.sel->np = np;
         a.sel->nslots = nslots;
-        *a.ncand = nslots;
+        a.ncand[0] = nslots;
+        a.ncand[1] = 0;   // k_pearson_u16's slab counter
         s_np = np; s_nslots = nslots;
     }
     __syncthreads();
@@ -1946,6 +2083,58 @@ static int pcm_check_params(bs_ctx* ctx, const bs_pcm_params* p, int dtype) {
     return BS_OK;
 }
 
+// Pearson sums of up to max_cands candidates (count in ncand[0]; ncand[1] zero) on the context's stream.
+// uint16 crops with 16-byte aligned bases take the slab-staged kernel; everything else the generic one.
+static int pearson_launch(bs_ctx* ctx, const void* d1, const void* d2, int dtype, const int d[3], const PearsonCand* cands,
+                          int max_cands, void* sums, int* ncand) {
+    const long long rows = (long long)d[1] * d[2];
+    if (dtype == BS_DTYPE_U16 && !((size_t)d1 & 15) && !((size_t)d2 & 15)) {
+        PearsonU16Args a;
+        a.img1 = (const unsigned short*)d1;
+        a.img2 = (const unsigned short*)d2;
+        a.dx = d[0]; a.dy = d[1]; a.dz = d[2];
+        a.slab_rows = std::max(1, std::min(PRS_ROWS, PRS_STAGE_ELEMS / d[0]));
+        a.stage_elems = ((a.slab_rows * d[0] + 32) + 7) & ~7;
+        a.nslabs = (int)((rows + a.slab_rows - 1) / a.slab_rows);
+        a.cands = cands;
+        a.sums = (unsigned long long*)sums;
+        a.ncand = ncand;
+        a.counter = ncand + 1;
+        const size_t smem = sizeof(unsigned short) * 2 * (size_t)a.stage_elems + (sizeof(PearsonCand) + 40) * max_cands;
+        if (!ctx->pearson_attr_done) {   // per device: the opt-in leaves room for the kernel's static shared memory
+            cudaFuncAttributes fa;
+            BS_CUDA(ctx, cudaFuncGetAttributes(&fa, k_pearson_u16));
+            BS_CUDA(ctx, cudaFuncSetAttribute(k_pearson_u16, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              (int)(PCM_SMEM_MAX - fa.sharedSizeBytes)));
+            ctx->pearson_attr_done = true;
+        }
+        if (ctx->pearson_smem != smem) {
+            int occ = 0;
+            BS_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pearson_u16, PCM_THREADS, smem));
+            if (occ < 1) return bs_set_error(ctx, BS_ERR_ARG, "pcm: %d Pearson candidates do not fit in shared memory", max_cands);
+            ctx->pearson_occ = occ;
+            ctx->pearson_smem = smem;
+        }
+        const int ctas = (int)std::min<long long>(a.nslabs, (long long)ctx->sm_count * ctx->pearson_occ);
+        bs_launch_scope sc(ctx, "pearson");
+        k_pearson_u16<<<ctas, PCM_THREADS, smem, ctx->stream>>>(a);
+    } else {
+        PearsonArgs a;
+        a.img1 = d1; a.img2 = d2;
+        a.dtype = dtype;
+        a.dx = d[0]; a.dy = d[1]; a.dz = d[2];
+        a.cands = cands;
+        a.sums_u = (unsigned long long*)sums;
+        a.sums_d = (double*)sums;
+        const long long chunks = (rows + PR_ROWS - 1) / PR_ROWS;
+        const int ctas = (int)std::max<long long>(1, std::min<long long>((chunks + 7) / 8, (long long)ctx->sm_count * 8));
+        bs_launch_scope sc(ctx, "pearson");
+        k_pearson<<<ctas, PCM_THREADS, sizeof(unsigned long long) * 5 * max_cands, ctx->stream>>>(a, ncand);
+    }
+    BS_CUDA(ctx, cudaGetLastError());
+    return BS_OK;
+}
+
 // everything of one pair that runs on the device, asynchronously, into result slot `slot`
 static int pcm_enqueue(bs_ctx* ctx, const void* d1, const void* d2, const long long dims[3], int dtype,
                        const bs_pcm_params* p, int slot) {
@@ -2016,21 +2205,9 @@ static int pcm_enqueue(bs_ctx* ctx, const void* d1, const void* d2, const long l
         k_pcm_select<<<1, 256, 0, ctx->stream>>>(a);
     }
     BS_CUDA(ctx, cudaGetLastError());
-    {
-        PearsonArgs a;
-        a.img1 = d1; a.img2 = d2;
-        a.dtype = dtype;
-        a.dx = g.d[0]; a.dy = g.d[1]; a.dz = g.d[2];
-        a.cands = (const PearsonCand*)(dsmall + pd.off_cands);
-        a.sums_u = (unsigned long long*)(dsmall + pd.off_sums);
-        a.sums_d = (double*)(dsmall + pd.off_sums);
-        const long long rows = (long long)g.d[1] * g.d[2];
-        const long long chunks = (rows + PR_ROWS - 1) / PR_ROWS;
-        const int ctas = (int)std::max<long long>(1, std::min<long long>((chunks + 7) / 8, (long long)ctx->sm_count * 8));
-        bs_launch_scope sc(ctx, "pearson");
-        k_pearson<<<ctas, PCM_THREADS, sizeof(unsigned long long) * 5 * 8 * K, ctx->stream>>>(a, (const int*)(dsmall + off_ncand));
-    }
-    BS_CUDA(ctx, cudaGetLastError());
+    if ((rc = pearson_launch(ctx, d1, d2, dtype, g.d, (const PearsonCand*)(dsmall + pd.off_cands), 8 * K,
+                             dsmall + pd.off_sums, (int*)(dsmall + off_ncand))))
+        return rc;
     BS_CUDA(ctx, cudaMemcpyAsync(hsmall, dsmall, readback, cudaMemcpyDeviceToHost, ctx->stream));
     if (!S->done[slot]) BS_CUDA(ctx, cudaEventCreateWithFlags(&S->done[slot], cudaEventDisableTiming));
     BS_CUDA(ctx, cudaEventRecord(S->done[slot], ctx->stream));
@@ -2334,6 +2511,54 @@ int bs_pcm_debug_pcm(bs_ctx* ctx, const void* img1, const void* img2, const long
     BS_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     if (pad_out) for (int d = 0; d < 3; ++d) pad_out[d] = g.P[d];
     return BS_OK;
+}
+
+int bs_pcm_debug_pearson(bs_ctx* ctx, const void* img1, const void* img2, const long long dims[3], int dtype, int n,
+                         const int* boxes, void* sums_out) {
+    if (!ctx) return BS_ERR_ARG;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (!img1 || !img2 || !dims || (n > 0 && (!boxes || !sums_out)))
+        return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_debug_pearson: NULL argument");
+    if (n < 0 || n > 8 * PCM_KMAX)
+        return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_debug_pearson: n must be in [0,%d]", 8 * PCM_KMAX);
+    if (dtype != BS_DTYPE_U16 && dtype != BS_DTYPE_F32 && dtype != BS_DTYPE_U8)
+        return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_debug_pearson: bad dtype %d", dtype);
+    int d[3];
+    for (int a = 0; a < 3; ++a) {
+        if (dims[a] <= 0 || dims[a] > 16384) return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_debug_pearson: dims out of range");
+        d[a] = (int)dims[a];
+    }
+    std::vector<PearsonCand> hc(std::max(n, 1));
+    for (int i = 0; i < n; ++i) {
+        const int* b = boxes + 9 * i;
+        PearsonCand& c = hc[i];
+        for (int a = 0; a < 3; ++a) {
+            c.o1[a] = b[a]; c.o2[a] = b[3 + a]; c.sz[a] = b[6 + a];
+            if (c.o1[a] < 0 || c.o2[a] < 0 || c.sz[a] < 0 || c.o1[a] + c.sz[a] > d[a] || c.o2[a] + c.sz[a] > d[a])
+                return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_debug_pearson: box %d leaves the volume (axis %d)", i, a);
+        }
+        c.pad = 0;
+    }
+    BS_CUDA(ctx, cudaSetDevice(ctx->device));
+    // device block: candidates, sums, {count, slab counter}
+    const size_t cb = sizeof(PearsonCand) * hc.size(), sb = sizeof(unsigned long long) * 5 * hc.size();
+    unsigned char* dev = nullptr;
+    BS_CUDA(ctx, cudaMalloc(&dev, cb + sb + 16));
+    const int cnt[2] = {n, 0};
+    int rc = BS_OK;
+    cudaError_t e = cudaMemcpyAsync(dev, hc.data(), cb, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(dev + cb, 0, sb, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(dev + cb + sb, cnt, sizeof(cnt), cudaMemcpyHostToDevice, ctx->stream);
+    if (e != cudaSuccess) rc = bs_set_error(ctx, BS_ERR_CUDA, "bs_pcm_debug_pearson: %s", cudaGetErrorString(e));
+    if (!rc) rc = pearson_launch(ctx, img1, img2, dtype, d, (const PearsonCand*)dev, (int)hc.size(), dev + cb, (int*)(dev + cb + sb));
+    if (!rc && n > 0) {
+        e = cudaMemcpyAsync(sums_out, dev + cb, sizeof(unsigned long long) * 5 * n, cudaMemcpyDeviceToHost, ctx->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+        if (e != cudaSuccess) rc = bs_set_error(ctx, BS_ERR_CUDA, "bs_pcm_debug_pearson: %s", cudaGetErrorString(e));
+    }
+    cudaStreamSynchronize(ctx->stream);
+    cudaFree(dev);
+    return rc;
 }
 
 }  // extern "C"

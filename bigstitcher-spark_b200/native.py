@@ -103,6 +103,7 @@ SYMBOLS = [
     "bs_version", "bs_init", "bs_destroy", "bs_last_error", "bs_synchronize", "bs_launch_count",
     "bs_profile_enable", "bs_profile_reset", "bs_profile_get", "bs_host_alloc", "bs_host_free",
     "bs_pcm_default_params", "bs_pcm_pair", "bs_pcm_batch", "bs_pcm_volumes_batch", "bs_good_fft_size", "bs_pcm_debug_pcm",
+    "bs_pcm_debug_pearson",
     "bs_fuse_default_params", "bs_volume_upload", "bs_volume_upload_async", "bs_volume_wrap", "bs_volume_free",
     "bs_content_weights", "bs_volume_info", "bs_volume_download", "bs_volume_devptr", "bs_downsample", "bs_fuse_block", "bs_fuse_blocks",
     "bs_fuse_block_to_volume", "bs_fuse_accumulate", "bs_fuse_finish", "bs_mask_blocks", "bs_dog_default_params", "bs_dog_detect",
@@ -142,6 +143,7 @@ def load_library():
     lib.bs_pcm_batch.argtypes = [vp, ip, P(vp), P(vp), P(ll), ip, P(PcmParams), ip, P(PcmResultC)]
     lib.bs_good_fft_size.argtypes = [ip, ip]
     lib.bs_pcm_debug_pcm.argtypes = [vp, vp, vp, P(ll), ip, P(ip), vp, P(ip)]
+    lib.bs_pcm_debug_pearson.argtypes = [vp, vp, vp, P(ll), ip, ip, P(ip), vp]
     lib.bs_fuse_default_params.argtypes = [P(FuseParamsC)]
     lib.bs_fuse_default_params.restype = None
     lib.bs_volume_upload.argtypes = [vp, vp, P(ll), ip, P(ull)]
@@ -333,6 +335,24 @@ class Context:
                                               _NP2BS[img1.dtype], ext, out.ctypes.data, pad))
         assert tuple(pad) == tuple(P)
         return out
+
+    def pcm_debug_pearson(self, img1, img2, boxes, dtype=None) -> np.ndarray:
+        """Pearson sums of explicit candidate boxes on two equal-shape crops on the device ([z,y,x] CUDA tensors),
+        computed by the production Pearson launch.  boxes: (n, 9) ints {o1 xyz, o2 xyz, sz xyz}.  Returns
+        (n, 5) {sum a, sum b, sum a^2, sum b^2, sum ab}: uint64 for integer input, float64 for float32."""
+        p1, d1, _ = _ptr_of(img1)
+        p2, d2, _ = _ptr_of(img2)
+        if not (d1 and d2):
+            raise ValueError("pcm_debug_pearson takes device tensors")
+        if tuple(img1.shape) != tuple(img2.shape):
+            raise ValueError("crops of a pair must have equal shape")
+        dims = (C.c_longlong * 3)(*[int(v) for v in tuple(img1.shape)[::-1]])
+        bx = np.ascontiguousarray(np.asarray(boxes, dtype=np.int32).reshape(-1, 9))
+        dt = _bs_dtype(img1, dtype)
+        out = np.zeros((max(len(bx), 1), 5), dtype=np.float64 if dt == DTYPE_F32 else np.uint64)
+        self._check(self.lib.bs_pcm_debug_pearson(self.h, p1, p2, dims, dt, len(bx),
+                                                  bx.ctypes.data_as(C.POINTER(C.c_int)), out.ctypes.data))
+        return out[:len(bx)]
 
     # -- hot path 2
     def volume_upload(self, vol: np.ndarray) -> int:

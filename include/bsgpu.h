@@ -131,6 +131,13 @@ int bs_good_fft_size(int n, int even);
 int bs_pcm_debug_pcm(bs_ctx* ctx, const void* img1, const void* img2, const long long dims[3],
                      int dtype, const int extension[3], float* out_pcm, int pad_out[3]);
 
+/* diagnostic: the Pearson sums of an explicit candidate list, computed by the same launch bs_pcm_* uses.
+ * img1/img2: DEVICE pointers to two crops of dims {x,y,z}.  boxes: n * 9 ints per candidate, {o1[3], o2[3], sz[3]}
+ * ({x,y,z} each): voxel o1 + p of img1 pairs with o2 + p of img2 for 0 <= p < sz; n <= 256.  sums_out: n * 5 values
+ * {sum a, sum b, sum a^2, sum b^2, sum ab}, uint64 for U16 / U8 and float64 for F32. */
+int bs_pcm_debug_pearson(bs_ctx* ctx, const void* img1, const void* img2, const long long dims[3], int dtype, int n,
+                         const int* boxes, void* sums_out);
+
 /* ---------------------------------------------------------------- hot path 2: affine fusion */
 typedef struct {
     double             src_to_world[12]; /* row-packed 3x4: source pixel -> world, i.e. the adjusted

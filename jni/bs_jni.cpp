@@ -319,6 +319,22 @@ JF(jlongArray, pcmDebugPcm)(JNIEnv* env, jclass, jlong ctx, jobject img1, jobjec
     return arr;
 }
 
+// diagnostic: Pearson sums of n explicit boxes (n x {o1[3], o2[3], sz[3]}) on two device crops (volumeDevptr);
+// sumsOut: long[5 n] (uint16 / uint8) or double[5 n] (float32)
+JF(void, pcmDebugPearson)(JNIEnv* env, jclass, jlong ctx, jlong dev1, jlong dev2, jlongArray dims, jint dtype, jintArray boxes,
+                          jobject sumsOut) {
+    long long d[3];
+    get3(env, dims, d);
+    const int n = boxes ? env->GetArrayLength(boxes) / 9 : 0;
+    int rc;
+    {
+        Pinned b(env, boxes), o(env, sumsOut);
+        rc = bs_pcm_debug_pearson(C(ctx), reinterpret_cast<const void*>(dev1), reinterpret_cast<const void*>(dev2), d, dtype, n,
+                                  static_cast<const int*>(b.p), o.p);
+    }
+    failed(env, ctx, rc);
+}
+
 // ---------------------------------------------------------------------------------------- hot path 2
 // BlockSupplier<T>.copy(interval, dest): dest is the primitive array BlockAlgoUtils.arrayImg allocated
 JF(void, fuseBlock)(JNIEnv* env, jclass, jlong ctx, jint nViews, jdoubleArray models, jlongArray handles, jfloatArray blend,

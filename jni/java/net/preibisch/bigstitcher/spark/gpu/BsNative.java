@@ -53,6 +53,8 @@ public final class BsNative
 	/** jobs: n x {vol1, vol2, min1[3], min2[3], dims[3]} */
 	public static native double[] pcmVolumesBatch( long ctx, long[] jobs, int[] iparams, double minOverlap );
 	public static native long[] pcmDebugPcm( long ctx, Object img1, Object img2, long[] dims, int dtype, int[] extension, Object outPcm );
+	/** device crops (volumeDevptr); boxes n x {o1[3], o2[3], sz[3]}; sumsOut long[5n] (integer input) or double[5n] (float32) */
+	public static native void pcmDebugPearson( long ctx, long dev1, long dev2, long[] dims, int dtype, int[] boxes, Object sumsOut );
 
 	/** models n*12, handles n*{volume, content}, blend n*{border[3], range[3]}, windows n*{fullDims[3], windowMin[3]} or null;
 	 *  iparams {fusionType, interpolation, outDtype, blendLutN, outBigEndian (1: N5 block payload byte order)}; dparams {minIntensity, maxIntensity} */
