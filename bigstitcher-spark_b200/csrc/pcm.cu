@@ -597,8 +597,7 @@ struct StridedArgs {
     const float2* tw;
     FftPlan plan;
     int tshift;          // log2(tile width in float2)
-    int mode;            // 0: forward in place on (blockIdx.z ? b : a); 1: cross-power (a,b) -> a
-    float thresh;        // normalisation threshold
+    float thresh;        // normalisation threshold (cross-power passes)
 };
 
 template <int UNR>
@@ -632,13 +631,24 @@ __device__ __forceinline__ void tile_store(float2* g, const float2* src, long lo
         __stcg(reinterpret_cast<float4*>(g + (long long)(i >> vshift) * estride) + (i & vmask), s4[i]);
 }
 
+// x / |x|, or 0 when |x| < thresh: the one unit-magnitude normalisation of the cross-power passes.  |x|^2 is formed
+// from h = x * 2^-46 (exact), so it does not overflow for |x| up to ~1.3e33 (x * x would past ~1.8e19), and above the
+// threshold it stays a normal number (thresh^2 * 2^-92 ~ 2e-38 > FLT_MIN): the reciprocal square root needs no
+// denormal fix-up, and h / |h| equals x / |x| bit for bit.
+__device__ __forceinline__ float rsqrt_ftz(float v) {
+    float r;
+    asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(v));
+    return r;
+}
 __device__ __forceinline__ float2 unit_or_zero(float2 x, float thresh) {
-    const float m2 = x.x * x.x + x.y * x.y;
-    if (m2 < thresh * thresh) return make_float2(0.f, 0.f);   // |x| < threshold
-    const float inv = rsqrtf(m2);
-    return make_float2(x.x * inv, x.y * inv);
+    const float2 h = make_float2(x.x * 0x1p-46f, x.y * 0x1p-46f);
+    const float m2 = h.x * h.x + h.y * h.y;
+    if (m2 < (thresh * thresh) * 0x1p-92f) return make_float2(0.f, 0.f);   // |x| < threshold
+    const float inv = rsqrt_ftz(m2);
+    return make_float2(h.x * inv, h.y * inv);
 }
 
+// forward FFT in place on (blockIdx.z ? b : a), one tile per CTA (y lengths whose pipelined tiles do not fit)
 template <class F>
 __global__ void __launch_bounds__(PCM_THREADS, 3) k_fft_strided(const __grid_constant__ StridedArgs a) {
     const int tshift = F::kStatic ? F::LSHIFT : a.tshift;
@@ -649,34 +659,14 @@ __global__ void __launch_bounds__(PCM_THREADS, 3) k_fft_strided(const __grid_con
     float2* B1 = B0 + (size_t)N * TW;
     const size_t base = (size_t)blockIdx.y * a.ostride + (size_t)blockIdx.x * TW;
     for (int i = threadIdx.x; i < N; i += blockDim.x) tw[i] = a.tw[i];
-    if (a.mode == 0) {
-        float2* g = (blockIdx.z ? a.b : a.a) + base;
-        tile_load<9>(B0, g, a.estride, N, tshift);
-        __syncthreads();
-        const float2* res = F::run(B0, B1, tw, a.plan, tshift, TW, 1);
-        tile_store(g, res, a.estride, N, tshift);
-    } else {
-        float2* B2 = B1 + (size_t)N * TW;
-        tile_load<9>(B0, a.a + base, a.estride, N, tshift);
-        tile_load<9>(B1, a.b + base, a.estride, N, tshift);
-        __syncthreads();
-        float2* rA = F::run(B0, B2, tw, a.plan, tshift, TW, 1);
-        float2* freeA = (rA == B0) ? B2 : B0;
-        float2* rB = F::run(B1, freeA, tw, a.plan, tshift, TW, 1);
-        float2* free2 = (rB == B1) ? freeA : B1;
-        const int tot = N * TW;
-        for (int i = threadIdx.x; i < tot; i += blockDim.x) {
-            const float2 x = unit_or_zero(rA[i], a.thresh);
-            const float2 y = unit_or_zero(rB[i], a.thresh);
-            rA[i] = make_float2(x.x * y.x + x.y * y.y, x.x * y.y - x.y * y.x);  // conj(x) * y
-        }
-        __syncthreads();
-        const float2* rQ = F::run(rA, free2, tw, a.plan, tshift, TW, 1);
-        tile_store(a.a + base, rQ, a.estride, N, tshift);
-    }
+    float2* g = (blockIdx.z ? a.b : a.a) + base;
+    tile_load<9>(B0, g, a.estride, N, tshift);
+    __syncthreads();
+    const float2* res = F::run(B0, B1, tw, a.plan, tshift, TW, 1);
+    tile_store(g, res, a.estride, N, tshift);
 }
 
-// Persistent, software-pipelined variant of mode 0: each CTA walks its tiles with three rotating
+// Persistent, software-pipelined variant of k_fft_strided: each CTA walks its tiles with three rotating
 // shared-memory buffers; the NEXT tile is pulled in with cp.async (LDGSTS, 16 B per thread and
 // request, no register staging) while the current one is transformed and stored.
 __device__ __forceinline__ void cp_async16(void* dst, const void* src) {
@@ -741,8 +731,8 @@ __global__ void __launch_bounds__(PCM_THREADS, 2) k_fft_strided_pipe(const __gri
     }
 }
 
-// Persistent, software-pipelined cross-power pass (z): same three tile buffers as k_fft_strided mode 1 (so two
-// CTAs still fit an SM), but the loads are cp.async groups that overlap the transforms:
+// Persistent, software-pipelined cross-power pass (z): three tile buffers (so two CTAs still fit an SM), the loads
+// are cp.async groups that overlap the transforms:
 //   A(t) lands -> FFT A   | B(t) still in flight
 //   B(t) lands -> FFT B -> normalise, conj(A) * B
 //   B's buffer is free    -> prefetch A(t+1) under the transform of the product
@@ -1789,51 +1779,63 @@ static void launch_col540(bs_ctx* ctx, const StridedArgs& a, int tiles_x, int n_
     else k_fft_xpower_col540<<<nctas, COL540_NT, smem, ctx->stream>>>(pp);
 }
 
-// forward pipeline up to the real PCM in ws.spec_a (row pitch 2*pitch floats)
-static int pcm_compute_pcm(bs_ctx* ctx, const void* d1, const void* d2, int dtype, const PcmGeometry& g,
-                           PcmDeviceTables* t) {
-    if (!ctx->pcm_attr_done) {
-        int rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c<FftGeneric>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_strided<FftGeneric>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r<FftGeneric>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c<FftX270>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c<FftX270L8>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_tma<FftX270L8>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_w<FftW270S>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_w<FftWGeneric>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r_w<FftW270>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r_w<FftWGeneric>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_tma<FftX270>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_tma<FftGeneric>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r<FftX270L8>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_strided_pipe<FftGeneric>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_xpower_pipe<FftGeneric>, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_col540, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_xpower_col540, 0))) return rc;
-        if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r<FftX270>, 0))) return rc;
-        ctx->pcm_attr_done = true;
-    }
+static int pcm_kernel_attrs(bs_ctx* ctx) {
+    if (ctx->pcm_attr_done) return BS_OK;
+    int rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c<FftGeneric>, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_strided<FftGeneric>, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r<FftGeneric>, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c<FftX270>, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c<FftX270L8>, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_tma<FftX270L8>, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_w<FftW270S>, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_w<FftWGeneric>, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r_w<FftW270>, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r_w<FftWGeneric>, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_tma<FftX270>, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_tma<FftGeneric>, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r<FftX270L8>, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_strided_pipe<FftGeneric>, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_xpower_pipe<FftGeneric>, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_col540, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_xpower_col540, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r<FftX270>, 0))) return rc;
+    ctx->pcm_attr_done = true;
+    return BS_OK;
+}
+
+// The five FFT passes.  Each launches one kernel on ctx->stream and, when `info` is not NULL, writes the
+// instantiation it chose (plus the plan's radices for runtime-planned kernels), e.g.
+// "k_fft_strided_pipe<FftGeneric> 15x12x3", into info[PCM_INFO_LEN].  bs_pcm_debug_pass runs them one at a time.
+#define PCM_INFO_LEN 128
+static void pass_info(char* info, const char* kernel, const FftPlan* plan) {
+    if (!info) return;
+    int n = snprintf(info, PCM_INFO_LEN, "%s", kernel);
+    for (int i = 0; plan && i < plan->nst && n < PCM_INFO_LEN; ++i)
+        n += snprintf(info + n, PCM_INFO_LEN - n, "%s%d", i ? "x" : " ", plan->radix[i]);
+}
+
+// pass 0: both crops -> blended mirrored extension + zero pad -> R2C along x into ws.spec_a / ws.spec_b
+static int pcm_pass_x_r2c(bs_ctx* ctx, const void* d1, const void* d2, int dtype, const PcmGeometry& g,
+                          PcmDeviceTables* t, char* info) {
     bs_pcm_workspace& ws = ctx->ws;
-    float2* sa = (float2*)ws.spec_a;
-    float2* sb = (float2*)ws.spec_b;
+    XR2CArgs a;
+    a.img[0] = d1; a.img[1] = d2;
+    a.spec[0] = (float2*)ws.spec_a; a.spec[1] = (float2*)ws.spec_b;
+    a.dtype = dtype;
+    a.dx = g.d[0]; a.dy = g.d[1]; a.dz = g.d[2];
+    a.Px = g.P[0]; a.Py = g.P[1]; a.Pz = g.P[2]; a.M = g.M; a.pitch = g.pitch;
+    a.ex = std::min(g.ext[0], g.d[0]);
+    a.Ex = g.E[0]; a.Ey = g.E[1]; a.Ez = g.E[2];
+    a.idx_x = t->idx[0]; a.w_x = t->w[0];
+    a.idx_y = t->idx[1]; a.w_y = t->w[1];
+    a.idx_z = t->idx[2]; a.w_z = t->w[2];
+    a.tw = t->tw[0];
+    a.plan = g.plan_x;
+    a.lshift = g.lshift_r2c;
+    const int LB = 1 << g.lshift_r2c;
+    dim3 grid((g.P[1] + LB - 1) / LB, g.P[2], 2);
     {
-        XR2CArgs a;
-        a.img[0] = d1; a.img[1] = d2;
-        a.spec[0] = sa; a.spec[1] = sb;
-        a.dtype = dtype;
-        a.dx = g.d[0]; a.dy = g.d[1]; a.dz = g.d[2];
-        a.Px = g.P[0]; a.Py = g.P[1]; a.Pz = g.P[2]; a.M = g.M; a.pitch = g.pitch;
-        a.ex = std::min(g.ext[0], g.d[0]);
-        a.Ex = g.E[0]; a.Ey = g.E[1]; a.Ez = g.E[2];
-        a.idx_x = t->idx[0]; a.w_x = t->w[0];
-        a.idx_y = t->idx[1]; a.w_y = t->w[1];
-        a.idx_z = t->idx[2]; a.w_z = t->w[2];
-        a.tw = t->tw[0];
-        a.plan = g.plan_x;
-        a.lshift = g.lshift_r2c;
-        const int LB = 1 << g.lshift_r2c;
-        dim3 grid((g.P[1] + LB - 1) / LB, g.P[2], 2);
         bs_launch_scope sc(ctx, "fft_x_r2c");
         const int esize = dtype == BS_DTYPE_U16 ? 2 : dtype == BS_DTYPE_F32 ? 4 : 1;
         const int row_bytes = g.d[0] * esize;
@@ -1844,74 +1846,112 @@ static int pcm_compute_pcm(bs_ctx* ctx, const void* d1, const void* d2, int dtyp
         const size_t smem_w = ((size_t)g.P[0] + (size_t)(PCM_THREADS / 32) * 2 * g.M) * sizeof(float2) +
                               (tma_ok ? (size_t)(PCM_THREADS / 32) * (2 * (size_t)row_bytes + 16) : 0);
         if (xmode && g.M <= 32 * XW_MAXV - 1 && smem_w <= PCM_SMEM_MAX && (((size_t)g.P[0] + 16 * (size_t)g.M) * 8) % 16 == 0) {
-            XWArgs t;
-            t.x = a;
-            t.row_bytes = row_bytes;
-            t.use_tma = tma_ok ? 1 : 0;
-            t.n_lines = 2LL * g.P[2] * g.P[1];
+            XWArgs w;
+            w.x = a;
+            w.row_bytes = row_bytes;
+            w.use_tma = tma_ok ? 1 : 0;
+            w.n_lines = 2LL * g.P[2] * g.P[1];
             const int per_sm = std::max(1, std::min(6, (int)(PCM_SMEM_MAX / (smem_w + 1024))));
-            const int nctas = (int)std::min<long long>((t.n_lines + 7) / 8, (long long)ctx->sm_count * per_sm);
-            if (g.M == FftW270S::N && env_int("BS_FFT_STATIC", 1)) k_fft_x_r2c_w<FftW270S><<<nctas, PCM_THREADS, smem_w, ctx->stream>>>(t);
-            else k_fft_x_r2c_w<FftWGeneric><<<nctas, PCM_THREADS, smem_w, ctx->stream>>>(t);
+            const int nctas = (int)std::min<long long>((w.n_lines + 7) / 8, (long long)ctx->sm_count * per_sm);
+            if (g.M == FftW270S::N && env_int("BS_FFT_STATIC", 1)) {
+                k_fft_x_r2c_w<FftW270S><<<nctas, PCM_THREADS, smem_w, ctx->stream>>>(w);
+                pass_info(info, tma_ok ? "k_fft_x_r2c_w<FftW270S> tma" : "k_fft_x_r2c_w<FftW270S>", nullptr);
+            } else {
+                k_fft_x_r2c_w<FftWGeneric><<<nctas, PCM_THREADS, smem_w, ctx->stream>>>(w);
+                pass_info(info, tma_ok ? "k_fft_x_r2c_w<FftWGeneric> tma" : "k_fft_x_r2c_w<FftWGeneric>", &g.plan_x);
+            }
         } else if (tma_ok) {
-            XR2CTmaArgs t;
-            t.x = a;
-            t.n_groups = (g.P[1] + LB - 1) / LB;
-            t.n_items = 2 * g.P[2] * t.n_groups;
-            t.row_bytes = row_bytes;
-            t.esize = esize;
+            XR2CTmaArgs m;
+            m.x = a;
+            m.n_groups = (g.P[1] + LB - 1) / LB;
+            m.n_items = 2 * g.P[2] * m.n_groups;
+            m.row_bytes = row_bytes;
+            m.esize = esize;
             const int per_sm = std::max(1, (int)(PCM_SMEM_MAX / (smem_tma + 1024)));
-            const int nctas = std::min(t.n_items, ctx->sm_count * std::min(per_sm, 4));
-            if (g.static_x && g.lshift_r2c == 3) k_fft_x_r2c_tma<FftX270L8><<<nctas, PCM_THREADS, smem_tma, ctx->stream>>>(t);
-            else if (g.static_x && g.lshift_r2c == 4) k_fft_x_r2c_tma<FftX270><<<nctas, PCM_THREADS, smem_tma, ctx->stream>>>(t);
-            else k_fft_x_r2c_tma<FftGeneric><<<nctas, PCM_THREADS, smem_tma, ctx->stream>>>(t);
-        } else if (g.static_x && g.lshift_r2c == 3) k_fft_x_r2c<FftX270L8><<<grid, PCM_THREADS, g.smem_x_r2c, ctx->stream>>>(a);
-        else if (g.static_x && g.lshift_r2c == 4) k_fft_x_r2c<FftX270><<<grid, PCM_THREADS, g.smem_x_r2c, ctx->stream>>>(a);
-        else k_fft_x_r2c<FftGeneric><<<grid, PCM_THREADS, g.smem_x_r2c, ctx->stream>>>(a);
+            const int nctas = std::min(m.n_items, ctx->sm_count * std::min(per_sm, 4));
+            if (g.static_x && g.lshift_r2c == 3) {
+                k_fft_x_r2c_tma<FftX270L8><<<nctas, PCM_THREADS, smem_tma, ctx->stream>>>(m);
+                pass_info(info, "k_fft_x_r2c_tma<FftX270L8>", nullptr);
+            } else if (g.static_x && g.lshift_r2c == 4) {
+                k_fft_x_r2c_tma<FftX270><<<nctas, PCM_THREADS, smem_tma, ctx->stream>>>(m);
+                pass_info(info, "k_fft_x_r2c_tma<FftX270>", nullptr);
+            } else {
+                k_fft_x_r2c_tma<FftGeneric><<<nctas, PCM_THREADS, smem_tma, ctx->stream>>>(m);
+                pass_info(info, "k_fft_x_r2c_tma<FftGeneric>", &g.plan_x);
+            }
+        } else if (g.static_x && g.lshift_r2c == 3) {
+            k_fft_x_r2c<FftX270L8><<<grid, PCM_THREADS, g.smem_x_r2c, ctx->stream>>>(a);
+            pass_info(info, "k_fft_x_r2c<FftX270L8>", nullptr);
+        } else if (g.static_x && g.lshift_r2c == 4) {
+            k_fft_x_r2c<FftX270><<<grid, PCM_THREADS, g.smem_x_r2c, ctx->stream>>>(a);
+            pass_info(info, "k_fft_x_r2c<FftX270>", nullptr);
+        } else {
+            k_fft_x_r2c<FftGeneric><<<grid, PCM_THREADS, g.smem_x_r2c, ctx->stream>>>(a);
+            pass_info(info, "k_fft_x_r2c<FftGeneric>", &g.plan_x);
+        }
     }
     BS_CUDA(ctx, cudaGetLastError());
+    return BS_OK;
+}
+
+// passes 1 and 3: forward FFT along y, in place, on both spectra (n_img = 2) or on the product in ws.spec_a (1)
+static int pcm_launch_y(bs_ctx* ctx, const PcmGeometry& g, PcmDeviceTables* t, int n_img, const char* tag, char* info) {
+    StridedArgs a;
+    a.a = (float2*)ctx->ws.spec_a; a.b = (float2*)ctx->ws.spec_b;
+    a.estride = g.pitch;
+    a.ostride = (long long)g.P[1] * g.pitch;
+    a.tw = t->tw[1];
+    a.plan = g.plan_y;
+    a.tshift = g.tshift_y;
+    a.thresh = 0.f;
+    dim3 grid(g.pitch >> g.tshift_y, g.P[2], n_img);
     {
-        StridedArgs a;
-        a.a = sa; a.b = sb;
-        a.estride = g.pitch;
-        a.ostride = (long long)g.P[1] * g.pitch;
-        a.tw = t->tw[1];
-        a.plan = g.plan_y;
-        a.tshift = g.tshift_y;
-        a.mode = 0;
-        a.thresh = 0.f;
-        dim3 grid(g.pitch >> g.tshift_y, g.P[2], 2);
-        bs_launch_scope sc(ctx, "fft_y");
+        bs_launch_scope sc(ctx, tag);
         const size_t smem_pipe = ((size_t)((g.P[1] + 1) & ~1) + 3 * (size_t)g.P[1] * (1 << g.tshift_y)) * sizeof(float2);
         if (g.static_y) {
-            launch_col540(ctx, a, g.pitch / COL540_TC, g.P[2], 2);
+            launch_col540(ctx, a, g.pitch / COL540_TC, g.P[2], n_img);
+            pass_info(info, "k_fft_col540", nullptr);
         } else if (smem_pipe <= PCM_SMEM_MAX) {
             StridedPipeArgs pp;
             pp.s = a;
             pp.tiles_x = g.pitch >> g.tshift_y;
             pp.n_other = g.P[2];
-            pp.n_tiles = pp.tiles_x * pp.n_other * 2;
+            pp.n_tiles = pp.tiles_x * pp.n_other * n_img;
             const int per_sm = std::max(1, std::min(2, (int)(PCM_SMEM_MAX / (smem_pipe + 1024))));
             const int nctas = std::min(pp.n_tiles, ctx->sm_count * per_sm);
             k_fft_strided_pipe<FftGeneric><<<nctas, PCM_THREADS, smem_pipe, ctx->stream>>>(pp);
-        } else k_fft_strided<FftGeneric><<<grid, PCM_THREADS, g.smem_y, ctx->stream>>>(a);
+            pass_info(info, "k_fft_strided_pipe<FftGeneric>", &g.plan_y);
+        } else {
+            k_fft_strided<FftGeneric><<<grid, PCM_THREADS, g.smem_y, ctx->stream>>>(a);
+            pass_info(info, "k_fft_strided<FftGeneric>", &g.plan_y);
+        }
     }
     BS_CUDA(ctx, cudaGetLastError());
+    return BS_OK;
+}
+
+// pass 1: forward y FFT of both spectra
+static int pcm_pass_y_fwd(bs_ctx* ctx, const PcmGeometry& g, PcmDeviceTables* t, char* info) {
+    return pcm_launch_y(ctx, g, t, 2, "fft_y", info);
+}
+
+// pass 2: forward z FFT of both spectra, unit-magnitude normalisation, conj(A) * B, forward z FFT of the product
+// into ws.spec_a
+static int pcm_pass_z_xpower(bs_ctx* ctx, const PcmGeometry& g, PcmDeviceTables* t, char* info) {
+    StridedArgs a;
+    a.a = (float2*)ctx->ws.spec_a; a.b = (float2*)ctx->ws.spec_b;
+    a.estride = (long long)g.P[1] * g.pitch;
+    a.ostride = g.pitch;
+    a.tw = t->tw[2];
+    a.plan = g.plan_z;
+    a.tshift = g.tshift_z;
+    a.thresh = 1e-5f;  // PhaseCorrelation2Util.normalizeInterval threshold
     {
-        StridedArgs a;
-        a.a = sa; a.b = sb;
-        a.estride = (long long)g.P[1] * g.pitch;
-        a.ostride = g.pitch;
-        a.tw = t->tw[2];
-        a.plan = g.plan_z;
-        a.tshift = g.tshift_z;
-        a.mode = 1;
-        a.thresh = 1e-5f;  // PhaseCorrelation2Util.normalizeInterval threshold
-        dim3 grid(g.pitch >> g.tshift_z, g.P[1], 1);
         bs_launch_scope sc(ctx, "fft_z_xpower");
         if (g.static_z) {
             launch_col540(ctx, a, g.pitch / COL540_TC, g.P[1], 0);
-        } else if (g.tshift_z >= 1) {
+            pass_info(info, "k_fft_xpower_col540", nullptr);
+        } else {
             StridedPipeArgs pp;
             pp.s = a;
             pp.tiles_x = g.pitch >> g.tshift_z;
@@ -1920,60 +1960,68 @@ static int pcm_compute_pcm(bs_ctx* ctx, const void* d1, const void* d2, int dtyp
             const int per_sm = std::max(1, std::min(2, (int)(PCM_SMEM_MAX / (g.smem_z + 1024))));
             const int nctas = std::min(pp.n_tiles, ctx->sm_count * per_sm);
             k_fft_xpower_pipe<FftGeneric><<<nctas, PCM_THREADS, g.smem_z, ctx->stream>>>(pp);
-        } else k_fft_strided<FftGeneric><<<grid, PCM_THREADS, g.smem_z, ctx->stream>>>(a);
+            pass_info(info, "k_fft_xpower_pipe<FftGeneric>", &g.plan_z);
+        }
     }
     BS_CUDA(ctx, cudaGetLastError());
+    return BS_OK;
+}
+
+// pass 3: forward y FFT of the product
+static int pcm_pass_y_inv(bs_ctx* ctx, const PcmGeometry& g, PcmDeviceTables* t, char* info) {
+    return pcm_launch_y(ctx, g, t, 1, "fft_y_inv", info);
+}
+
+// pass 4: conj + C2R along x with scale 1 / (M * Py * Pz), in place -> real PCM in ws.spec_a (row pitch 2*pitch floats)
+static int pcm_pass_x_c2r(bs_ctx* ctx, const PcmGeometry& g, PcmDeviceTables* t, char* info) {
+    XC2RArgs a;
+    a.spec = (float2*)ctx->ws.spec_a;
+    a.Px = g.P[0]; a.Py = g.P[1]; a.Pz = g.P[2]; a.M = g.M; a.pitch = g.pitch;
+    a.tw = t->tw[0];
+    a.plan = g.plan_x;
+    a.lshift = g.lshift_x;
+    a.scale = (float)(1.0 / ((double)g.M * (double)g.P[1] * (double)g.P[2]));
+    const int LB = 1 << g.lshift_x;
+    dim3 grid((g.P[1] + LB - 1) / LB, g.P[2], 1);
     {
-        StridedArgs a;
-        a.a = sa; a.b = sb;
-        a.estride = g.pitch;
-        a.ostride = (long long)g.P[1] * g.pitch;
-        a.tw = t->tw[1];
-        a.plan = g.plan_y;
-        a.tshift = g.tshift_y;
-        a.mode = 0;
-        a.thresh = 0.f;
-        dim3 grid(g.pitch >> g.tshift_y, g.P[2], 1);
-        bs_launch_scope sc(ctx, "fft_y_inv");
-        const size_t smem_pipe = ((size_t)((g.P[1] + 1) & ~1) + 3 * (size_t)g.P[1] * (1 << g.tshift_y)) * sizeof(float2);
-        if (g.static_y) {
-            launch_col540(ctx, a, g.pitch / COL540_TC, g.P[2], 1);
-        } else if (smem_pipe <= PCM_SMEM_MAX) {
-            StridedPipeArgs pp;
-            pp.s = a;
-            pp.tiles_x = g.pitch >> g.tshift_y;
-            pp.n_other = g.P[2];
-            pp.n_tiles = pp.tiles_x * pp.n_other * 1;
-            const int per_sm = std::max(1, std::min(2, (int)(PCM_SMEM_MAX / (smem_pipe + 1024))));
-            const int nctas = std::min(pp.n_tiles, ctx->sm_count * per_sm);
-            k_fft_strided_pipe<FftGeneric><<<nctas, PCM_THREADS, smem_pipe, ctx->stream>>>(pp);
-        } else k_fft_strided<FftGeneric><<<grid, PCM_THREADS, g.smem_y, ctx->stream>>>(a);
-    }
-    BS_CUDA(ctx, cudaGetLastError());
-    {
-        XC2RArgs a;
-        a.spec = sa;
-        a.Px = g.P[0]; a.Py = g.P[1]; a.Pz = g.P[2]; a.M = g.M; a.pitch = g.pitch;
-        a.tw = t->tw[0];
-        a.plan = g.plan_x;
-        a.lshift = g.lshift_x;
-        a.scale = (float)(1.0 / ((double)g.M * (double)g.P[1] * (double)g.P[2]));
-        const int LB = 1 << g.lshift_x;
-        dim3 grid((g.P[1] + LB - 1) / LB, g.P[2], 1);
         bs_launch_scope sc(ctx, "fft_x_c2r");
         const size_t smem_w = ((size_t)g.P[0] + (size_t)(PCM_THREADS / 32) * 2 * (g.M + 1)) * sizeof(float2);
         if (env_int("BS_FFT_X_WARP", 1) && g.M <= 32 * XW_MAXV - 1 && smem_w <= PCM_SMEM_MAX) {
             const long long n_lines = (long long)g.P[1] * g.P[2];
             const int per_sm = std::max(1, std::min(6, (int)(PCM_SMEM_MAX / (smem_w + 1024))));
             const int nctas = (int)std::min<long long>((n_lines + 7) / 8, (long long)ctx->sm_count * per_sm);
-            if (g.M == FftW270::N && env_int("BS_FFT_STATIC", 1)) k_fft_x_c2r_w<FftW270><<<nctas, PCM_THREADS, smem_w, ctx->stream>>>(a);
-            else k_fft_x_c2r_w<FftWGeneric><<<nctas, PCM_THREADS, smem_w, ctx->stream>>>(a);
-        } else if (g.static_x && g.lshift_x == 3) k_fft_x_c2r<FftX270L8><<<grid, PCM_THREADS, g.smem_x_c2r, ctx->stream>>>(a);
-        else if (g.static_x) k_fft_x_c2r<FftX270><<<grid, PCM_THREADS, g.smem_x_c2r, ctx->stream>>>(a);
-        else k_fft_x_c2r<FftGeneric><<<grid, PCM_THREADS, g.smem_x_c2r, ctx->stream>>>(a);
+            if (g.M == FftW270::N && env_int("BS_FFT_STATIC", 1)) {
+                k_fft_x_c2r_w<FftW270><<<nctas, PCM_THREADS, smem_w, ctx->stream>>>(a);
+                pass_info(info, "k_fft_x_c2r_w<FftW270>", nullptr);
+            } else {
+                k_fft_x_c2r_w<FftWGeneric><<<nctas, PCM_THREADS, smem_w, ctx->stream>>>(a);
+                pass_info(info, "k_fft_x_c2r_w<FftWGeneric>", &g.plan_x);
+            }
+        } else if (g.static_x && g.lshift_x == 3) {
+            k_fft_x_c2r<FftX270L8><<<grid, PCM_THREADS, g.smem_x_c2r, ctx->stream>>>(a);
+            pass_info(info, "k_fft_x_c2r<FftX270L8>", nullptr);
+        } else if (g.static_x) {
+            k_fft_x_c2r<FftX270><<<grid, PCM_THREADS, g.smem_x_c2r, ctx->stream>>>(a);
+            pass_info(info, "k_fft_x_c2r<FftX270>", nullptr);
+        } else {
+            k_fft_x_c2r<FftGeneric><<<grid, PCM_THREADS, g.smem_x_c2r, ctx->stream>>>(a);
+            pass_info(info, "k_fft_x_c2r<FftGeneric>", &g.plan_x);
+        }
     }
     BS_CUDA(ctx, cudaGetLastError());
     return BS_OK;
+}
+
+// forward pipeline up to the real PCM in ws.spec_a (row pitch 2*pitch floats)
+static int pcm_compute_pcm(bs_ctx* ctx, const void* d1, const void* d2, int dtype, const PcmGeometry& g,
+                           PcmDeviceTables* t) {
+    int rc;
+    if ((rc = pcm_kernel_attrs(ctx))) return rc;
+    if ((rc = pcm_pass_x_r2c(ctx, d1, d2, dtype, g, t, nullptr))) return rc;
+    if ((rc = pcm_pass_y_fwd(ctx, g, t, nullptr))) return rc;
+    if ((rc = pcm_pass_z_xpower(ctx, g, t, nullptr))) return rc;
+    if ((rc = pcm_pass_y_inv(ctx, g, t, nullptr))) return rc;
+    return pcm_pass_x_c2r(ctx, g, t, nullptr);
 }
 
 static void solve3(const double H[3][3], const double rhs[3], double out[3]) {
@@ -2510,6 +2558,58 @@ int bs_pcm_debug_pcm(bs_ctx* ctx, const void* img1, const void* img2, const long
                                    sizeof(float) * g.P[0], (size_t)g.P[1] * g.P[2], cudaMemcpyDeviceToHost, ctx->stream));
     BS_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     if (pad_out) for (int d = 0; d < 3; ++d) pad_out[d] = g.P[d];
+    return BS_OK;
+}
+
+int bs_pcm_debug_pass(bs_ctx* ctx, int pass, const long long dims[3], int dtype, const int extension[3], const void* in_a,
+                      const void* in_b, void* out_a, void* out_b, int poison, int pad_out[3], char info[128]) {
+    if (!ctx) return BS_ERR_ARG;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (pass < 0 || pass > 4) return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_debug_pass: pass %d not in [0,4]", pass);
+    const bool two = pass <= 2;          // passes 0..2 read both spectra / crops
+    if (!dims || !extension || !in_a || (two && !in_b) || !out_a || (pass <= 1 && !out_b))
+        return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_debug_pass: NULL argument");
+    if (pass == 0 && dtype != BS_DTYPE_U16 && dtype != BS_DTYPE_F32 && dtype != BS_DTYPE_U8)
+        return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_debug_pass: bad dtype %d", dtype);
+    BS_CUDA(ctx, cudaSetDevice(ctx->device));
+    PcmGeometry g;
+    int rc = pcm_geometry(ctx, dims, extension, &g);
+    if (rc) return rc;
+    PcmDeviceTables* t;
+    if ((rc = pcm_tables(ctx, g, &t))) return rc;
+    if ((rc = pcm_workspace(ctx, g))) return rc;
+    if ((rc = pcm_kernel_attrs(ctx))) return rc;
+    bs_pcm_workspace& ws = ctx->ws;
+    const size_t spec_bytes = (size_t)g.P[2] * g.P[1] * g.pitch * sizeof(float2);
+    const size_t row = (size_t)(g.M + 1) * sizeof(float2), rows = (size_t)g.P[1] * g.P[2];
+    void* spec[2] = {ws.spec_a, ws.spec_b};
+    const void* in[2] = {in_a, in_b};
+    void* out[2] = {out_a, out_b};
+    for (int i = 0; i < 2; ++i) BS_CUDA(ctx, cudaMemsetAsync(spec[i], poison ? 0xff : 0, spec_bytes, ctx->stream));
+    if (pass >= 1)
+        for (int i = 0; i < (two ? 2 : 1); ++i)
+            BS_CUDA(ctx, cudaMemcpy2DAsync(spec[i], sizeof(float2) * g.pitch, in[i], row, row, rows, cudaMemcpyHostToDevice,
+                                           ctx->stream));
+    char buf[PCM_INFO_LEN] = "";
+    switch (pass) {
+        case 0: rc = pcm_pass_x_r2c(ctx, in_a, in_b, dtype, g, t, buf); break;
+        case 1: rc = pcm_pass_y_fwd(ctx, g, t, buf); break;
+        case 2: rc = pcm_pass_z_xpower(ctx, g, t, buf); break;
+        case 3: rc = pcm_pass_y_inv(ctx, g, t, buf); break;
+        default: rc = pcm_pass_x_c2r(ctx, g, t, buf); break;
+    }
+    if (rc) return rc;
+    if (pass == 4) {
+        BS_CUDA(ctx, cudaMemcpy2DAsync(out_a, sizeof(float) * g.P[0], ws.spec_a, sizeof(float2) * g.pitch,
+                                       sizeof(float) * g.P[0], rows, cudaMemcpyDeviceToHost, ctx->stream));
+    } else {
+        for (int i = 0; i < (pass <= 1 ? 2 : 1); ++i)
+            BS_CUDA(ctx, cudaMemcpy2DAsync(out[i], row, spec[i], sizeof(float2) * g.pitch, row, rows,
+                                           cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    BS_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (pad_out) for (int d = 0; d < 3; ++d) pad_out[d] = g.P[d];
+    if (info) memcpy(info, buf, PCM_INFO_LEN);
     return BS_OK;
 }
 

@@ -103,7 +103,7 @@ SYMBOLS = [
     "bs_version", "bs_init", "bs_destroy", "bs_last_error", "bs_synchronize", "bs_launch_count",
     "bs_profile_enable", "bs_profile_reset", "bs_profile_get", "bs_host_alloc", "bs_host_free",
     "bs_pcm_default_params", "bs_pcm_pair", "bs_pcm_batch", "bs_pcm_volumes_batch", "bs_good_fft_size", "bs_pcm_debug_pcm",
-    "bs_pcm_debug_pearson",
+    "bs_pcm_debug_pearson", "bs_pcm_debug_pass",
     "bs_fuse_default_params", "bs_volume_upload", "bs_volume_upload_async", "bs_volume_wrap", "bs_volume_free",
     "bs_content_weights", "bs_volume_info", "bs_volume_download", "bs_volume_devptr", "bs_downsample", "bs_fuse_block", "bs_fuse_blocks",
     "bs_fuse_block_to_volume", "bs_fuse_accumulate", "bs_fuse_finish", "bs_mask_blocks", "bs_dog_default_params", "bs_dog_detect",
@@ -144,6 +144,7 @@ def load_library():
     lib.bs_good_fft_size.argtypes = [ip, ip]
     lib.bs_pcm_debug_pcm.argtypes = [vp, vp, vp, P(ll), ip, P(ip), vp, P(ip)]
     lib.bs_pcm_debug_pearson.argtypes = [vp, vp, vp, P(ll), ip, ip, P(ip), vp]
+    lib.bs_pcm_debug_pass.argtypes = [vp, ip, P(ll), ip, P(ip), vp, vp, vp, vp, ip, P(ip), C.c_char_p]
     lib.bs_fuse_default_params.argtypes = [P(FuseParamsC)]
     lib.bs_fuse_default_params.restype = None
     lib.bs_volume_upload.argtypes = [vp, vp, P(ll), ip, P(ull)]
@@ -335,6 +336,42 @@ class Context:
                                               _NP2BS[img1.dtype], ext, out.ctypes.data, pad))
         assert tuple(pad) == tuple(P)
         return out
+
+    def pcm_debug_pass(self, pass_no: int, dims_xyz, in_a, in_b=None, dtype=None, extension=(10, 10, 10), poison=True):
+        """Run one FFT pass of the PCM pipeline with the production launch (include/bsgpu.h bs_pcm_debug_pass states
+        what each pass computes).  Pass 0 takes two device crops ([z,y,x] CUDA tensors or int device pointers with
+        ``dtype``); passes 1-4 take host complex64 spectra [Pz, Py, M+1].  Returns (out_a, out_b, info): complex64
+        spectra (out_b is None from pass 2 on), or for pass 4 the float32 PCM [Pz, Py, Px] as out_a."""
+        dims = (C.c_longlong * 3)(*[int(v) for v in dims_xyz])
+        ext = (C.c_int * 3)(*[int(e) for e in extension])
+        P = [good_fft_size(d + (2 * d if d < e else 2 * e), i == 0) for i, (d, e) in enumerate(zip(dims_xyz, extension))]
+        M = P[0] // 2
+        spec_shape = (P[2], P[1], M + 1)
+        keep = []
+        if pass_no == 0:
+            (pa, da, _), (pb, db, _) = _ptr_of(in_a), _ptr_of(in_b)
+            if not (da and db):
+                raise ValueError("pass 0 takes device crops")
+            dt = _bs_dtype(in_a, dtype)
+        else:
+            dt = DTYPE_F32
+            ins = [in_a] + ([in_b] if pass_no <= 2 else [])
+            for x in ins:
+                x = np.ascontiguousarray(x, dtype=np.complex64)
+                if x.shape != spec_shape:
+                    raise ValueError(f"pass {pass_no} takes complex64 spectra of shape {spec_shape}, got {x.shape}")
+                keep.append(x)
+            pa = keep[0].ctypes.data
+            pb = keep[1].ctypes.data if len(keep) > 1 else None
+        out_a = np.empty((P[2], P[1], P[0]), np.float32) if pass_no == 4 else np.empty(spec_shape, np.complex64)
+        out_b = np.empty(spec_shape, np.complex64) if pass_no <= 1 else None
+        pad = (C.c_int * 3)()
+        info = C.create_string_buffer(128)
+        self._check(self.lib.bs_pcm_debug_pass(self.h, int(pass_no), dims, dt, ext, pa, pb, out_a.ctypes.data,
+                                               out_b.ctypes.data if out_b is not None else None, 1 if poison else 0,
+                                               pad, info))
+        assert tuple(pad) == tuple(P)
+        return out_a, out_b, info.value.decode()
 
     def pcm_debug_pearson(self, img1, img2, boxes, dtype=None) -> np.ndarray:
         """Pearson sums of explicit candidate boxes on two equal-shape crops on the device ([z,y,x] CUDA tensors),

@@ -131,6 +131,31 @@ int bs_good_fft_size(int n, int even);
 int bs_pcm_debug_pcm(bs_ctx* ctx, const void* img1, const void* img2, const long long dims[3],
                      int dtype, const int extension[3], float* out_pcm, int pad_out[3]);
 
+/* diagnostic: ONE pass of the PCM's FFT pipeline, with exactly the launch bs_pcm_* uses, on explicit inputs.
+ * Geometry as in bs_pcm_debug_pcm: P = padded dims {x,y,z}, M = P[0] / 2.  A "spectrum" is a host complex64 array
+ * [P[2]][P[1]][M+1] (x fastest; interleaved re, im float32).  All transforms are unnormalised forward DFTs
+ * F(v)[k] = sum_n v[n] exp(-2 pi i k n / N) along one axis:
+ *   pass 0  x R2C.   in_a / in_b: DEVICE pointers to the two crops (dims {x,y,z}, dtype); each is blended-mirror
+ *                    extended and zero padded to P (oracle/pcm_oracle.py blend_extend_pad), then out = rfft along x.
+ *                    out_a / out_b: the two spectra.
+ *   pass 1  y.       in_a / in_b: two spectra; out = F_y(in) for each.
+ *   pass 2  z cross-power.  in_a = A, in_b = B: out_a = F_z(conj(n(F_z A)) * n(F_z B)), n(c) = c / |c|, or 0 when
+ *                    |c| < 1e-5.
+ *   pass 3  y.       in_a: one spectrum; out_a = F_y(in_a).
+ *   pass 4  x C2R.   in_a: one spectrum H; out_a: float32 [P[2]][P[1]][P[0]] with, per line,
+ *                    out = irfft(conj(H), P[0]) / (P[1] P[2])   (numpy's irfft, 1 / P[0] normalised; the kernel
+ *                    scales its half-length transform by 1 / (M P[1] P[2])).  As in any C2R the imaginary parts of
+ *                    bins 0 and M are expected to be 0.
+ * The conjugations make passes 3 and 4 the inverse transforms: pass4(pass3(pass2(pass1(pass0(a, b))))) is the PCM
+ * irfftn(n(rfftn A) conj(n(rfftn B))) of bs_pcm_debug_pcm.
+ * in_b / out_b are ignored (may be NULL) for passes 3 and 4, out_b also for pass 2.  poison != 0 fills the device
+ * spectra with NaN bytes first, so anything a pass fails to write shows up as NaN.  info (may be NULL) receives the
+ * kernel instantiation launched, and for runtime-planned kernels the radices of the plan, e.g.
+ * "k_fft_strided_pipe<FftGeneric> 15x12x3" (NUL-terminated, at most 128 bytes). */
+int bs_pcm_debug_pass(bs_ctx* ctx, int pass, const long long dims[3], int dtype, const int extension[3],
+                      const void* in_a, const void* in_b, void* out_a, void* out_b, int poison, int pad_out[3],
+                      char info[128]);
+
 /* diagnostic: the Pearson sums of an explicit candidate list, computed by the same launch bs_pcm_* uses.
  * img1/img2: DEVICE pointers to two crops of dims {x,y,z}.  boxes: n * 9 ints per candidate, {o1[3], o2[3], sz[3]}
  * ({x,y,z} each): voxel o1 + p of img1 pairs with o2 + p of img2 for 0 <= p < sz; n <= 256.  sums_out: n * 5 values

@@ -319,6 +319,32 @@ JF(jlongArray, pcmDebugPcm)(JNIEnv* env, jclass, jlong ctx, jobject img1, jobjec
     return arr;
 }
 
+// diagnostic: one FFT pass of the PCM pipeline (include/bsgpu.h bs_pcm_debug_pass).  Pass 0: devA / devB are device
+// crops (volumeDevptr) and inA / inB are ignored; passes 1-4: inA / inB are complex64 spectra (float[2 * Pz*Py*(M+1)],
+// interleaved).  outA / outB: float[] spectra, or float[Pz*Py*Px] for pass 4.  padOut (may be null) receives {Px, Py, Pz};
+// returns the kernel info string.
+JF(jstring, pcmDebugPass)(JNIEnv* env, jclass, jlong ctx, jint pass, jlongArray dims, jint dtype, jintArray extension, jlong devA,
+                          jlong devB, jobject inA, jobject inB, jobject outA, jobject outB, jint poison, jlongArray padOut) {
+    long long d[3];
+    get3(env, dims, d);
+    jint e[3];
+    env->GetIntArrayRegion(extension, 0, 3, e);
+    const int ext[3] = {e[0], e[1], e[2]};
+    int pad[3] = {0, 0, 0};
+    char info[128] = "";
+    int rc;
+    {
+        Pinned ia(env, inA), ib(env, inB), oa(env, outA), ob(env, outB);
+        const void* a = pass == 0 ? reinterpret_cast<const void*>(devA) : ia.p;
+        const void* b = pass == 0 ? reinterpret_cast<const void*>(devB) : ib.p;
+        rc = bs_pcm_debug_pass(C(ctx), pass, d, dtype, ext, a, b, oa.p, ob.p, poison, pad, info);
+    }
+    if (failed(env, ctx, rc)) return nullptr;
+    const jlong p[3] = {pad[0], pad[1], pad[2]};
+    if (padOut) env->SetLongArrayRegion(padOut, 0, 3, p);
+    return env->NewStringUTF(info);
+}
+
 // diagnostic: Pearson sums of n explicit boxes (n x {o1[3], o2[3], sz[3]}) on two device crops (volumeDevptr);
 // sumsOut: long[5 n] (uint16 / uint8) or double[5 n] (float32)
 JF(void, pcmDebugPearson)(JNIEnv* env, jclass, jlong ctx, jlong dev1, jlong dev2, jlongArray dims, jint dtype, jintArray boxes,

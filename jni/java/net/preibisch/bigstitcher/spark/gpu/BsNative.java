@@ -55,6 +55,11 @@ public final class BsNative
 	public static native long[] pcmDebugPcm( long ctx, Object img1, Object img2, long[] dims, int dtype, int[] extension, Object outPcm );
 	/** device crops (volumeDevptr); boxes n x {o1[3], o2[3], sz[3]}; sumsOut long[5n] (integer input) or double[5n] (float32) */
 	public static native void pcmDebugPearson( long ctx, long dev1, long dev2, long[] dims, int dtype, int[] boxes, Object sumsOut );
+	/** one FFT pass (0..4) of the PCM pipeline: pass 0 reads the device crops devA / devB, passes 1..4 the interleaved
+	 *  complex64 spectra inA / inB (float[2 * Pz*Py*(M+1)]); outA / outB float[] spectra (pass 4: float[Pz*Py*Px] PCM);
+	 *  padOut (long[3], may be null) receives {Px, Py, Pz}; returns the kernel instantiation launched */
+	public static native String pcmDebugPass( long ctx, int pass, long[] dims, int dtype, int[] extension, long devA, long devB,
+			Object inA, Object inB, Object outA, Object outB, int poison, long[] padOut );
 
 	/** models n*12, handles n*{volume, content}, blend n*{border[3], range[3]}, windows n*{fullDims[3], windowMin[3]} or null;
 	 *  iparams {fusionType, interpolation, outDtype, blendLutN, outBigEndian (1: N5 block payload byte order)}; dparams {minIntensity, maxIntensity} */

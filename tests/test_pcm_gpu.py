@@ -1,15 +1,30 @@
 """GPU parity tests, hot path 1: libbsgpu (through the C ABI) against oracle/pcm_oracle.py.
 
 Bars (BASELINE.json north_star): integer peak / shift bit-identical; sub-pixel within 1e-3 px;
-Pearson r (exact integer sums on the device) within 1e-9.
+Pearson r (exact integer sums on the device) within 1e-9.  PCM volumes: relative L2 error against the float64
+PCM (oracle/pcm_passes.py) within PCM_BAR times the float32 oracle's own error on the same pair.
 """
 import numpy as np
 import pytest
 
 from oracle import pcm_oracle as po
+from oracle import pcm_passes as pp
 from tests import synth
 
 pytestmark = pytest.mark.gpu
+
+#: allowed relative L2 error of the device PCM, in multiples of the float32 oracle's error (about 1e-5 or less)
+PCM_BAR = 4.0
+
+
+def _check_pcm_volume(pg, a, b):
+    """Device PCM against the float64 PCM: relative L2 within PCM_BAR x the float32 oracle's, same argmax."""
+    ref = pp.pcm(a, b)
+    pc = po.calculate_pcm(a, b, workers=-1)
+    assert pg.shape == pc.shape == ref.shape
+    e32, eg = pp.rel_l2(pc, ref), pp.rel_l2(pg, ref)
+    assert eg <= PCM_BAR * e32, (eg, e32)
+    assert np.unravel_index(np.argmax(pg), pg.shape) == np.unravel_index(np.argmax(ref), ref.shape)
 
 
 def _check(ctx, a, b, **kw):
@@ -32,12 +47,7 @@ def _check(ctx, a, b, **kw):
 
 def test_pcm_volume_matches_oracle(ctx):
     a, b = synth.shifted_pair((40, 48, 56), (3, -2, 1), seed=1)
-    pg = ctx.pcm_debug_pcm(a, b)
-    pc = po.calculate_pcm(a, b)
-    assert pg.shape == pc.shape
-    scale = np.abs(pc).max()
-    assert np.abs(pg - pc).max() < 2e-4 * scale
-    assert np.unravel_index(np.argmax(pg), pg.shape) == np.unravel_index(np.argmax(pc), pc.shape)
+    _check_pcm_volume(ctx.pcm_debug_pcm(a, b), a, b)
 
 
 @pytest.mark.parametrize("shape,shift,seed", [
@@ -162,17 +172,15 @@ def test_oversized_dims_rejected_before_any_copy(ctx):
 # selected per axis, so three thin crops reach each of them cheaply; the full 512^3 pair is the bench unit.
 @pytest.mark.parametrize("shape,shift", [
     ((24, 24, 500), (7, -3, 2)),     # x pads to 540  -> k_fft_x_r2c_w / k_fft_x_c2r_w <FftWStatic<270>>
-    ((24, 500, 24), (-2, 9, 1)),     # y pads to 540  -> k_fft_strided_pipe <FftStatic<540>>
-    ((500, 24, 24), (3, 2, -11)),    # z pads to 540  -> k_fft_strided mode 1 (cross-power) <FftStatic<540>>
+    ((24, 500, 24), (-2, 9, 1)),     # y pads to 540  -> k_fft_col540
+    ((500, 24, 24), (3, 2, -11)),    # z pads to 540  -> k_fft_xpower_col540 (cross-power)
     ((500, 500, 24), (1, -8, 6)),    # y and z static, x generic
 ])
 def test_static_540_plans_thin_crops(ctx, shape, shift):
     a, b = synth.shifted_pair(shape, shift, seed=80 + shape[0] % 7, margin=16)
     g, o = _check(ctx, a, b)
     assert 540 in g.pad
-    pg = ctx.pcm_debug_pcm(a, b)
-    pc = po.calculate_pcm(a, b, workers=-1)
-    assert np.abs(pg - pc).max() < 2e-4 * np.abs(pc).max()
+    _check_pcm_volume(ctx.pcm_debug_pcm(a, b), a, b)
 
 
 def test_static_540_thin_subpixel(ctx):
@@ -196,6 +204,8 @@ def test_full_512_pair_subpixel_bench_unit(ctx):
     assert g.n_overlap_px == o.n_overlap_px and abs(g.r - o.r) < 1e-9
     assert np.allclose(g.shift_sub, o.shift_sub, atol=1e-3), (g.shift_sub, o.shift_sub)
     assert np.allclose(g.shift_sub, (11.37, -4.62, 7.3), atol=0.2)
+    # The float64 PCM of this size needs several GB of host memory, so the volume keeps the float32 oracle's
+    # max-norm bar; the per-pass tests (test_pcm_fft_passes_gpu.py) cover the 540-point kernels in float64.
     pg = ctx.pcm_debug_pcm(a, b)
     pc = po.calculate_pcm(a, b, workers=-1)
     assert np.abs(pg - pc).max() < 2e-4 * np.abs(pc).max()
