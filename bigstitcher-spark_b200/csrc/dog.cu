@@ -15,6 +15,7 @@
 // detections with a global counter.  HBM-bound stencil work, no tensor cores.
 #include <algorithm>
 #include <cmath>
+#include <cstdio>
 #include <cstring>
 #include <vector>
 
@@ -224,7 +225,8 @@ struct ExtremaArgs {
     int e0[3];              // first candidate voxel inside the region (halo + 1)
     int cdims[3];           // candidate box
     long long rmin[3];      // region origin in image coordinates
-    float thr_initial, thr_final;
+    float thr_initial;      // candidates: |DoG| >= (float)(threshold / 3), a float32 compare
+    double thr_final;       // kept: |value| >= threshold, compared in double like the oracle (PARITY_GAPS #26)
     int find_max, find_min, localize;
     bs_dog_point* out;
     int max_points;
@@ -290,7 +292,7 @@ __global__ void __launch_bounds__(256) k_dog_extrema(const __grid_constant__ Ext
                 d[0] = d[1] = d[2] = 0.0;
             }
             if (fabs(val) < a.thr_final) return;
-        } else if (fabsf(v) < a.thr_final) {
+        } else if (fabs((double)v) < a.thr_final) {
             return;
         }
         const int slot = atomicAdd(a.counter, 1);
@@ -319,6 +321,114 @@ std::vector<float> dog_kernel(double sigma, int* r_out) {
     return out;
 }
 
+// blur variants (bs_dog_debug_dog's `blur` argument; 0 = the production choice from rb)
+enum { DOG_BLUR_AUTO = 0, DOG_BLUR_GENERIC = 1, DOG_BLUR_WIN6 = 2, DOG_BLUR_WIN12 = 3 };
+
+// the region one block is computed on: interval + halo per axis, rows padded to a multiple of 8 floats
+struct DogRegion {
+    long long rmin[3];      // origin in image coordinates (may be negative)
+    int rdims[3];           // rdims[0] is the padded row pitch
+    int halo;               // max(ra, rb) + 1: kernel reach + the 3x3x3 neighbourhood
+    const float* dog;       // (G_sa * I' - G_sb * I') / (k - 1) over the region (context workspace)
+};
+
+// Checks the interval and the intensity / sigma parameters, then runs k_dog_load and the three blur passes of one
+// block on the context's stream: the single copy of these launches, shared by bs_dog_detect and bs_dog_debug_dog.
+// Called with ctx->mu held.  info (may be NULL): the blur instantiation launched and the radii.
+int dog_load_blur(bs_ctx* ctx, const char* who, const bs_volume& v, const long long interval_min[3],
+                  const long long interval_size[3], const bs_dog_params* p, int blur, DogRegion* reg, char* info) {
+    if (!(p->sigma > 0.5) || !(p->max_intensity > p->min_intensity))
+        return bs_set_error(ctx, BS_ERR_ARG, "%s: need sigma > 0.5 (image sigma), max_intensity > min_intensity", who);
+    for (int d = 0; d < 3; ++d)
+        if (interval_size[d] <= 0 || interval_min[d] < 0 || interval_min[d] + interval_size[d] > v.dims[d])
+            return bs_set_error(ctx, BS_ERR_ARG, "%s: interval outside the volume (axis %d)", who, d);
+    // DoGImgLib2.computeSigmas: 4 steps per octave, image sigma 0.5
+    const double k = std::pow(2.0, 0.25), image_sigma = 0.5;
+    const double s1 = p->sigma, s2 = p->sigma * k;
+    const double sa = std::sqrt(s1 * s1 - image_sigma * image_sigma), sb = std::sqrt(s2 * s2 - image_sigma * image_sigma);
+    int ra, rb;
+    const std::vector<float> ka = dog_kernel(sa, &ra), kb = dog_kernel(sb, &rb);
+    if (rb > DOG_MAXR) return bs_set_error(ctx, BS_ERR_UNSUPPORTED, "%s: sigma too large (kernel radius %d > %d)", who, rb, DOG_MAXR);
+    if (blur == DOG_BLUR_AUTO) blur = rb <= 6 ? DOG_BLUR_WIN6 : (rb <= DOG_WIN_MAXR ? DOG_BLUR_WIN12 : DOG_BLUR_GENERIC);
+    if (blur < DOG_BLUR_GENERIC || blur > DOG_BLUR_WIN12 || (blur == DOG_BLUR_WIN6 && rb > 6) || (blur == DOG_BLUR_WIN12 && rb > 12))
+        return bs_set_error(ctx, BS_ERR_ARG, "%s: blur variant %d cannot run kernel radius %d", who, blur, rb);
+    const int halo = std::max(ra, rb) + 1;
+    long long nreg = 1;
+    for (int d = 0; d < 3; ++d) {
+        reg->rmin[d] = interval_min[d] - halo;
+        const long long rd = interval_size[d] + 2LL * halo;
+        if (rd > 0x7fffffffLL) return bs_set_error(ctx, BS_ERR_ARG, "%s: interval too large", who);
+        reg->rdims[d] = (int)rd;
+        nreg *= rd;
+    }
+    int* rdims = reg->rdims;
+    if (rdims[1] > 65535 || rdims[2] > 65535)
+        return bs_set_error(ctx, BS_ERR_ARG, "%s: block too large in y / z (%d x %d incl. halo, limit 65535): detect block-wise", who, rdims[1], rdims[2]);
+    // the region's rows are padded to a multiple of 8 floats (more halo on the right: the extra columns hold real
+    // mirror-extended image data, so every used voxel is unchanged) -> aligned float4 windows in the x pass
+    nreg = nreg / rdims[0];
+    rdims[0] = (rdims[0] + 7) & ~7;
+    nreg *= rdims[0];
+    reg->halo = halo;
+    if (!ctx->dog) ctx->dog = new DogWs();
+    DogWs* W = (DogWs*)ctx->dog;
+    for (int i = 0; i < 4; ++i) {
+        const int rc = bs_ensure_dev(ctx, &W->buf[i], &W->cap[i], sizeof(float) * (size_t)nreg);
+        if (rc) return rc;
+    }
+    float *r0 = (float*)W->buf[0], *r1 = (float*)W->buf[1], *r2 = (float*)W->buf[2], *r3 = (float*)W->buf[3];
+    const int blocks = (int)std::min<long long>((nreg + 255) / 256, (long long)ctx->sm_count * 32);
+    {
+        LoadArgs a;
+        a.src = v.dev; a.dtype = v.dtype;
+        for (int d = 0; d < 3; ++d) { a.vdims[d] = (int)v.dims[d]; a.rmin[d] = reg->rmin[d]; a.rdims[d] = rdims[d]; }
+        a.offset = (float)p->min_intensity;
+        a.scale = (float)(1.0 / (p->max_intensity - p->min_intensity));
+        a.out = r0;
+        bs_launch_scope sc(ctx, "dog_load");
+        k_dog_load<<<dim3((unsigned)((rdims[0] + 255) / 256), (unsigned)rdims[1], (unsigned)rdims[2]), 256, 0, ctx->stream>>>(a);
+    }
+    BS_CUDA(ctx, cudaGetLastError());
+    const float dog_scale = (float)(1.0 / (k - 1.0));           // K_MIN1_INV
+    if (blur != DOG_BLUR_GENERIC) {
+        BlurWinArgs b;
+        memset(&b, 0, sizeof(b));
+        for (int d = 0; d < 3; ++d) b.dims[d] = rdims[d];
+        b.scale = dog_scale;
+        for (int t = 0; t <= ra; ++t) b.ka[t] = ka[(size_t)(ra + t)];
+        for (int t = 0; t <= rb; ++t) b.kb[t] = kb[(size_t)(rb + t)];
+        const int wblocks = (int)std::min<long long>((nreg / DOG_CH + 255) / 256 + 1, (long long)ctx->sm_count * 32);
+        if (blur == DOG_BLUR_WIN6) dog_blur_windowed<6>(ctx, b, r0, r1, r2, r3, wblocks);
+        else dog_blur_windowed<12>(ctx, b, r0, r1, r2, r3, wblocks);
+        BS_CUDA(ctx, cudaGetLastError());
+    } else {
+        BlurArgs b;
+        memset(&b, 0, sizeof(b));
+        for (int d = 0; d < 3; ++d) b.dims[d] = rdims[d];
+        b.ra = ra; b.rb = rb;
+        memcpy(b.ka, ka.data(), sizeof(float) * ka.size());
+        memcpy(b.kb, kb.data(), sizeof(float) * kb.size());
+        b.scale = dog_scale;
+        // x: r0 -> (r1, r2); y: (r1, r2) -> (r3, r0); z: (r3, r0) -> r1 = DoG
+        const float* ina[3] = {r0, r1, r3};
+        const float* inb[3] = {r0, r2, r0};
+        float* outa[3] = {r1, r3, r1};
+        float* outb[3] = {r2, r0, nullptr};
+        for (int axis = 0; axis < 3; ++axis) {
+            b.in_a = ina[axis]; b.in_b = inb[axis]; b.out_a = outa[axis]; b.out_b = outb[axis]; b.axis = axis;
+            bs_launch_scope sc(ctx, "dog_blur");
+            k_dog_blur<<<blocks, 256, 0, ctx->stream>>>(b);
+            BS_CUDA(ctx, cudaGetLastError());
+        }
+    }
+    reg->dog = r1;
+    if (info) {
+        const char* name = blur == DOG_BLUR_GENERIC ? "k_dog_blur" : (blur == DOG_BLUR_WIN6 ? "k_dog_blur_x<6>" : "k_dog_blur_x<12>");
+        snprintf(info, 128, "%s ra=%d rb=%d", name, ra, rb);
+    }
+    return BS_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -344,105 +454,29 @@ int bs_dog_detect(bs_ctx* ctx, unsigned long long vol_handle, const long long in
     *n_found = 0;
     auto it = ctx->vols.find(vol_handle);
     if (it == ctx->vols.end()) return bs_set_error(ctx, BS_ERR_ARG, "bs_dog_detect: unknown handle %llu", vol_handle);
-    if (!(p->sigma > 0.5) || !(p->max_intensity > p->min_intensity) || !(p->threshold >= 0.0))
-        return bs_set_error(ctx, BS_ERR_ARG, "bs_dog_detect: need sigma > 0.5 (image sigma), max_intensity > min_intensity, threshold >= 0");
+    if (!(p->threshold >= 0.0)) return bs_set_error(ctx, BS_ERR_ARG, "bs_dog_detect: need threshold >= 0");
     BS_CUDA(ctx, cudaSetDevice(ctx->device));
     int rc = bs_volume_acquire(ctx, it->second);
     if (rc) return rc;
     const bs_volume v = it->second;
-    for (int d = 0; d < 3; ++d)
-        if (interval_size[d] <= 0 || interval_min[d] < 0 || interval_min[d] + interval_size[d] > v.dims[d])
-            return bs_set_error(ctx, BS_ERR_ARG, "bs_dog_detect: interval outside the volume (axis %d)", d);
-    // DoGImgLib2.computeSigmas: 4 steps per octave, image sigma 0.5
-    const double k = std::pow(2.0, 0.25), image_sigma = 0.5;
-    const double s1 = p->sigma, s2 = p->sigma * k;
-    const double sa = std::sqrt(s1 * s1 - image_sigma * image_sigma), sb = std::sqrt(s2 * s2 - image_sigma * image_sigma);
-    int ra, rb;
-    const std::vector<float> ka = dog_kernel(sa, &ra), kb = dog_kernel(sb, &rb);
-    if (rb > DOG_MAXR) return bs_set_error(ctx, BS_ERR_UNSUPPORTED, "bs_dog_detect: sigma too large (kernel radius %d > %d)", rb, DOG_MAXR);
-    const int halo = std::max(ra, rb) + 1;      // kernel reach + the 3x3x3 neighbourhood
-    long long rmin[3];
-    int rdims[3];
-    long long nreg = 1;
-    for (int d = 0; d < 3; ++d) {
-        rmin[d] = interval_min[d] - halo;
-        const long long rd = interval_size[d] + 2LL * halo;
-        if (rd > 0x7fffffffLL) return bs_set_error(ctx, BS_ERR_ARG, "bs_dog_detect: interval too large");
-        rdims[d] = (int)rd;
-        nreg *= rd;
-    }
-    if (rdims[1] > 65535 || rdims[2] > 65535)
-        return bs_set_error(ctx, BS_ERR_ARG, "bs_dog_detect: block too large in y / z (%d x %d incl. halo, limit 65535): detect block-wise", rdims[1], rdims[2]);
-    // the region's rows are padded to a multiple of 8 floats (more halo on the right: the extra columns hold real
-    // mirror-extended image data, so every used voxel is unchanged) -> aligned float4 windows in the x pass
-    nreg = nreg / rdims[0];
-    rdims[0] = (rdims[0] + 7) & ~7;
-    nreg *= rdims[0];
-    if (!ctx->dog) ctx->dog = new DogWs();
+    DogRegion reg;
+    rc = dog_load_blur(ctx, "bs_dog_detect", v, interval_min, interval_size, p, DOG_BLUR_AUTO, &reg, nullptr);
+    if (rc) return rc;
     DogWs* W = (DogWs*)ctx->dog;
-    for (int i = 0; i < 4; ++i) {
-        rc = bs_ensure_dev(ctx, &W->buf[i], &W->cap[i], sizeof(float) * (size_t)nreg);
-        if (rc) return rc;
-    }
     rc = bs_ensure_dev(ctx, &W->pts, &W->pts_cap, sizeof(bs_dog_point) * (size_t)std::max(1, max_points));
     if (rc) return rc;
     if (!W->count) BS_CUDA(ctx, cudaMalloc(&W->count, sizeof(int)));
-    float *r0 = (float*)W->buf[0], *r1 = (float*)W->buf[1], *r2 = (float*)W->buf[2], *r3 = (float*)W->buf[3];
     bs_dog_point* dpts = (bs_dog_point*)W->pts;
     int* dcount = W->count;
 #define DOG_CUDA(call) BS_CUDA(ctx, call)
     DOG_CUDA(cudaMemsetAsync(dcount, 0, sizeof(int), ctx->stream));
-    const int blocks = (int)std::min<long long>((nreg + 255) / 256, (long long)ctx->sm_count * 32);
-    {
-        LoadArgs a;
-        a.src = v.dev; a.dtype = v.dtype;
-        for (int d = 0; d < 3; ++d) { a.vdims[d] = (int)v.dims[d]; a.rmin[d] = rmin[d]; a.rdims[d] = rdims[d]; }
-        a.offset = (float)p->min_intensity;
-        a.scale = (float)(1.0 / (p->max_intensity - p->min_intensity));
-        a.out = r0;
-        bs_launch_scope sc(ctx, "dog_load");
-        k_dog_load<<<dim3((unsigned)((rdims[0] + 255) / 256), (unsigned)rdims[1], (unsigned)rdims[2]), 256, 0, ctx->stream>>>(a);
-    }
-    DOG_CUDA(cudaGetLastError());
-    const float dog_scale = (float)(1.0 / (k - 1.0));           // K_MIN1_INV
-    if (rb <= DOG_WIN_MAXR) {
-        BlurWinArgs b;
-        memset(&b, 0, sizeof(b));
-        for (int d = 0; d < 3; ++d) b.dims[d] = rdims[d];
-        b.scale = dog_scale;
-        for (int t = 0; t <= ra; ++t) b.ka[t] = ka[(size_t)(ra + t)];
-        for (int t = 0; t <= rb; ++t) b.kb[t] = kb[(size_t)(rb + t)];
-        const int wblocks = (int)std::min<long long>((nreg / DOG_CH + 255) / 256 + 1, (long long)ctx->sm_count * 32);
-        if (rb <= 6) dog_blur_windowed<6>(ctx, b, r0, r1, r2, r3, wblocks);
-        else dog_blur_windowed<12>(ctx, b, r0, r1, r2, r3, wblocks);
-        DOG_CUDA(cudaGetLastError());
-    } else {
-        BlurArgs b;
-        memset(&b, 0, sizeof(b));
-        for (int d = 0; d < 3; ++d) b.dims[d] = rdims[d];
-        b.ra = ra; b.rb = rb;
-        memcpy(b.ka, ka.data(), sizeof(float) * ka.size());
-        memcpy(b.kb, kb.data(), sizeof(float) * kb.size());
-        b.scale = dog_scale;
-        // x: r0 -> (r1, r2); y: (r1, r2) -> (r3, r0); z: (r3, r0) -> r1 = DoG
-        const float* ina[3] = {r0, r1, r3};
-        const float* inb[3] = {r0, r2, r0};
-        float* outa[3] = {r1, r3, r1};
-        float* outb[3] = {r2, r0, nullptr};
-        for (int axis = 0; axis < 3; ++axis) {
-            b.in_a = ina[axis]; b.in_b = inb[axis]; b.out_a = outa[axis]; b.out_b = outb[axis]; b.axis = axis;
-            bs_launch_scope sc(ctx, "dog_blur");
-            k_dog_blur<<<blocks, 256, 0, ctx->stream>>>(b);
-            DOG_CUDA(cudaGetLastError());
-        }
-    }
     {
         ExtremaArgs a;
-        a.dog = r1;
+        a.dog = reg.dog;
         for (int d = 0; d < 3; ++d) {
-            a.rdims[d] = rdims[d]; a.e0[d] = halo; a.cdims[d] = (int)interval_size[d]; a.rmin[d] = rmin[d];
+            a.rdims[d] = reg.rdims[d]; a.e0[d] = reg.halo; a.cdims[d] = (int)interval_size[d]; a.rmin[d] = reg.rmin[d];
         }
-        a.thr_final = (float)p->threshold;
+        a.thr_final = p->threshold;
         a.thr_initial = p->localization ? (float)(p->threshold / 3.0) : (float)p->threshold;
         a.find_max = p->find_max; a.find_min = p->find_min; a.localize = p->localization ? 1 : 0;
         a.out = dpts; a.max_points = max_points; a.counter = dcount;
@@ -467,6 +501,35 @@ int bs_dog_detect(bs_ctx* ctx, unsigned long long vol_handle, const long long in
     }
 #undef DOG_CUDA
     *n_found = n;      // > max_points: the caller's buffer was too small, the first max_points (unsorted subset) were kept
+    return BS_OK;
+}
+
+int bs_dog_debug_dog(bs_ctx* ctx, unsigned long long vol_handle, const long long interval_min[3],
+                     const long long interval_size[3], const bs_dog_params* p, int blur, float* out, char info[128]) {
+    if (!ctx) return BS_ERR_ARG;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (!interval_min || !interval_size || !p || !out)
+        return bs_set_error(ctx, BS_ERR_ARG, "bs_dog_debug_dog: bad argument");
+    auto it = ctx->vols.find(vol_handle);
+    if (it == ctx->vols.end()) return bs_set_error(ctx, BS_ERR_ARG, "bs_dog_debug_dog: unknown handle %llu", vol_handle);
+    BS_CUDA(ctx, cudaSetDevice(ctx->device));
+    int rc = bs_volume_acquire(ctx, it->second);
+    if (rc) return rc;
+    const bs_volume v = it->second;
+    DogRegion reg;
+    char buf[128] = "";
+    rc = dog_load_blur(ctx, "bs_dog_debug_dog", v, interval_min, interval_size, p, blur, &reg, buf);
+    if (rc) return rc;
+    // the box the extremum stage reads: region voxels [halo - 1, halo + size + 1) per axis
+    const size_t bx = (size_t)interval_size[0] + 2, by = (size_t)interval_size[1] + 2, bz = (size_t)interval_size[2] + 2;
+    const size_t pitch = (size_t)reg.rdims[0] * sizeof(float);
+    for (size_t z = 0; z < bz; ++z) {
+        const float* src = reg.dog + ((size_t)(reg.halo - 1 + z) * reg.rdims[1] + (size_t)(reg.halo - 1)) * reg.rdims[0] + (reg.halo - 1);
+        BS_CUDA(ctx, cudaMemcpy2DAsync(out + z * bx * by, bx * sizeof(float), src, pitch, bx * sizeof(float), by,
+                                       cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    BS_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (info) memcpy(info, buf, sizeof(buf));
     return BS_OK;
 }
 

@@ -107,7 +107,7 @@ SYMBOLS = [
     "bs_fuse_default_params", "bs_volume_upload", "bs_volume_upload_async", "bs_volume_wrap", "bs_volume_free",
     "bs_content_weights", "bs_volume_info", "bs_volume_download", "bs_volume_devptr", "bs_downsample", "bs_fuse_block", "bs_fuse_blocks",
     "bs_fuse_block_to_volume", "bs_fuse_accumulate", "bs_fuse_finish", "bs_mask_blocks", "bs_dog_default_params", "bs_dog_detect",
-    "bs_comm_unique_id", "bs_comm_init", "bs_comm_destroy", "bs_fuse_allreduce",
+    "bs_dog_debug_dog", "bs_comm_unique_id", "bs_comm_init", "bs_comm_destroy", "bs_fuse_allreduce",
 ]
 
 
@@ -170,6 +170,7 @@ def load_library():
     lib.bs_dog_default_params.argtypes = [P(DogParamsC)]
     lib.bs_dog_default_params.restype = None
     lib.bs_dog_detect.argtypes = [vp, ull, P(ll), P(ll), P(DogParamsC), P(DogPointC), ip, P(ip)]
+    lib.bs_dog_debug_dog.argtypes = [vp, ull, P(ll), P(ll), P(DogParamsC), ip, vp, C.c_char_p]
     _lib = lib
     return lib
 
@@ -471,6 +472,19 @@ class Context:
                 break
             max_points = n.value
         return [(tuple(buf[i].loc), buf[i].value, tuple(buf[i].voxel), bool(buf[i].is_max)) for i in range(n.value)]
+
+    def dog_debug_dog(self, handle: int, interval_min_xyz, interval_size_xyz, sigma=1.8, min_intensity=0.0,
+                      max_intensity=65535.0, blur=0):
+        """The DoG box dog_detect's extremum stage reads for this interval (include/bsgpu.h bs_dog_debug_dog): float32
+        [sz + 2, sy + 2, sx + 2] over [min - 1, min + size + 1) per axis, and the blur instantiation launched.
+        blur: 0 production choice, 1 generic, 2 window R 6, 3 window R 12."""
+        p = DogParamsC(float(sigma), 0.0, float(min_intensity), float(max_intensity), 1, 0, 1, 0)
+        mn = (C.c_longlong * 3)(*[int(v) for v in interval_min_xyz])
+        sz = (C.c_longlong * 3)(*[int(v) for v in interval_size_xyz])
+        out = np.empty([int(v) + 2 for v in interval_size_xyz][::-1], dtype=np.float32)
+        info = C.create_string_buffer(128)
+        self._check(self.lib.bs_dog_debug_dog(self.h, handle, mn, sz, C.byref(p), int(blur), out.ctypes.data, info))
+        return out, info.value.decode()
 
     @staticmethod
     def fuse_params(fusion_type=FUSE_AVG_BLEND, interpolation=1, out_dtype=DTYPE_F32, blend_lut_n=0,

@@ -303,6 +303,15 @@ void bs_dog_default_params(bs_dog_params* p);
 int bs_dog_detect(bs_ctx* ctx, unsigned long long vol_handle, const long long interval_min[3], const long long interval_size[3],
                   const bs_dog_params* params, bs_dog_point* out, int max_points, int* n_found);
 
+/* diagnostic: the DoG (G_sa * I' - G_sb * I') / (k - 1) that bs_dog_detect's extremum stage reads for this interval,
+ * i.e. over [interval_min - 1, interval_min + interval_size + 1) per axis (mirror-double extension outside the image),
+ * computed by the same load / blur launches.  out: host float32, (size + 2) per axis, x fastest.
+ * blur: 0 = the production choice, 1 = generic k_dog_blur, 2 = window R 6, 3 = window R 12
+ * (BS_ERR_ARG when the kernel radius does not fit the forced window).
+ * info (may be NULL): the blur instantiation launched and the radii, e.g. "k_dog_blur_x<12> ra=6 rb=7". */
+int bs_dog_debug_dog(bs_ctx* ctx, unsigned long long vol_handle, const long long interval_min[3],
+                     const long long interval_size[3], const bs_dog_params* params, int blur, float* out, char info[128]);
+
 #ifdef __cplusplus
 }
 #endif

@@ -504,3 +504,25 @@ JF(jdoubleArray, dogDetect)(JNIEnv* env, jclass, jlong ctx, jlong handle, jlongA
     env->SetDoubleArrayRegion(arr, 0, n * 8, out.data());
     return arr;
 }
+
+// diagnostic: the DoG box the extremum stage reads (include/bsgpu.h bs_dog_debug_dog); out: float[(sx + 2)(sy + 2)(sz + 2)],
+// x fastest; blur 0 production, 1 generic, 2 window R 6, 3 window R 12; returns the blur instantiation launched
+JF(jstring, dogDebugDog)(JNIEnv* env, jclass, jlong ctx, jlong handle, jlongArray intervalMin, jlongArray intervalSize,
+                         jdoubleArray dparams /* sigma, minI, maxI */, jint blur, jobject out) {
+    long long mn[3], sz[3];
+    get3(env, intervalMin, mn);
+    get3(env, intervalSize, sz);
+    jdouble dp[3];
+    env->GetDoubleArrayRegion(dparams, 0, 3, dp);
+    bs_dog_params p;
+    bs_dog_default_params(&p);
+    p.sigma = dp[0]; p.min_intensity = dp[1]; p.max_intensity = dp[2];
+    char info[128] = "";
+    int rc;
+    {
+        Pinned o(env, out);
+        rc = bs_dog_debug_dog(C(ctx), (unsigned long long)handle, mn, sz, &p, blur, static_cast<float*>(o.p), info);
+    }
+    if (failed(env, ctx, rc)) return nullptr;
+    return env->NewStringUTF(info);
+}

@@ -83,4 +83,7 @@ public final class BsNative
 
 	/** n x {locX, locY, locZ, value, voxelX, voxelY, voxelZ, isMax}; dparams {sigma, threshold, minI, maxI}; iparams {findMax, findMin, localization} */
 	public static native double[] dogDetect( long ctx, long handle, long[] intervalMin, long[] intervalSize, double[] dparams, int[] iparams );
+	/** the DoG box the extremum stage reads, [min - 1, min + size + 1) per axis: out float[(sx+2)(sy+2)(sz+2)], x fastest;
+	 *  dparams {sigma, minI, maxI}; blur 0 production, 1 generic, 2 window R 6, 3 window R 12; returns the blur launched */
+	public static native String dogDebugDog( long ctx, long handle, long[] intervalMin, long[] intervalSize, double[] dparams, int blur, Object out );
 }

@@ -183,6 +183,46 @@ def content_weights(img, sigma1=DEFAULT_CONTENT_SIGMA1, sigma2=DEFAULT_CONTENT_S
     return gauss3((d * d).astype(np.float32), sigma2)
 
 
+def _mirror_single_index(i, n):
+    """Views.extendMirrorSingle: ... c b | a b c ... (the border pixel is not repeated); a length-1 axis is constant."""
+    if n == 1:
+        return np.zeros_like(i)
+    period = 2 * n - 2
+    i = np.mod(i, period)
+    return np.where(i < n, i, period - i)
+
+
+def _gauss3_f64(vol, k, drop_outer_tap_axis=None):
+    """Separable correlation with the taps ``k`` in float64, mirror-single border, x then y then z."""
+    r = len(k) // 2
+    out = np.asarray(vol, dtype=np.float64)
+    for d in (0, 1, 2):             # x, y, z
+        ax = 2 - d
+        kk = np.array(k, dtype=np.float64)
+        if d == drop_outer_tap_axis:
+            kk[0] = kk[-1] = 0.0
+        n = out.shape[ax]
+        ext = np.take(out, _mirror_single_index(np.arange(-r, n + r), n), axis=ax)
+        acc = np.zeros(out.shape)
+        sl = [slice(None)] * 3
+        for t, kt in enumerate(kk):
+            sl[ax] = slice(t, t + n)
+            acc += kt * ext[tuple(sl)]
+        out = acc
+    return out
+
+
+def content_weights_reference(img, sigma1=DEFAULT_CONTENT_SIGMA1, sigma2=DEFAULT_CONTENT_SIGMA2, drop_outer_tap_axis=None):
+    """Float64 reference of content_weights: the float32 taps of gauss_kernel, mirror-single borders, no intermediate
+    rounding.  Returns (c, f, G_s1 f, d = f - G_s1 f), float64 [z, y, x]; f, G_s1 f and d set the error bar of a float32
+    implementation.  ``drop_outer_tap_axis`` (0 = x, 1 = y, 2 = z) zeroes the outermost taps of both kernels on that axis:
+    a wrong reference, used to show that a test's bar can tell it apart."""
+    f = np.asarray(img, dtype=np.float32).astype(np.float64)
+    g1 = _gauss3_f64(f, gauss_kernel(sigma1), drop_outer_tap_axis)
+    d = f - g1
+    return _gauss3_f64(d * d, gauss_kernel(sigma2), drop_outer_tap_axis), f, g1, d
+
+
 @dataclass
 class View:
     img: np.ndarray            # [z, y, x] uint16 or float32

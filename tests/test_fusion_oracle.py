@@ -172,3 +172,20 @@ def test_mask_block_semantics():
     f = fo.mask_block(geom, (0, 0, 0), (48, 16, 8), (0.0, 0.0, 0.0), "float32")
     assert f.dtype == np.float32 and np.array_equal(f > 0, m > 0) and f.max() == 1.0
     assert not fo.mask_block([], (0, 0, 0), (4, 4, 4)).any()
+
+
+def test_content_weights_reference_agrees_with_the_float32_oracle():
+    """The float64 content weights equal the float32 pipeline within the rounding of its stored intermediates, also on
+    axes of length 1 (mirror-single of a single sample is that sample) and on float32 input with negative values."""
+    rng = np.random.default_rng(0)
+    u = 2.0 ** -24
+    for shape in [(12, 14, 16), (1, 14, 16), (12, 1, 16), (12, 14, 1), (9, 7, 33)]:
+        vol = (rng.normal(0, 50, shape) + 20).astype(np.float32)
+        for s1, s2 in ((2.0, 4.0), (1.0, 2.0)):
+            c, f, g1, d = fo.content_weights_reference(vol, s1, s2)
+            assert np.array_equal(f, vol.astype(np.float64))
+            bar = u * (c + fo._gauss3_f64(2 * np.abs(d) * (np.abs(f) + 2 * np.abs(g1)), fo.gauss_kernel(s2)))
+            assert np.all(np.abs(fo.content_weights(vol, s1, s2) - c) <= 2 * bar), (shape, s1, s2)
+    # a single sample along x: the blur along x is the identity
+    line = rng.normal(0, 5, (6, 7, 1)).astype(np.float32)
+    assert np.allclose(fo._gauss3_f64(line, fo.gauss_kernel(3.0)), fo._gauss3_f64(line[:, :, 0:1], fo.gauss_kernel(3.0)))
