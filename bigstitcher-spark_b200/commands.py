@@ -5,6 +5,7 @@
   stitching               J/SparkPairwiseStitching.java:110-392
   create_fusion_container J/CreateFusionContainer.java:122-519   (N5 or OME-ZARR, all channels / timepoints, pyramid)
   affine_fusion           J/SparkAffineFusion.java:179-800       (s0 + multi-resolution pyramid)
+  detect_interestpoints   J/SparkInterestPointDetection.java:173-964 (block-wise DoG, interestpoints.n5 + the XML)
 
 No argument parsing here (the picocli layer is out of scope); keyword names follow the CLI flags.
 """
@@ -12,6 +13,8 @@ from __future__ import annotations
 
 import math
 import os
+import shutil
+from decimal import Decimal
 
 import numpy as np
 
@@ -488,3 +491,212 @@ def _fuse_chunk(ctx, chunk, bb_min, vdims, vregs, views, params, np_dt):
         hi = np.maximum(hi, wmin + np.asarray(size) - 1)
     vids = [v for v in bf.find_overlapping_views(vdims, vregs, lo.astype(np.int64), hi.astype(np.int64), sorted(views))]
     return ctx.fuse_blocks([views[v] for v in vids], mins, sizes, params)
+
+
+# --------------------------------------------------------------------------------------------- detect-interestpoints
+IP_POWERS = (1, 2, 4, 8, 16, 32, 64, 128)        # J/SparkInterestPointDetection.java:1005
+IP_N5_BLOCK_LENGTH = 300000                      # InterestPointsN5.defaultBlockSize (recalled, PARITY_GAPS)
+IP_N5_GROUP_ATTRIBUTES = {"pointcloud": "1.0.0", "type": "list", "list version": "1.0.0"}   # recalled, PARITY_GAPS
+
+
+def java_double(v) -> str:
+    """Double.toString: shortest round-trip digits, plain in [1e-3, 1e7), else computerized scientific ("1.0E-4")."""
+    v = float(v)
+    if math.isnan(v):
+        return "NaN"
+    if math.isinf(v):
+        return "Infinity" if v > 0 else "-Infinity"
+    if v == 0.0:
+        return "-0.0" if math.copysign(1.0, v) < 0 else "0.0"
+    if 1e-3 <= abs(v) < 1e7:
+        return repr(v)
+    sign, digits, exp = Decimal(repr(abs(v))).as_tuple()
+    digits = list(digits)
+    while len(digits) > 1 and digits[-1] == 0:
+        digits.pop()
+        exp += 1
+    e = len(digits) - 1 + exp
+    frac = "".join(str(d) for d in digits[1:]) or "0"
+    return f"{'-' if v < 0 else ''}{digits[0]}.{frac}E{e}"
+
+
+def _java(v) -> str:
+    if isinstance(v, bool):
+        return "true" if v else "false"
+    if isinstance(v, int):
+        return str(v)
+    return java_double(v)
+
+
+def interestpoint_params(sigma, threshold, overlapping_only, find_min, find_max, downsample_xy, downsample_z,
+                         min_intensity, max_intensity) -> str:
+    """The params attribute of <ViewInterestPointsFile> (J/SparkInterestPointDetection.java:898-899)."""
+    return (f"DOG (Spark) s={_java(float(sigma))} t={_java(float(threshold))} overlappingOnly={_java(bool(overlapping_only))} "
+            f"min={_java(bool(find_min))} max={_java(bool(find_max))} downsampleXY={int(downsample_xy)} "
+            f"downsampleZ={int(downsample_z)} minIntensity={_java(float(min_intensity))} "
+            f"maxIntensity={_java(float(max_intensity))}")
+
+
+def interestpoint_level(factors, downsample_xyz):
+    """openAndDownsample's level choice (J/SparkInterestPointDetection.java:1026-1044): the LAST mipmap level whose
+    rounded factors are all <= the requested ones and powers of two <= 128; returns (level, remaining factors) with
+    remaining = requested / level factor per axis.  No requested downsampling reads level 0."""
+    ds = [int(v) for v in downsample_xyz]
+    if all(v == 1 for v in ds):
+        return 0, (1, 1, 1)
+    best = 0
+    for lvl, f in enumerate(factors):
+        r = [int(math.floor(float(v) + 0.5)) for v in f]       # Math.round
+        if all(r[d] <= ds[d] and r[d] in IP_POWERS for d in range(3)):
+            best = lvl
+    r = [int(math.floor(float(v) + 0.5)) for v in factors[best]]
+    return best, tuple(ds[d] // r[d] for d in range(3))
+
+
+def interestpoint_transform(mipmap_transform, remaining_xyz):
+    """Downsampled pixel -> full-resolution view pixel: mipmapTransform[level] o scale(remaining), no extra shift
+    (J/SparkInterestPointDetection.java:1067-1081, applied by correctForDownsampling at :606-609)."""
+    M = np.vstack([np.asarray(mipmap_transform, dtype=np.float64).reshape(3, 4), [0, 0, 0, 1]])
+    S = np.diag([float(v) for v in remaining_xyz] + [1.0])
+    return (M @ S)[:3]
+
+
+def interestpoint_blocks(dims_xyz, block_size):
+    """The DoG intervals of one view: the reference's Grid.create blocks in job order, each passed to bs_dog_detect
+    as it is, but shrunk by one voxel on faces that lie on the view border.  The reference expands every block by one
+    voxel inside the image and computeDoG tests only the interior of its interval (J/SparkInterestPointDetection.java:
+    397-424, PARITY_GAPS), so every voxel but the view's outermost layer is tested exactly once."""
+    out = []
+    for off, size, _ in bf.grid_create([int(v) for v in dims_xyz], [int(v) for v in block_size]):
+        lo = [max(off[d], 1) for d in range(3)]
+        hi = [min(off[d] + size[d], int(dims_xyz[d]) - 1) for d in range(3)]
+        if all(hi[d] > lo[d] for d in range(3)):
+            out.append((tuple(lo), tuple(hi[d] - lo[d] for d in range(3))))
+    return out
+
+
+def _check_device_memory(ctx, nbytes, what):
+    import torch
+    free, _ = torch.cuda.mem_get_info(ctx.device)
+    if nbytes > free:
+        raise MemoryError(f"detect-interestpoints: {what} needs {nbytes / 2**30:.2f} GiB on device {ctx.device}, "
+                          f"{free / 2**30:.2f} GiB are free; use a larger --downsampleXY / --downsampleZ")
+
+
+def _detect_view(ctx, src, view, level, remaining, mt, sigma, threshold, min_intensity, max_intensity, find_max,
+                 find_min, localization, block_size, median_filter, need_intensities):
+    ds_name = bn5.bdv_dataset(view[1], view[0], level)
+    a = src.dataset_attributes(ds_name)
+    ldims = [int(v) for v in a["dimensions"]]
+    vox = int(np.prod(ldims))
+    dvox = int(np.prod([max(ldims[d] // remaining[d], 0) for d in range(3)]))
+    blk = int(np.prod([min(int(block_size[d]), ldims[d]) + 64 for d in range(3)]))
+    _check_device_memory(ctx, vox * np.dtype(bn5._DTYPES[a["dataType"]]).itemsize + 4 * (2 * dvox + 4 * blk),
+                         f"view {view} (level s{level}, {ldims[0]}x{ldims[1]}x{ldims[2]})")
+    handles = []
+    try:
+        h = ctx.volume_upload(src.read_volume(ds_name))
+        handles.append(h)
+        img = h
+        if any(v > 1 for v in remaining):
+            img = ctx.downsample_float(h, remaining)
+            handles.append(img)
+            ctx.volume_free(h)
+            handles.remove(h)
+        det = img
+        if median_filter:
+            det = ctx.median_divide(img, int(median_filter))
+            handles.append(det)
+        dims, _ = ctx.volume_info(det)
+        locs = []
+        for mn, sz in interestpoint_blocks(dims, block_size):
+            pts = ctx.dog_detect(det, mn, sz, sigma=sigma, threshold=threshold, min_intensity=min_intensity,
+                                 max_intensity=max_intensity, find_max=find_max, find_min=find_min,
+                                 localization=localization)
+            locs.extend(p[0] for p in pts)
+        loc = np.array(locs, dtype=np.float64).reshape(-1, 3)
+        inten = ctx.sample_nlinear(img, loc) if need_intensities else None
+    finally:
+        for hh in handles:
+            ctx.volume_free(hh)
+    T = interestpoint_transform(mt, remaining)
+    return loc @ T[:, :3].T + T[:, 3], inten
+
+
+def detect_interestpoints(xml_path, ctx: Context, label, sigma, threshold, min_intensity, max_intensity, type="MAX",
+                          localization="QUADRATIC", downsample_xy=2, downsample_z=1, block_size=(512, 512, 128),
+                          median_filter=None, store_intensities=False, max_spots=0, view_selection=None, dry_run=False,
+                          shard=(0, 1), allgather=None, overlapping_only=False, only_compare_overlap_tiles=False,
+                          max_spots_per_overlap=False, prefetch=False, keep_temporary_n5=False):
+    """`./detect-interestpoints -x dataset.xml -l beads -s 1.8 -t 0.008 -i0 0 -i1 2048 [--type MAX|MIN|BOTH]
+    [--localization NONE|QUADRATIC] [-dsxy 2] [-dsz 1] [--blockSize 512,512,128] [--medianFilter r]
+    [--storeIntensities] [--maxSpots N]`: per selected view, read the mipmap level openAndDownsample picks, finish the
+    downsampling on the device in float (bs_downsample_float), optionally divide every z-slice by its median
+    (bs_median_divide), run bs_dog_detect over the reference's block grid, map the points to full-resolution pixels and
+    write them to `interestpoints.n5` next to the XML plus a <ViewInterestPointsFile> per view (also views without
+    points).  Returns {(tp, setup): (loc (n, 3) float64, intensities float32 (n,) or None)}.
+
+    ``prefetch`` and ``keep_temporary_n5`` tune the reference's Spark execution and are accepted without effect.
+    ``overlapping_only``, ``only_compare_overlap_tiles`` and ``max_spots_per_overlap`` are not implemented.
+
+    Multi-GPU: rank r of w (``shard``) takes views[r::w]; ``allgather(obj) -> [obj of every rank]`` merges the results
+    and rank 0 writes."""
+    for flag, on in (("--overlappingOnly", overlapping_only), ("--onlyCompareOverlapTiles", only_compare_overlap_tiles),
+                     ("--maxSpotsPerOverlap", max_spots_per_overlap)):
+        if on:
+            raise NotImplementedError(f"detect-interestpoints {flag} is not implemented")
+    type = type.upper()
+    if type not in ("MIN", "MAX", "BOTH") or localization.upper() not in ("NONE", "QUADRATIC"):
+        raise ValueError(f"--type {type} / --localization {localization}")
+    find_min, find_max = type in ("MIN", "BOTH"), type in ("MAX", "BOTH")
+    for v in (downsample_xy, downsample_z):
+        if int(v) not in IP_POWERS:
+            raise ValueError(f"downsampling {v} is not a power of two <= 128")
+    if median_filter is not None and not 0 < int(median_filter) <= native.MEDIAN_MAX_RADIUS:
+        raise ValueError(f"--medianFilter {median_filter} outside [1, {native.MEDIAN_MAX_RADIUS}]")
+    data = SpimData2.load(xml_path)
+    fmt, n5_path = data.image_loader()
+    if fmt != "bdv.n5":
+        raise NotImplementedError(f"ImageLoader format {fmt}")
+    src = bn5.N5Store(n5_path)
+    views = data.select_views(**view_selection) if view_selection else data.view_ids()
+    rank, world = shard
+    results = {}
+    for v in views[rank::world]:
+        factors, mts = _mipmap_info(src, v[1])
+        level, remaining = interestpoint_level(factors, (downsample_xy, downsample_xy, downsample_z))
+        loc, inten = _detect_view(ctx, src, v, level, remaining, mts[level], sigma, threshold, min_intensity, max_intensity,
+                                  find_max, find_min, localization.upper() == "QUADRATIC", block_size, median_filter,
+                                  store_intensities or max_spots > 0)
+        if max_spots > 0 and len(loc) > max_spots:
+            order = sorted(range(len(loc)), key=lambda i: -float(inten[i]))[:max_spots]   # stable, descending
+            loc, inten = loc[order], inten[order]
+        results[v] = (loc, inten if store_intensities else None)
+    if world > 1:
+        merged = {}
+        for part in allgather(results):
+            merged.update(part)
+        results = {v: merged[v] for v in views if v in merged}
+        if rank != 0:
+            return results
+    if dry_run:
+        return results
+    base = os.path.join(os.path.dirname(os.path.abspath(xml_path)), data.root.findtext("BasePath") or ".")
+    store = bn5.N5Store(os.path.join(base, "interestpoints.n5"), create=True)
+    paths = {}
+    for (tp, setup), (loc, inten) in sorted(results.items()):
+        group = f"tpId_{tp}_viewSetupId_{setup}/{label}"
+        shutil.rmtree(os.path.join(store.root, group), ignore_errors=True)     # re-running a label replaces it
+        store.set_attributes(group + "/interestpoints", IP_N5_GROUP_ATTRIBUTES)
+        store.write_list(group + "/interestpoints/id", np.arange(len(loc), dtype=np.uint64).reshape(-1, 1),
+                         IP_N5_BLOCK_LENGTH, "zstd")
+        store.write_list(group + "/interestpoints/loc", loc.astype(np.float64), IP_N5_BLOCK_LENGTH, "zstd")
+        if inten is not None:
+            store.write_list(group + "/intensities", inten.astype(np.float32).reshape(-1, 1), IP_N5_BLOCK_LENGTH,
+                             "zstd")
+        paths[(tp, setup)] = group
+    data.set_interest_points(label, interestpoint_params(sigma, threshold, overlapping_only, find_min, find_max,
+                                                         downsample_xy, downsample_z, min_intensity, max_intensity),
+                             paths)
+    data.save(xml_path)
+    return results

@@ -56,7 +56,7 @@ int bs_volume_acquire(bs_ctx* ctx, bs_volume& v) {
 
 extern "C" {
 
-int bs_version(void) { return 105; }
+int bs_version(void) { return 106; }
 
 int bs_init(bs_ctx** out, int device, void* stream) {
     if (!out) return bs_set_error(nullptr, BS_ERR_ARG, "bs_init: out is NULL");

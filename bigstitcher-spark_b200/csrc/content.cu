@@ -286,28 +286,28 @@ template <> __device__ __forceinline__ unsigned char avg2<unsigned char>(unsigne
     return (unsigned char)(((unsigned)a + (unsigned)b + 1u) >> 1);
 }
 
-template <typename T>
-__global__ void k_downsample(const T* __restrict__ in, T* __restrict__ out, int dx, int dy, int dz, int ox, int oy,
+template <typename T, typename Tout = T>
+__global__ void k_downsample(const T* __restrict__ in, Tout* __restrict__ out, int dx, int dy, int dz, int ox, int oy,
                              int oz, int fx, int fy, int fz) {
     const long long n = (long long)ox * oy * oz;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
         const int x = (int)(i % ox);
         const long long r = i / ox;
         const int y = (int)(r % oy), z = (int)(r / oy);
-        T vz[2];
+        Tout vz[2];
 #pragma unroll
         for (int kz = 0; kz < 2; ++kz) {
             if (kz >= fz) { vz[kz] = vz[0]; continue; }
-            T vy[2];
+            Tout vy[2];
 #pragma unroll
             for (int ky = 0; ky < 2; ++ky) {
                 if (ky >= fy) { vy[ky] = vy[0]; continue; }
                 const T* p = in + ((size_t)(z * fz + kz) * dy + (y * fy + ky)) * dx + (size_t)x * fx;
-                vy[ky] = fx == 2 ? avg2<T>(p[0], p[1]) : p[0];
+                vy[ky] = fx == 2 ? avg2<Tout>((Tout)p[0], (Tout)p[1]) : (Tout)p[0];
             }
-            vz[kz] = fy == 2 ? avg2<T>(vy[0], vy[1]) : vy[0];
+            vz[kz] = fy == 2 ? avg2<Tout>(vy[0], vy[1]) : vy[0];
         }
-        out[i] = fz == 2 ? avg2<T>(vz[0], vz[1]) : vz[0];
+        out[i] = fz == 2 ? avg2<Tout>(vz[0], vz[1]) : vz[0];
     }
 }
 
@@ -349,6 +349,100 @@ extern "C" int bs_downsample(bs_ctx* ctx, unsigned long long vol_handle, const i
         cudaFree(v.dev);
         return bs_set_error(ctx, BS_ERR_CUDA, "bs_downsample: %s", cudaGetErrorString(e));
     }
+    *out_handle = ctx->next_handle++;
+    ctx->vols[*out_handle] = v;
+    return BS_OK;
+}
+
+// --------------------------------------------------------------------------------------------------------------------
+// Interest-point detection input (J/SparkInterestPointDetection.java:1085-1095): the remaining downsampling after the
+// mipmap level is a chain of LazyDownsample2x steps to FloatType -- every x halving, then every y, then every z -- each
+// the float pair average 0.5f * (a + b) of k_downsample with floor(d / 2) output dims.  One axis per launch, because
+// the order of the roundings is part of the result.
+static int ds_float_step(bs_ctx* ctx, const void* in, int dtype, float* out, const long long di[3], const long long dout[3],
+                         const int f[3]) {
+    const long long n = dout[0] * dout[1] * dout[2];
+    const int blocks = (int)std::min<long long>((n + 255) / 256, (long long)ctx->sm_count * 16);
+    const int a[9] = {(int)di[0], (int)di[1], (int)di[2], (int)dout[0], (int)dout[1], (int)dout[2], f[0], f[1], f[2]};
+    bs_launch_scope sc(ctx, "downsample");
+    if (dtype == BS_DTYPE_U16)
+        k_downsample<unsigned short, float><<<blocks, 256, 0, ctx->stream>>>((const unsigned short*)in, out, a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7], a[8]);
+    else if (dtype == BS_DTYPE_F32)
+        k_downsample<float, float><<<blocks, 256, 0, ctx->stream>>>((const float*)in, out, a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7], a[8]);
+    else
+        k_downsample<unsigned char, float><<<blocks, 256, 0, ctx->stream>>>((const unsigned char*)in, out, a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7], a[8]);
+    return cudaGetLastError() == cudaSuccess ? BS_OK : BS_ERR_CUDA;
+}
+
+extern "C" int bs_downsample_float(bs_ctx* ctx, unsigned long long vol_handle, const int factors[3],
+                                   unsigned long long* out_handle) {
+    if (!ctx) return BS_ERR_ARG;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    if (!factors || !out_handle) return bs_set_error(ctx, BS_ERR_ARG, "bs_downsample_float: NULL argument");
+    auto it = ctx->vols.find(vol_handle);
+    if (it == ctx->vols.end()) return bs_set_error(ctx, BS_ERR_ARG, "bs_downsample_float: unknown handle %llu", vol_handle);
+    const bs_volume src = it->second;
+    std::vector<int> axes;                       // one entry per 2x step, in the reference's order
+    long long dims[3] = {src.dims[0], src.dims[1], src.dims[2]};
+    for (int d = 0; d < 3; ++d) {
+        const int f = factors[d];
+        if (f < 1 || f > 128 || (f & (f - 1)))
+            return bs_set_error(ctx, BS_ERR_ARG, "bs_downsample_float: factor %d of axis %d is not a power of two <= 128", f, d);
+        for (int g = f; g > 1; g >>= 1) {
+            axes.push_back(d);
+            dims[d] /= 2;
+        }
+        if (dims[d] < 1) return bs_set_error(ctx, BS_ERR_ARG, "bs_downsample_float: dimension %d too small", d);
+    }
+    { int rc0 = bs_volume_acquire(ctx, it->second); if (rc0) return rc0; }
+    BS_CUDA(ctx, cudaSetDevice(ctx->device));
+    if (axes.empty()) axes.push_back(-1);        // no halving: a plain conversion to float
+    const void* cur = src.dev;
+    int cur_dtype = src.dtype;
+    long long cd[3] = {src.dims[0], src.dims[1], src.dims[2]};
+    float* prev = nullptr;                       // intermediate owned here (freed once the next step has run)
+    int rc = BS_OK;
+    for (int ax : axes) {
+        int f[3] = {1, 1, 1};
+        long long nd[3] = {cd[0], cd[1], cd[2]};
+        if (ax >= 0) {
+            f[ax] = 2;
+            nd[ax] /= 2;
+        }
+        float* next = nullptr;
+        cudaError_t e = cudaMalloc(&next, sizeof(float) * (size_t)(nd[0] * nd[1] * nd[2]));
+        if (e != cudaSuccess) {
+            rc = bs_set_error(ctx, BS_ERR_NOMEM, "bs_downsample_float: cudaMalloc: %s", cudaGetErrorString(e));
+            break;
+        }
+        if (ds_float_step(ctx, cur, cur_dtype, next, cd, nd, f) != BS_OK) {
+            rc = bs_set_error(ctx, BS_ERR_CUDA, "bs_downsample_float: launch failed");
+            cudaFree(next);
+            break;
+        }
+        if (prev) {                              // the step just queued reads it
+            cudaStreamSynchronize(ctx->stream);
+            cudaFree(prev);
+        }
+        prev = next;
+        cur = next;
+        cur_dtype = BS_DTYPE_F32;
+        for (int d = 0; d < 3; ++d) cd[d] = nd[d];
+    }
+    if (!rc) {
+        cudaError_t e = cudaStreamSynchronize(ctx->stream);
+        if (e != cudaSuccess) rc = bs_set_error(ctx, BS_ERR_CUDA, "bs_downsample_float: %s", cudaGetErrorString(e));
+    }
+    if (rc) {
+        cudaStreamSynchronize(ctx->stream);
+        if (prev) cudaFree(prev);
+        return rc;
+    }
+    bs_volume v;
+    v.dev = prev;
+    for (int d = 0; d < 3; ++d) v.dims[d] = cd[d];
+    v.dtype = BS_DTYPE_F32;
+    v.owned = true;
     *out_handle = ctx->next_handle++;
     ctx->vols[*out_handle] = v;
     return BS_OK;

@@ -38,7 +38,7 @@ def bs_attr_get(attrs: dict, key, default=None):
         return nested[key]
     return attrs.get(BS_KEY + "/" + key, default)
 
-_DTYPES = {"uint8": np.uint8, "uint16": np.uint16, "uint32": np.uint32, "int16": np.int16,
+_DTYPES = {"uint8": np.uint8, "uint16": np.uint16, "uint32": np.uint32, "uint64": np.uint64, "int16": np.int16,
            "float32": np.float32, "float64": np.float64}
 
 
@@ -211,6 +211,33 @@ class N5Store:
                         continue
                     blk = volume[kz * bs[2]:(kz + 1) * bs[2], ky * bs[1]:(ky + 1) * bs[1], kx * bs[0]:(kx + 1) * bs[0]]
                     self.write_block(path, g, blk)
+
+    def write_list(self, path, values: np.ndarray, block_length, compression="raw"):
+        """A list of n k-vectors as the 2-D dataset {k, n} (k fastest) in blocks {k, block_length}, the layout of
+        InterestPointsN5 and the --storeIntensities dataset; an empty list is the 1-D dataset {0}, block {1}, with
+        no block files (J/SparkInterestPointDetection.java:917-925)."""
+        values = np.asarray(values)
+        if values.shape[0] == 0:
+            self.create_dataset(path, [0], [1], values.dtype, compression)
+            return
+        k = values.shape[1]
+        self.create_dataset(path, [k, values.shape[0]], [k, block_length], values.dtype, compression)
+        for j, s0 in enumerate(range(0, values.shape[0], block_length)):
+            self.write_block(path, (0, j), np.ascontiguousarray(values[s0:s0 + block_length]))
+
+    def read_list(self, path) -> np.ndarray:
+        """The (n, k) array of a dataset written by write_list ((0, 0) when empty)."""
+        a = self.dataset_attributes(path)
+        dims, bs = a["dimensions"], a["blockSize"]
+        dt = _DTYPES[a["dataType"]]
+        if len(dims) == 1:
+            return np.zeros((0, 0), dtype=dt)
+        out = np.zeros((dims[1], dims[0]), dtype=dt)
+        for j in range(-(-dims[1] // bs[1])):
+            b = self.read_block(path, (0, j))
+            if b is not None:
+                out[j * bs[1]:j * bs[1] + b.shape[0]] = b
+        return out
 
     def write_volume(self, path, volume: np.ndarray, block_size, compression="raw"):
         self.create_dataset(path, volume.shape[::-1], block_size, volume.dtype, compression)

@@ -108,7 +108,11 @@ SYMBOLS = [
     "bs_content_weights", "bs_volume_info", "bs_volume_download", "bs_volume_devptr", "bs_downsample", "bs_fuse_block", "bs_fuse_blocks",
     "bs_fuse_block_to_volume", "bs_fuse_accumulate", "bs_fuse_finish", "bs_mask_blocks", "bs_dog_default_params", "bs_dog_detect",
     "bs_dog_debug_dog", "bs_comm_unique_id", "bs_comm_init", "bs_comm_destroy", "bs_fuse_allreduce",
+    "bs_downsample_float", "bs_median_divide", "bs_sample_nlinear",
 ]
+
+#: largest --medianFilter radius bs_median_divide accepts (BS_MEDIAN_MAX_RADIUS in include/bsgpu.h)
+MEDIAN_MAX_RADIUS = 32
 
 
 def load_library():
@@ -171,6 +175,9 @@ def load_library():
     lib.bs_dog_default_params.restype = None
     lib.bs_dog_detect.argtypes = [vp, ull, P(ll), P(ll), P(DogParamsC), P(DogPointC), ip, P(ip)]
     lib.bs_dog_debug_dog.argtypes = [vp, ull, P(ll), P(ll), P(DogParamsC), ip, vp, C.c_char_p]
+    lib.bs_downsample_float.argtypes = [vp, ull, P(ip), P(ull)]
+    lib.bs_median_divide.argtypes = [vp, ull, ip, P(ull)]
+    lib.bs_sample_nlinear.argtypes = [vp, ull, ip, P(dbl), vp]
     _lib = lib
     return lib
 
@@ -485,6 +492,30 @@ class Context:
         info = C.create_string_buffer(128)
         self._check(self.lib.bs_dog_debug_dog(self.h, handle, mn, sz, C.byref(p), int(blur), out.ctypes.data, info))
         return out, info.value.decode()
+
+    # -- detect-interestpoints helpers
+    def downsample_float(self, handle: int, factors_xyz) -> int:
+        """New float32 volume: the LazyDownsample2x chain (every x halving, then y, then z; 0.5f * (a + b), floor dims)
+        of a resident volume; ``factors_xyz`` are powers of two <= 128 (all 1: a float copy)."""
+        f = (C.c_int * 3)(*[int(v) for v in factors_xyz])
+        h = C.c_ulonglong()
+        self._check(self.lib.bs_downsample_float(self.h, handle, f, C.byref(h)))
+        return h.value
+
+    def median_divide(self, handle: int, radius: int) -> int:
+        """New float32 volume: every z-slice divided by its circular (ImageJ RankFilters) median of ``radius``, 0 where
+        the median is <= 0 (``--medianFilter``)."""
+        h = C.c_ulonglong()
+        self._check(self.lib.bs_median_divide(self.h, handle, int(radius), C.byref(h)))
+        return h.value
+
+    def sample_nlinear(self, handle: int, loc_xyz) -> np.ndarray:
+        """float32 n-linear samples (border extension) of a resident volume at (n, 3) pixel coordinates {x, y, z}."""
+        loc = np.ascontiguousarray(np.asarray(loc_xyz, dtype=np.float64).reshape(-1, 3))
+        out = np.empty(len(loc), dtype=np.float32)
+        self._check(self.lib.bs_sample_nlinear(self.h, handle, len(loc), loc.ctypes.data_as(C.POINTER(C.c_double)),
+                                               out.ctypes.data))
+        return out
 
     @staticmethod
     def fuse_params(fusion_type=FUSE_AVG_BLEND, interpolation=1, out_dtype=DTYPE_F32, blend_lut_n=0,

@@ -8,6 +8,8 @@ extensions) -- the fields the two hot paths consume and produce:
   * ImageLoader format="bdv.n5" path (J/SparkResaveN5.java:424-433)
   * <StitchingResults><PairwiseResult view_setup_a/b tp_a/b> shift (12 doubles), correlation, hash,
     overlap_boundingbox (6 doubles)                                   (J/SparkPairwiseStitching.java:284-301,328-390)
+  * <ViewInterestPoints><ViewInterestPointsFile timepoint setup label params>path of the label's group in
+    interestpoints.n5 (InterestPointTools.addInterestPoints, J/SparkInterestPointDetection.java:898-903)
 
 Host-side plumbing only.  Everything else in the file is preserved verbatim on save.
 """
@@ -277,6 +279,35 @@ class SpimData2:
             ET.SubElement(pr, "correlation").text = repr(float(res["r"]))
             ET.SubElement(pr, "hash").text = repr(float(res["hash"]))
             ET.SubElement(pr, "overlap_boundingbox").text = _fmt(list(res["bbox_min"]) + list(res["bbox_max"]))
+
+    # ------------------------------------------------------------------ interest points
+    def interest_points(self):
+        """{(tp, setup): {label: dict(params=..., path=...)}} of <ViewInterestPoints>."""
+        out = {}
+        vip = self.root.find("ViewInterestPoints")
+        if vip is None:
+            return out
+        for f in vip.findall("ViewInterestPointsFile"):
+            key = (int(f.get("timepoint")), int(f.get("setup")))
+            out.setdefault(key, {})[f.get("label")] = dict(params=f.get("params"), path=(f.text or "").strip())
+        return out
+
+    def set_interest_points(self, label, params, paths):
+        """Add or replace the ``label`` entry of every view in ``paths`` ({(tp, setup): path}); other labels are kept.
+        Entries stay ordered by (timepoint, setup, label)."""
+        vip = self.root.find("ViewInterestPoints")
+        if vip is None:
+            vip = ET.SubElement(self.root, "ViewInterestPoints")
+        entries = {}
+        for f in vip.findall("ViewInterestPointsFile"):
+            entries[(int(f.get("timepoint")), int(f.get("setup")), f.get("label"))] = f
+            vip.remove(f)
+        for (tp, setup), path in paths.items():
+            f = ET.Element("ViewInterestPointsFile", timepoint=str(tp), setup=str(setup), label=label, params=params)
+            f.text = path
+            entries[(int(tp), int(setup), label)] = f
+        for k in sorted(entries):
+            vip.append(entries[k])
 
 
 # ---------------------------------------------------------------------------------------------

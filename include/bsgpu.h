@@ -68,7 +68,7 @@ long long bs_launch_count(bs_ctx* ctx);
 /* per-kernel device timing with CUDA events on the context's stream.  Enabling inserts an
  * event pair around every kernel launch; bs_profile_get returns the accumulated milliseconds
  * and launch count for a kernel tag ("fft_x_r2c", "fft_y", "fft_z_xpower", "fft_y_inv",
- * "fft_x_c2r", "peaks", "pearson", "fuse", "content_gauss"). */
+ * "fft_x_c2r", "peaks", "pearson", "fuse", "content_gauss", "downsample", "median", "sample"). */
 int bs_profile_enable(bs_ctx* ctx, int on);
 int bs_profile_reset(bs_ctx* ctx);
 int bs_profile_get(bs_ctx* ctx, const char* tag, double* ms_total, long long* launches);
@@ -311,6 +311,31 @@ int bs_dog_detect(bs_ctx* ctx, unsigned long long vol_handle, const long long in
  * info (may be NULL): the blur instantiation launched and the radii, e.g. "k_dog_blur_x<12> ra=6 rb=7". */
 int bs_dog_debug_dog(bs_ctx* ctx, unsigned long long vol_handle, const long long interval_min[3],
                      const long long interval_size[3], const bs_dog_params* params, int blur, float* out, char info[128]);
+
+/* ---------------------------------------------------------------- detect-interestpoints helpers (ABI 106)
+ * The per-view steps SparkInterestPointDetection.call() runs around computeDoG (J/SparkInterestPointDetection.java:
+ * 532-604, openAndDownsample :991-1111).  Each returns a NEW resident volume (free it with bs_volume_free) or host
+ * values; the input volume is unchanged. */
+
+/* the remaining downsampling after the mipmap level (J/SparkInterestPointDetection.java:1085-1095): LazyDownsample2x to
+ * FloatType, first every x halving, then every y, then every z, each out[i] = 0.5f * (in[2i] + in[2i+1]) with
+ * floor(d / 2) output dims.  vol: U16, U8 or F32; factors: powers of two <= 128 per axis (all 1: a float copy);
+ * out: F32.  BS_ERR_ARG when an axis would shrink to 0. */
+int bs_downsample_float(bs_ctx* ctx, unsigned long long vol_handle, const int factors[3], unsigned long long* out_handle);
+
+/* --medianFilter r (LazyBackgroundSubtract, J/detection/LazyBackgroundSubtract.java:74-140, applied at
+ * J/SparkInterestPointDetection.java:532-547): per z-slice, m = the exact median of the values under ImageJ's circular
+ * RankFilters kernel of radius r (r2 = r*r + 1, row dy spans |dx| <= floor(sqrt(r2 - dy*dy + 1e-10)), an odd number of
+ * points) over the slice's mirror-double extension; out = v / m when m > 0, else 0, in float32.  vol: U16, U8 or F32;
+ * out: F32, same dims.  1 <= radius <= BS_MEDIAN_MAX_RADIUS, else BS_ERR_ARG.  Profile tag "median". */
+#define BS_MEDIAN_MAX_RADIUS 32
+int bs_median_divide(bs_ctx* ctx, unsigned long long vol_handle, int radius, unsigned long long* out_handle);
+
+/* --storeIntensities / --maxSpots (J/SparkInterestPointDetection.java:577-604): n-linear interpolation of the resident
+ * volume (converted to float) on its border extension at n host points loc_xyz[3n] (pixel coordinates {x,y,z}), like
+ * imglib2's NLinearInterpolator on FloatType: double weights, each corner term rounded to float and summed in float.
+ * out: n floats on the host.  Profile tag "sample". */
+int bs_sample_nlinear(bs_ctx* ctx, unsigned long long vol_handle, int n, const double* loc_xyz, float* out);
 
 #ifdef __cplusplus
 }

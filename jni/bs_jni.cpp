@@ -526,3 +526,30 @@ JF(jstring, dogDebugDog)(JNIEnv* env, jclass, jlong ctx, jlong handle, jlongArra
     if (failed(env, ctx, rc)) return nullptr;
     return env->NewStringUTF(info);
 }
+
+// ---------------------------------------------------------------------------------------- detect-interestpoints helpers
+JF(jlong, downsampleFloat)(JNIEnv* env, jclass, jlong ctx, jlong handle, jintArray factors) {
+    jint f[3];
+    env->GetIntArrayRegion(factors, 0, 3, f);
+    const int ff[3] = {f[0], f[1], f[2]};
+    unsigned long long h = 0;
+    return failed(env, ctx, bs_downsample_float(C(ctx), (unsigned long long)handle, ff, &h)) ? 0 : (jlong)h;
+}
+
+JF(jlong, medianDivide)(JNIEnv* env, jclass, jlong ctx, jlong handle, jint radius) {
+    unsigned long long h = 0;
+    return failed(env, ctx, bs_median_divide(C(ctx), (unsigned long long)handle, radius, &h)) ? 0 : (jlong)h;
+}
+
+// loc: double[3n] {x, y, z} per point; out: float[n] (or a direct ByteBuffer of n floats)
+JF(void, sampleNlinear)(JNIEnv* env, jclass, jlong ctx, jlong handle, jdoubleArray loc, jobject out) {
+    const jint n = env->GetArrayLength(loc) / 3;
+    std::vector<jdouble> l((size_t)n * 3);
+    env->GetDoubleArrayRegion(loc, 0, n * 3, l.data());
+    int rc;
+    {
+        Pinned o(env, out);
+        rc = bs_sample_nlinear(C(ctx), (unsigned long long)handle, n, l.data(), static_cast<float*>(o.p));
+    }
+    failed(env, ctx, rc);
+}

@@ -86,4 +86,11 @@ public final class BsNative
 	/** the DoG box the extremum stage reads, [min - 1, min + size + 1) per axis: out float[(sx+2)(sy+2)(sz+2)], x fastest;
 	 *  dparams {sigma, minI, maxI}; blur 0 production, 1 generic, 2 window R 6, 3 window R 12; returns the blur launched */
 	public static native String dogDebugDog( long ctx, long handle, long[] intervalMin, long[] intervalSize, double[] dparams, int blur, Object out );
+
+	/** detect-interestpoints: LazyDownsample2x chain to float32 (x halvings, then y, then z); factors powers of two <= 128 */
+	public static native long downsampleFloat( long ctx, long handle, int[] factors );
+	/** --medianFilter: every z-slice divided by its ImageJ circular median of the radius (0 where the median is <= 0) */
+	public static native long medianDivide( long ctx, long handle, int radius );
+	/** n-linear intensities (border extension) at loc = n x {x, y, z} into out: float[n] or a direct ByteBuffer */
+	public static native void sampleNlinear( long ctx, long handle, double[] loc, Object out );
 }
