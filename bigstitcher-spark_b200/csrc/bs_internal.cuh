@@ -1,5 +1,7 @@
 // Internal declarations shared by the translation units of libbsgpu.so (sm_90a only).
 #pragma once
+#include <cuda.h>
+#include <cudaTypedefs.h>
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
@@ -142,6 +144,8 @@ int bs_volume_acquire(bs_ctx* ctx, bs_volume& v);
 void bs_pcm_workspace_free(bs_ctx* ctx);
 // fuse_tma.cu
 void bs_fuse2_free(bs_ctx* ctx);
+// the driver's cuTensorMapEncodeTiled, or NULL when the driver does not provide it
+PFN_cuTensorMapEncodeTiled_v12000 bs_tensor_map_encoder();
 void bs_dog_free(bs_ctx* ctx);
 // comm.cu
 void bs_comm_free(bs_ctx* ctx);

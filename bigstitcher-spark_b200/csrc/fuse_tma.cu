@@ -982,9 +982,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) fuse_tma_kernel(const __grid_cons
 // ==========================================================================================
 // host side
 // ==========================================================================================
-namespace {
-
-PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
+PFN_cuTensorMapEncodeTiled_v12000 bs_tensor_map_encoder() {
     static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
     static bool tried = false;
     if (!tried) {
@@ -998,12 +996,14 @@ PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
     return fn;
 }
 
+namespace {
+
 // the two tensor maps of a uint16 volume (translation box, general box), copied once to device memory
 bool ensure_tmaps(bs_ctx* ctx, bs_volume& vol) {
     if (vol.tma_state != 0) return vol.tma_state > 0;
     vol.tma_state = -1;
     if (vol.dtype != BS_DTYPE_U16 || (vol.dims[0] & 7) != 0 || ((size_t)vol.dev & 15) != 0) return false;
-    auto enc = get_encode();
+    auto enc = bs_tensor_map_encoder();
     if (!enc) return false;
     alignas(64) CUtensorMap tm[2];
     const cuuint64_t gdim[3] = {(cuuint64_t)vol.dims[0], (cuuint64_t)vol.dims[1], (cuuint64_t)vol.dims[2]};

@@ -31,7 +31,7 @@
 #define PCM_KMAX 32
 #define PCM_SMEM_MAX 232448  // 227 KB opt-in limit per CTA on sm_90
 
-extern __shared__ __align__(16) float2 bs_sm[];
+extern __shared__ __align__(128) float2 bs_sm[];   // 128: tensor-map copies into it need 128-byte aligned targets
 
 // ------------------------------------------------------------------------------------------
 // x pass, real -> complex
@@ -793,16 +793,17 @@ __global__ void __launch_bounds__(PCM_THREADS, 2) k_fft_xpower_pipe(const __grid
 }
 
 // ------------------------------------------------------------------------------------------
-// Strided passes of the static 540-point plan (540 = 20 x 27, RegFft2): tiles of 540 rows x TC columns, data in
-// registers from the global load to the global store, one shared-memory exchange and one block barrier per
-// transform.  Persistent CTAs; the next tile's loads go out into the stage-1 registers as soon as the current
-// tile's stage 1 has written them to the exchange buffer, so they are in flight under stage 2 and the stores (a
+// Strided passes of the static 540-point plan (540 = 20 x 27, RegFft2): tiles of 540 rows x TC columns, one
+// shared-memory exchange and one block barrier per transform.  Persistent CTAs.  The y pass keeps the data in
+// registers from the global load to the global store; the next tile's loads go out into the stage-1 registers as
+// soon as the current tile's stage 1 has written them to the exchange buffer, so they are in flight under stage 2
+// and the stores (a
 // register double buffer would need twice the stage-1 registers; a cp.async staging tile would add two
 // shared-memory passes per element and cost the occupancy a second 69 KB buffer allows).
 //
 // TC = 16 (128 B row segments), NT = 320: stage 1 has 27 x 16 = 432 items of 20 points (threads 0..111 take two),
-// stage 2 has 20 x 16 = 320 items of 27 points (one per thread).  One CTA per SM (a 69 KB exchange buffer each for
-// A, B and the product in the z pass).
+// stage 2 has 20 x 16 = 320 items of 27 points (one per thread).  One CTA per SM (three 69 KB tile buffers in the z
+// pass).
 #define COL540_TC 16
 #define COL540_NT 320
 typedef RegFft2<20, 27, COL540_TC, COL540_NT> Col540;      // forward: 20 first, then 27
@@ -838,35 +839,89 @@ __global__ void __launch_bounds__(COL540_NT, 1) k_fft_col540(const __grid_consta
 }
 
 // z cross-power: forward z FFT of A and B, unit-magnitude normalisation and conj(A) * B, then the forward FFT of
-// the product as RegFft2<27, 20>, which starts on the registers holding the product.  A's spectrum stays in its
-// exchange buffer (each stage-2 item writes its 27 outputs back to the 27 slots it read), so B's loads can be in
-// flight under A's stage 2 without the 54 registers of A's column on top.  Three exchange buffers (A, B, product),
-// three barriers per tile.  B(t) loads under A's stage 2, A(t+1) under the product's stage 2 and the stores.
-__global__ void __launch_bounds__(COL540_NT, 1) k_fft_xpower_col540(const __grid_constant__ StridedPipeArgs p) {
+// the product as RegFft2<27, 20>, which starts on the registers holding the product.
+//
+// The tiles reach shared memory by tensor-map TMA copies issued by one thread and completing on the buffer's
+// mbarrier, so a load is in flight from the moment its buffer is released until the tile needs it, with no registers
+// held for it.  Three 69 KB buffers: B always lands in buffer 1, A alternates between buffers 0 and 2.  Per tile t,
+// with A(t) in XA, B(t) landing in XB and XZ free:
+//   A: stage 1 in place in XA | barrier | copy A(t+1) into XZ, stage 2 in place (the spectrum stays in XA)
+//   B: stage 1 in place in XB | barrier | stage 2 with the normalisation and conj(A) * B into registers
+//   barrier (XA, XB read out) | copy B(t+1) into XB, product stage 1 into XA | barrier | product stage 2 + stores
+// so A(t+1) has five phases to land and B(t+1) four.  XA becomes the next tile's free buffer.
+//
+// A tile is 540 rows of 128 B, one z-stride apart.  As 1-D bulk copies that is 1080 copies per tile pair, and the
+// copy engine's per-copy cost made the pass 2.8x slower than register loads (H100 80GB HBM3, 700 W).  A 3-D tensor map
+// of each spectrum ([Pz][Py][2 pitch] floats, encoded per launch) moves the tile in COL540_ZBOXES boxes of
+// 32 floats x 1 x 180 rows.
+#define COL540_ZBOXES 3
+static_assert(Col540::N % COL540_ZBOXES == 0 && Col540::N / COL540_ZBOXES <= 256, "a TMA box has at most 256 rows");
+struct XpowerCol540Args {
+    CUtensorMap tm[2];   // spectra A and B
+    StridedPipeArgs p;
+};
+
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* tm, int x, int y, int z, unsigned long long* bar) {
+    asm volatile(
+        "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
+        ::"r"(smem_u32(dst)), "l"(tm), "r"(x), "r"(y), "r"(z), "r"(smem_u32(bar))
+        : "memory");
+}
+
+__global__ void __launch_bounds__(COL540_NT, 1) k_fft_xpower_col540(const __grid_constant__ XpowerCol540Args P) {
+    const StridedPipeArgs& p = P.p;
     const StridedArgs& a = p.s;
-    float2* tw = bs_sm;
-    float2* XA = bs_sm + Col540::N;
-    float2* XB = XA + Col540::XSIZE;
-    float2* XQ = XB + Col540::XSIZE;
+    float2* X0 = bs_sm;   // the copies need 128-byte aligned targets: buffers first
+    float2* tw = X0 + 3 * Col540::XSIZE;
+    unsigned long long* bars = reinterpret_cast<unsigned long long*>(tw + Col540::N);
     auto tile_off = [&](int t) -> size_t {
         return (size_t)(t / p.tiles_x) * a.ostride + (size_t)(t % p.tiles_x) * COL540_TC;
     };
-    Col540::In v;
-    Col540Q::In q;   // q[u] = product column of Col540's stage-2 item u
-    int t = blockIdx.x;
-    if (t < p.n_tiles) Col540::load(v, a.a + tile_off(t), a.estride);
+    // thread 0: copy tile t of spectrum im into buffer b.  The fence orders the generic-proxy accesses to b before
+    // the barrier that released it ahead of the async-proxy writes of the copy.
+    auto fetch = [&](int im, int t, int b) {
+        constexpr int rows = Col540::N / COL540_ZBOXES;
+        fence_proxy_async_smem();
+        mbar_expect_tx(&bars[b], Col540::XSIZE * sizeof(float2));
+        float2* dst = X0 + b * Col540::XSIZE;
+        const int x = (t % p.tiles_x) * 2 * COL540_TC, y = t / p.tiles_x;
+#pragma unroll
+        for (int k = 0; k < COL540_ZBOXES; ++k) tma_load_3d(dst + k * rows * COL540_TC, &P.tm[im], x, y, k * rows, &bars[b]);
+    };
+    if (threadIdx.x == 0) {
+        for (int b = 0; b < 3; ++b) mbar_init(&bars[b], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
     col540_tw(tw, a.tw);
     __syncthreads();
-    for (; t < p.n_tiles; t += gridDim.x) {
-        const size_t off = tile_off(t);
+    int t = blockIdx.x;
+    if (threadIdx.x == 0 && t < p.n_tiles) {
+        fetch(0, t, 0);
+        fetch(1, t, 1);
+    }
+    int ia = 0;                // A's buffer; the free one is 2 - ia
+    unsigned int phase = 0u;   // bit b: parity of bars[b]'s next phase (the roles rotate, so it is kept per buffer)
+    Col540::In v;
+    Col540Q::In q;   // q[u] = product column of Col540's stage-2 item u
+    for (; t < p.n_tiles; t += gridDim.x, ia = 2 - ia) {
+        const int tn = t + gridDim.x;
+        float2* XA = X0 + ia * Col540::XSIZE;
+        float2* XB = X0 + Col540::XSIZE;
+        mbar_wait(&bars[ia], (phase >> ia) & 1u);
+        phase ^= 1u << ia;
+        Col540::load_shared(v, XA);
         Col540::stage1(v, XA, tw);
-        Col540::load(v, a.b + off, a.estride);
-        __syncthreads();
+        __syncthreads();   // also: the previous tile's product stage 2 has read XZ out
+        if (threadIdx.x == 0 && tn < p.n_tiles) fetch(0, tn, 2 - ia);
         Col540::stage2(XA, [&](const float2 (&w)[27], int, int k1, int c) {
             float2* s = Col540::slot(XA, k1, c);
 #pragma unroll
             for (int k2 = 0; k2 < 27; ++k2) s[k2 * COL540_TC] = w[k2];
         });
+        mbar_wait(&bars[1], (phase >> 1) & 1u);
+        phase ^= 2u;
+        Col540::load_shared(v, XB);
         Col540::stage1(v, XB, tw);
         __syncthreads();
         Col540::stage2(XB, [&](const float2 (&w)[27], int u, int k1, int c) {
@@ -878,12 +933,12 @@ __global__ void __launch_bounds__(COL540_NT, 1) k_fft_xpower_col540(const __grid
                 q[u][k2] = make_float2(x.x * y.x + x.y * y.y, x.x * y.y - x.y * y.x);  // conj(x) * y
             }
         });
-        Col540Q::stage1(q, XQ, tw);
-        const int tn = t + gridDim.x;
-        if (tn < p.n_tiles) Col540::load(v, a.a + tile_off(tn), a.estride);
         __syncthreads();
-        float2* g = a.a + off;
-        Col540Q::stage2(XQ, [&](const float2 (&w)[20], int, int k1, int c) { Col540Q::store(w, g, a.estride, k1, c); });
+        if (threadIdx.x == 0 && tn < p.n_tiles) fetch(1, tn, 1);
+        Col540Q::stage1(q, XA, tw);
+        __syncthreads();
+        float2* g = a.a + tile_off(t);
+        Col540Q::stage2(XA, [&](const float2 (&w)[20], int, int k1, int c) { Col540Q::store(w, g, a.estride, k1, c); });
     }
 }
 
@@ -1767,16 +1822,37 @@ static int set_smem(bs_ctx* ctx, const void* fn, size_t bytes) {
 }
 
 // n_img: 1 or 2 spectra through k_fft_col540 (y), 0 for the cross-power k_fft_xpower_col540 (z)
-static void launch_col540(bs_ctx* ctx, const StridedArgs& a, int tiles_x, int n_other, int n_img) {
+static int launch_col540(bs_ctx* ctx, const StridedArgs& a, int tiles_x, int n_other, int n_img) {
     StridedPipeArgs pp;
     pp.s = a;
     pp.tiles_x = tiles_x;
     pp.n_other = n_other;
     pp.n_tiles = tiles_x * n_other * (n_img ? n_img : 1);
     const int nctas = std::min(pp.n_tiles, ctx->sm_count);   // one CTA per SM (shared memory, registers)
-    const size_t smem = (Col540::N + (n_img ? 2 : 3) * (size_t)Col540::XSIZE) * sizeof(float2);
-    if (n_img) k_fft_col540<<<nctas, COL540_NT, smem, ctx->stream>>>(pp);
-    else k_fft_xpower_col540<<<nctas, COL540_NT, smem, ctx->stream>>>(pp);
+    if (n_img) {
+        const size_t smem = (Col540::N + 2 * (size_t)Col540::XSIZE) * sizeof(float2);
+        k_fft_col540<<<nctas, COL540_NT, smem, ctx->stream>>>(pp);
+        return BS_OK;
+    }
+    // z pass: spectra [Pz = 540][Py = n_other][pitch] as floats, one 128 B x 1 x 180-row box per copy
+    XpowerCol540Args xa;
+    xa.p = pp;
+    auto enc = bs_tensor_map_encoder();
+    if (!enc) return bs_set_error(ctx, BS_ERR_CUDA, "pcm: cuTensorMapEncodeTiled is not available");
+    const cuuint64_t gdim[3] = {(cuuint64_t)tiles_x * 2 * COL540_TC, (cuuint64_t)n_other, (cuuint64_t)Col540::N};
+    const cuuint64_t gstr[2] = {(cuuint64_t)a.ostride * sizeof(float2), (cuuint64_t)a.estride * sizeof(float2)};
+    const cuuint32_t box[3] = {2 * COL540_TC, 1, Col540::N / COL540_ZBOXES};
+    const cuuint32_t estr[3] = {1, 1, 1};
+    for (int i = 0; i < 2; ++i) {
+        const CUresult r = enc(&xa.tm[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, i ? (void*)a.b : (void*)a.a, gdim, gstr, box,
+                               estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                               CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (r != CUDA_SUCCESS) return bs_set_error(ctx, BS_ERR_CUDA, "pcm: cuTensorMapEncodeTiled failed (%d)", (int)r);
+    }
+    // buffers, twiddles, one mbarrier per buffer
+    const size_t smem = (3 * (size_t)Col540::XSIZE + Col540::N) * sizeof(float2) + 3 * sizeof(unsigned long long);
+    k_fft_xpower_col540<<<nctas, COL540_NT, smem, ctx->stream>>>(xa);
+    return BS_OK;
 }
 
 static int pcm_kernel_attrs(bs_ctx* ctx) {
@@ -1909,7 +1985,8 @@ static int pcm_launch_y(bs_ctx* ctx, const PcmGeometry& g, PcmDeviceTables* t, i
         bs_launch_scope sc(ctx, tag);
         const size_t smem_pipe = ((size_t)((g.P[1] + 1) & ~1) + 3 * (size_t)g.P[1] * (1 << g.tshift_y)) * sizeof(float2);
         if (g.static_y) {
-            launch_col540(ctx, a, g.pitch / COL540_TC, g.P[2], n_img);
+            int rc;
+            if ((rc = launch_col540(ctx, a, g.pitch / COL540_TC, g.P[2], n_img))) return rc;
             pass_info(info, "k_fft_col540", nullptr);
         } else if (smem_pipe <= PCM_SMEM_MAX) {
             StridedPipeArgs pp;
@@ -1949,7 +2026,8 @@ static int pcm_pass_z_xpower(bs_ctx* ctx, const PcmGeometry& g, PcmDeviceTables*
     {
         bs_launch_scope sc(ctx, "fft_z_xpower");
         if (g.static_z) {
-            launch_col540(ctx, a, g.pitch / COL540_TC, g.P[1], 0);
+            int rc;
+            if ((rc = launch_col540(ctx, a, g.pitch / COL540_TC, g.P[1], 0))) return rc;
             pass_info(info, "k_fft_xpower_col540", nullptr);
         } else {
             StridedPipeArgs pp;

@@ -354,6 +354,17 @@ struct RegFft2 {
             for (int n1 = 0; n1 < RA; ++n1) v[u][n1] = __ldcg(p + (long long)(RB * n1) * estride);
         }
     }
+    // the same items from a tile staged in shared memory as X[n TC + c].  Item (n2, c) reads the RA slots that its
+    // stage 1 writes (n = RB n1 + n2 and k1 RB + n2), so stage1(v, X, tw) may follow without a barrier.
+    static __device__ __forceinline__ void load_shared(In& v, const float2* __restrict__ X) {
+#pragma unroll
+        for (int u = 0; u < IT1; ++u) {
+            if (!live1(u)) continue;
+            const float2* p = X + threadIdx.x + u * NT;
+#pragma unroll
+            for (int n1 = 0; n1 < RA; ++n1) v[u][n1] = p[RB * n1 * TC];
+        }
+    }
     static __device__ __forceinline__ void stage1(In& v, float2* __restrict__ X, const float2* __restrict__ tw) {
 #pragma unroll
         for (int u = 0; u < IT1; ++u) {
