@@ -5,6 +5,7 @@
   stitching               J/SparkPairwiseStitching.java:110-392
   create_fusion_container J/CreateFusionContainer.java:122-519   (N5 or OME-ZARR, all channels / timepoints, pyramid)
   affine_fusion           J/SparkAffineFusion.java:179-800       (s0 + multi-resolution pyramid)
+  nonrigid_fusion         J/SparkNonRigidFusion.java:124-446     (MLS grids from interest-point correspondences)
   detect_interestpoints   J/SparkInterestPointDetection.java:173-964 (block-wise DoG, interestpoints.n5 + the XML)
 
 No argument parsing here (the picocli layer is out of scope); keyword names follow the CLI flags.
@@ -700,3 +701,192 @@ def detect_interestpoints(xml_path, ctx: Context, label, sigma, threshold, min_i
                              paths)
     data.save(xml_path)
     return results
+
+
+# --------------------------------------------------------------------------------------------- nonrigid-fusion
+NONRIGID_FUSE_EXPAND = 50      # viewsToFuse: transformed bounding box expanded by 50 (J/SparkNonRigidFusion.java:333-340)
+NONRIGID_USE_EXPAND = 25       # viewsToUse: both boxes expanded by 25 (J/SparkNonRigidFusion.java:349-371)
+
+
+def nonrigid_views_for_block(view_dims, registrations, block_min, block_max, view_ids):
+    """(viewsToFuse, viewsToUse) of one super-block (J/SparkNonRigidFusion.java:317-371): the views whose transformed
+    bounding box, expanded by 50, overlaps the block; and every view whose box expanded by 25 overlaps the box of a
+    fused view expanded by 25 (the fused views included)."""
+    fuse = bf.find_overlapping_views(view_dims, registrations, block_min, block_max, view_ids, expand=NONRIGID_FUSE_EXPAND)
+    boxes = {v: bf.transformed_bounding_box(view_dims[v], registrations[v]) for v in view_ids}
+    e = NONRIGID_USE_EXPAND
+    use = [v for v in view_ids
+           if any(np.all(np.minimum(boxes[v][1] + e, boxes[f][1] + e) >= np.maximum(boxes[v][0] - e, boxes[f][0] - e))
+                  for f in fuse)]
+    return fuse, use
+
+
+class _InterestPoints:
+    """Every selected view's points and correspondences of the `-ip` labels, read once from interestpoints.n5, with
+    their world positions (the view's registration applied to the full-resolution pixel location)."""
+
+    def __init__(self, store: bn5.N5Store, view_ids, labels, registrations):
+        self.labels = list(labels)
+        self.loc, self.world, self.index, self.corr = {}, {}, {}, {}
+        for v in view_ids:
+            for label in self.labels:
+                group = f"tpId_{v[0]}_viewSetupId_{v[1]}/{label}"
+                if "dimensions" not in store.get_attributes(group + "/interestpoints/loc"):
+                    continue
+                ids = store.read_list(group + "/interestpoints/id").reshape(-1).astype(np.int64)
+                loc = store.read_list(group + "/interestpoints/loc").astype(np.float64).reshape(-1, 3)
+                M = np.asarray(registrations[v], dtype=np.float64).reshape(3, 4)
+                self.loc[(v, label)] = loc
+                self.world[(v, label)] = loc @ M[:, :3].T + M[:, 3]
+                self.index[(v, label)] = {int(i): k for k, i in enumerate(ids)}
+                self.corr[(v, label)] = store.read_correspondences(group)
+
+    def targets(self, view, views_to_use):
+        """N2: (target world (n, 3), local pixel (n, 3)) of one view to fuse: every point with at least one
+        correspondence whose partner is in ``views_to_use`` and has one of the labels; the target is the mean of the
+        point's own world position and its direct partners' world positions."""
+        use = set(views_to_use)
+        ts, ls = [], []
+        for label in self.labels:
+            key = (view, label)
+            if key not in self.loc:
+                continue
+            acc = np.zeros_like(self.world[key])
+            cnt = np.zeros(len(acc), dtype=np.int64)
+            for (pid, pv, pl, qid) in self.corr[key]:
+                if pv in use and pl in self.labels and (pv, pl) in self.loc:
+                    k = self.index[key][pid]
+                    acc[k] += self.world[(pv, pl)][self.index[(pv, pl)][qid]]
+                    cnt[k] += 1
+            sel = cnt > 0
+            ts.append((self.world[key][sel] + acc[sel]) / (cnt[sel] + 1)[:, None])
+            ls.append(self.loc[key][sel])
+        if not ts:
+            return np.zeros((0, 3)), np.zeros((0, 3))
+        return np.concatenate(ts), np.concatenate(ls)
+
+
+def nonrigid_fusion(xml_path, ctx: Context, out_path, n5_dataset, interest_points, storage="N5",
+                    block_size=(128, 128, 128), block_scale=(2, 2, 1), data_type="FLOAT32", min_intensity=None,
+                    max_intensity=None, view_selection=None, bdv=None, xml_out=None, bounding_box=None, dry_run=False,
+                    shard=(0, 1), retries=5, blocks_per_call=16):
+    """`./nonrigid-fusion -x dataset.xml -o fused.n5 -d /ch0/s0 -ip beads [-ip nuclei] [-s N5|ZARR] [--blockSize ...]
+    [--blockScale 2,2,1] [-p FLOAT32|UINT16|UINT8 --minIntensity --maxIntensity]` (J/SparkNonRigidFusion.java:124-446):
+    the maximal bounding box of the selected views becomes dataset ``n5_dataset`` (Zstandard, attribute offset = bb.min);
+    every super-block of Grid.create(dims, blockSize * blockScale, blockSize) that some view reaches is fused on the
+    device with per-view moving-least-squares grids fitted to the corresponding interest points of the ``-ip`` labels
+    (bs_nonrigid_fuse_blocks, AVG_BLEND, control points every 10 px) and saved; blocks no view reaches are not written.
+    Returns the list of written grid positions.  ZARR output is the (t, c, z, y, x) array with singleton t and c.
+
+    ``--bdv`` / ``-xo``, named ``-b`` bounding boxes, multi-GPU sharding and ``--dryRun`` raise NotImplementedError."""
+    for flag, on in (("--bdv", bdv is not None), ("-xo", xml_out is not None), ("-b", bounding_box is not None),
+                     ("--dryRun", dry_run), ("multi-GPU sharding", shard[1] > 1)):
+        if on:
+            raise NotImplementedError(f"nonrigid-fusion {flag} is not implemented")
+    dt = data_type.upper()
+    if dt not in ("FLOAT32", "UINT16", "UINT8"):
+        raise ValueError(f"-p {data_type}")
+    if dt != "FLOAT32" and (min_intensity is None or max_intensity is None):
+        raise ValueError("When selecting UINT8 or UINT16 you need to specify minIntensity and maxIntensity.")
+    if not interest_points:
+        raise ValueError("no interest points defined, exiting.")
+    labels = list(interest_points)
+    data = SpimData2.load(xml_path)
+    fmt, n5_in = data.image_loader()
+    if fmt != "bdv.n5":
+        raise NotImplementedError(f"ImageLoader format {fmt}")
+    src = bn5.N5Store(n5_in)
+    views = sorted(data.select_views(**view_selection) if view_selection else data.view_ids())
+    regs = {v: data.model(*v) for v in views}
+    vdims = {v: tuple(int(d) for d in data.setups[v[1]].size) for v in views}
+    lo = np.full(3, np.iinfo(np.int64).max, dtype=np.int64)
+    hi = np.full(3, np.iinfo(np.int64).min, dtype=np.int64)
+    for v in views:
+        bmin, bmax = bf.transformed_bounding_box(vdims[v], regs[v])
+        lo, hi = np.minimum(lo, bmin), np.maximum(hi, bmax)
+    dims = [int(hi[d] - lo[d] + 1) for d in range(3)]
+    bs = [int(b) for b in block_size]
+    np_dt = {"FLOAT32": np.float32, "UINT16": np.uint16, "UINT8": np.uint8}[dt]
+    od = native._NP2BS[np.dtype(np_dt)]
+    is_zarr = storage.upper() == "ZARR"
+    if is_zarr:
+        store = bzarr.ZarrStore(out_path, create=True)
+        store.create_array(n5_dataset, [1, 1] + dims[::-1], [1, 1] + bs[::-1], np.dtype(np_dt).name, "zstd")
+    else:
+        store = bn5.N5Store(out_path, create=True)
+        store.create_dataset(n5_dataset, dims, bs, np_dt, "zstd")
+    store.set_attributes(n5_dataset, {"offset": [int(v) for v in lo]})
+    sink = _Sink(store, is_zarr, 0, 0)
+    params = ctx.fuse_params(native.FUSE_AVG_BLEND, 1, od, 0, float(min_intensity or 0.0),
+                             float(max_intensity if max_intensity is not None else 65535.0))
+
+    base = os.path.join(os.path.dirname(os.path.abspath(xml_path)), data.root.findtext("BasePath") or ".")
+    ips = _InterestPoints(bn5.N5Store(os.path.join(base, "interestpoints.n5")), views, labels, regs)
+    blending = {v: bf.adjust_blending(regs[v]) for v in views}
+
+    # super-blocks grouped by (viewsToFuse, viewsToUse): one set of MLS point lists per group
+    compute = [bs[d] * int(block_scale[d]) for d in range(3)]
+    groups = {}
+    for gb in bf.grid_create(dims, compute, bs):
+        off, size, _ = gb
+        mn = lo + np.asarray(off, dtype=np.int64)
+        fuse, use = nonrigid_views_for_block(vdims, regs, mn, mn + np.asarray(size) - 1, views)
+        if fuse:
+            groups.setdefault((tuple(fuse), tuple(use)), []).append(gb)
+    written = []
+    cpd = (native.NONRIGID_CP_DISTANCE,) * 3
+    for (fuse, use), gbs in groups.items():
+        nviews = {}
+        for v in fuse:
+            t, l = ips.targets(v, use)
+            border, rng = blending[v]
+            nviews[v] = dict(src_to_world=regs[v], vol_handle=0, blend_border=border, blend_range=rng,
+                             full_dims=vdims[v], target_world_xyz=t, local_xyz=l)
+        todo, attempt = list(gbs), 0
+        while todo:
+            attempt += 1
+            if attempt > retries:
+                raise RuntimeError(f"nonrigid-fusion: {len(todo)} block(s) still failing after {retries} attempts")
+            failed = []
+            for c0 in range(0, len(todo), blocks_per_call):
+                chunk = todo[c0:c0 + blocks_per_call]
+                try:
+                    outs = _nonrigid_chunk(ctx, src, chunk, lo, fuse, nviews, vdims, params, cpd)
+                except native.BsError:
+                    failed.extend(chunk)
+                    continue
+                for (off, size, gpos), blk in zip(chunk, outs):
+                    sink.save(n5_dataset, blk, gpos)
+                    written.append(tuple(gpos))
+            todo = failed
+    return written
+
+
+def _nonrigid_chunk(ctx, src, chunk, bb_min, fuse, nviews, vdims, params, cpd):
+    """Fuse a list of super-blocks that share their views.  Each view's source window is the range its control-point
+    grids map to over the chunk (+2 px for the n-linear taps), read from level s0 and uploaded as a windowed view."""
+    mins = [tuple(int(v) for v in bb_min + np.asarray(off, dtype=np.int64)) for off, _, _ in chunk]
+    sizes = [tuple(int(v) for v in size) for _, size, _ in chunk]
+    staged, gviews = [], []
+    try:
+        for v in fuse:
+            nv = nviews[v]
+            glo = np.full(3, np.inf)
+            ghi = np.full(3, -np.inf)
+            for mn, sz in zip(mins, sizes):
+                g = ctx.nonrigid_debug_grid(nv, mn, sz, cpd).reshape(-1, 3)
+                glo, ghi = np.minimum(glo, g.min(axis=0)), np.maximum(ghi, g.max(axis=0))
+            dims = np.asarray(vdims[v], dtype=np.int64)
+            wlo = np.maximum(np.floor(glo).astype(np.int64) - 2, 0)
+            whi = np.minimum(np.ceil(ghi).astype(np.int64) + 2, dims - 1)
+            if np.any(whi < wlo):
+                continue                                  # the view's grids never reach its pixels in this chunk
+            h = ctx.volume_upload(src.read_region(bn5.bdv_dataset(v[1], v[0], 0), wlo, whi - wlo + 1))
+            staged.append(h)
+            gviews.append(dict(nv, vol_handle=h, window_min=tuple(int(x) for x in wlo)))
+        if not gviews:
+            return [np.zeros(tuple(s)[::-1], dtype=native._out_dtype(params)) for s in sizes]
+        return ctx.nonrigid_fuse_blocks(gviews, mins, sizes, params, cpd)
+    finally:
+        for h in staged:
+            ctx.volume_free(h)

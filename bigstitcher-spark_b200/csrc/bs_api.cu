@@ -56,7 +56,7 @@ int bs_volume_acquire(bs_ctx* ctx, bs_volume& v) {
 
 extern "C" {
 
-int bs_version(void) { return 106; }
+int bs_version(void) { return 107; }
 
 int bs_init(bs_ctx** out, int device, void* stream) {
     if (!out) return bs_set_error(nullptr, BS_ERR_ARG, "bs_init: out is NULL");
@@ -131,6 +131,7 @@ void bs_destroy(bs_ctx* ctx) {
     bs_pcm_workspace_free(ctx);
     bs_fuse2_free(ctx);
     bs_dog_free(ctx);
+    bs_nonrigid_free(ctx);
     bs_comm_free(ctx);
     if (ctx->fuse_ring_dev) cudaFree(ctx->fuse_ring_dev);
     if (ctx->fuse_ring_host) cudaFreeHost(ctx->fuse_ring_host);

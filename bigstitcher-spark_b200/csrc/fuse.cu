@@ -44,48 +44,6 @@ struct FuseArgs {
     const struct TilePlan* plan;   // per-tile view lists from fuse_plan_kernel (or nullptr)
 };
 
-template <typename T>
-__device__ __forceinline__ float ld_as_float(const T* p, size_t i) {
-    return (float)__ldg(p + i);
-}
-
-template <typename T, bool LINEAR>
-__device__ __forceinline__ float sample(const T* __restrict__ d, int dx, int dy, int dz, float sx, float sy,
-                                        float sz) {
-    if (LINEAR) {
-        float fx = floorf(sx), fy = floorf(sy), fz = floorf(sz);
-        float rx = sx - fx, ry = sy - fy, rz = sz - fz;
-        int x0 = (int)fx, y0 = (int)fy, z0 = (int)fz;
-        int x1 = min(x0 + 1, dx - 1), y1 = min(y0 + 1, dy - 1), z1 = min(z0 + 1, dz - 1);
-        size_t r00 = ((size_t)z0 * dy + y0) * dx, r01 = ((size_t)z0 * dy + y1) * dx;
-        size_t r10 = ((size_t)z1 * dy + y0) * dx, r11 = ((size_t)z1 * dy + y1) * dx;
-        float a000 = ld_as_float(d, r00 + x0), a001 = ld_as_float(d, r00 + x1);
-        float a010 = ld_as_float(d, r01 + x0), a011 = ld_as_float(d, r01 + x1);
-        float a100 = ld_as_float(d, r10 + x0), a101 = ld_as_float(d, r10 + x1);
-        float a110 = ld_as_float(d, r11 + x0), a111 = ld_as_float(d, r11 + x1);
-        float c00 = a000 + rx * (a001 - a000);
-        float c01 = a010 + rx * (a011 - a010);
-        float c10 = a100 + rx * (a101 - a100);
-        float c11 = a110 + rx * (a111 - a110);
-        float c0 = c00 + ry * (c01 - c00);
-        float c1 = c10 + ry * (c11 - c10);
-        return c0 + rz * (c1 - c0);
-    } else {
-        int xi = min(max((int)floorf(sx + 0.5f), 0), dx - 1);
-        int yi = min(max((int)floorf(sy + 0.5f), 0), dy - 1);
-        int zi = min(max((int)floorf(sz + 0.5f), 0), dz - 1);
-        return ld_as_float(d, ((size_t)zi * dy + yi) * dx + xi);
-    }
-}
-
-template <bool LINEAR>
-__device__ __forceinline__ float sample_any(const void* d, int dtype, int dx, int dy, int dz, float sx,
-                                            float sy, float sz) {
-    if (dtype == BS_DTYPE_U16) return sample<unsigned short, LINEAR>((const unsigned short*)d, dx, dy, dz, sx, sy, sz);
-    if (dtype == BS_DTYPE_F32) return sample<float, LINEAR>((const float*)d, dx, dy, dz, sx, sy, sz);
-    return sample<unsigned char, LINEAR>((const unsigned char*)d, dx, dy, dz, sx, sy, sz);
-}
-
 // ---- staged footprint: a fixed FS_X x FS_Y x FS_Z float box per (CTA tile, view) in shared memory
 #define FS_X 40
 #define FS_Y 12
@@ -262,14 +220,7 @@ __global__ void fuse_plan_kernel(const FuseViewDev* __restrict__ views, int nvie
 
 template <int OUT>
 __device__ __forceinline__ void store_voxel(const FuseArgs& a, size_t o, float res) {
-    if (OUT == BS_DTYPE_F32) {
-        __stcs((float*)a.out + o, res);
-    } else {
-        double c = floor(((double)res - a.cmin) * a.cscale + 0.5);
-        c = fmin(fmax(c, 0.0), a.ctop);
-        if (OUT == BS_DTYPE_U16) ((unsigned short*)a.out)[o] = (unsigned short)c;
-        else ((unsigned char*)a.out)[o] = (unsigned char)c;
-    }
+    bs_store_converted<OUT>(a.out, o, res, a.cmin, a.cscale, a.ctop);
 }
 
 // KIND 0: weighted average family (AVG, AVG_BLEND, *_CONTENT); KIND 1: winner family.

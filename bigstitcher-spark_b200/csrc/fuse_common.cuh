@@ -1,11 +1,79 @@
-// Pieces shared by the two fusion translation units (fuse.cu: generic tile kernel; fuse_tma.cu: TMA-staged
-// z-marching kernels).
+// Pieces shared by the fusion translation units (fuse.cu: generic tile kernel; fuse_tma.cu: TMA-staged
+// z-marching kernels; nonrigid.cu: moving-least-squares grids and non-rigid fusion).
 #pragma once
 #include <cmath>
 
 #include "bs_internal.cuh"
 
 #define FUSE_MAX_LUT 256
+
+template <typename T>
+__device__ __forceinline__ float ld_as_float(const T* p, size_t i) {
+    return (float)__ldg(p + i);
+}
+
+// n-linear (LINEAR) or nearest-neighbour sample of a dense x-fastest volume at (sx, sy, sz); the upper taps are
+// clamped to the volume (border extension), the caller keeps the coordinate >= 0
+template <typename T, bool LINEAR>
+__device__ __forceinline__ float sample(const T* __restrict__ d, int dx, int dy, int dz, float sx, float sy,
+                                        float sz) {
+    if (LINEAR) {
+        float fx = floorf(sx), fy = floorf(sy), fz = floorf(sz);
+        float rx = sx - fx, ry = sy - fy, rz = sz - fz;
+        int x0 = (int)fx, y0 = (int)fy, z0 = (int)fz;
+        int x1 = min(x0 + 1, dx - 1), y1 = min(y0 + 1, dy - 1), z1 = min(z0 + 1, dz - 1);
+        size_t r00 = ((size_t)z0 * dy + y0) * dx, r01 = ((size_t)z0 * dy + y1) * dx;
+        size_t r10 = ((size_t)z1 * dy + y0) * dx, r11 = ((size_t)z1 * dy + y1) * dx;
+        float a000 = ld_as_float(d, r00 + x0), a001 = ld_as_float(d, r00 + x1);
+        float a010 = ld_as_float(d, r01 + x0), a011 = ld_as_float(d, r01 + x1);
+        float a100 = ld_as_float(d, r10 + x0), a101 = ld_as_float(d, r10 + x1);
+        float a110 = ld_as_float(d, r11 + x0), a111 = ld_as_float(d, r11 + x1);
+        float c00 = a000 + rx * (a001 - a000);
+        float c01 = a010 + rx * (a011 - a010);
+        float c10 = a100 + rx * (a101 - a100);
+        float c11 = a110 + rx * (a111 - a110);
+        float c0 = c00 + ry * (c01 - c00);
+        float c1 = c10 + ry * (c11 - c10);
+        return c0 + rz * (c1 - c0);
+    } else {
+        int xi = min(max((int)floorf(sx + 0.5f), 0), dx - 1);
+        int yi = min(max((int)floorf(sy + 0.5f), 0), dy - 1);
+        int zi = min(max((int)floorf(sz + 0.5f), 0), dz - 1);
+        return ld_as_float(d, ((size_t)zi * dy + yi) * dx + xi);
+    }
+}
+
+template <bool LINEAR>
+__device__ __forceinline__ float sample_any(const void* d, int dtype, int dx, int dy, int dz, float sx,
+                                            float sy, float sz) {
+    if (dtype == BS_DTYPE_U16) return sample<unsigned short, LINEAR>((const unsigned short*)d, dx, dy, dz, sx, sy, sz);
+    if (dtype == BS_DTYPE_F32) return sample<float, LINEAR>((const float*)d, dx, dy, dz, sx, sy, sz);
+    return sample<unsigned char, LINEAR>((const unsigned char*)d, dx, dy, dz, sx, sy, sz);
+}
+
+// Output element encoding: the kernels' OUT template value = output dtype | OUT_BE.  Big-endian output
+// (bs_fuse_params.out_big_endian) is a compile-time property of the instantiation, so the native-order kernels carry
+// no byte-order code at all and the big-endian ones pay one PRMT per store.
+#define OUT_BE 8
+#define OUT_DT(OUT) ((OUT) & 7)
+__device__ __forceinline__ unsigned int bswap32(unsigned int v) { return __byte_perm(v, 0u, 0x0123); }
+__device__ __forceinline__ unsigned int bswap16x2(unsigned int v) { return __byte_perm(v, 0u, 0x2301); }
+
+// one output voxel: float32 as it is, integer types through the converter (v - cmin) * cscale, rounded as
+// floor(x + 0.5) and clamped to [0, ctop]
+template <int OUT>
+__device__ __forceinline__ void bs_store_converted(void* out, size_t o, float res, double cmin, double cscale, double ctop) {
+    constexpr bool BE = (OUT & OUT_BE) != 0;
+    if (OUT_DT(OUT) == BS_DTYPE_F32) {
+        if (BE) __stcs((unsigned int*)out + o, bswap32(__float_as_uint(res)));
+        else __stcs((float*)out + o, res);
+    } else {
+        double c = floor(((double)res - cmin) * cscale + 0.5);
+        c = fmin(fmax(c, 0.0), ctop);
+        if (OUT_DT(OUT) == BS_DTYPE_U16) ((unsigned short*)out)[o] = (unsigned short)(BE ? bswap16x2((unsigned int)c) : (unsigned int)c);
+        else ((unsigned char*)out)[o] = (unsigned char)c;
+    }
+}
 
 // cosine blending weight along one axis (l = absolute source coordinate); false when weight is 0
 __device__ __forceinline__ bool blend_axis(float l, float dm1, float border, float inv_range, int lut_n,

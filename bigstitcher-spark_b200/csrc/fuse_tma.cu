@@ -280,14 +280,7 @@ __global__ void fuse_plan2_kernel(const ViewDev* __restrict__ views, const Block
 }
 
 // ------------------------------------------------------------------------------------------ output
-// The kernels' OUT template value = output dtype | OUT_BE: big-endian output (bs_fuse_params.out_big_endian) is a
-// compile-time property of the instantiation, so the native-order kernels carry no byte-order code at all and the
-// big-endian ones pay one PRMT per store.
-#define OUT_BE 8
-#define OUT_DT(OUT) ((OUT) & 7)
-__device__ __forceinline__ unsigned int bswap32(unsigned int v) { return __byte_perm(v, 0u, 0x0123); }
-__device__ __forceinline__ unsigned int bswap16x2(unsigned int v) { return __byte_perm(v, 0u, 0x2301); }
-
+// (OUT = output dtype | OUT_BE, see fuse_common.cuh)
 template <int OUT>
 __device__ __forceinline__ unsigned int conv_int(const FuseArgs2& a, float res) {
     double c = floor(((double)res - a.cmin) * a.cscale + 0.5);

@@ -77,10 +77,12 @@ def transformed_bounding_box(dims_xyz, m):
     return np.floor(w.min(axis=0)).astype(np.int64), np.ceil(w.max(axis=0)).astype(np.int64)
 
 
-def find_overlapping_views(view_dims: dict, registrations: dict, block_min, block_max, view_ids=None):
-    """OverlappingViews.findOverlappingViews: transformed bbox intersects the block expanded by 2."""
-    lo = np.asarray(block_min, dtype=np.int64) - AFFINE_EXPANSION
-    hi = np.asarray(block_max, dtype=np.int64) + AFFINE_EXPANSION
+def find_overlapping_views(view_dims: dict, registrations: dict, block_min, block_max, view_ids=None,
+                           expand=AFFINE_EXPANSION):
+    """OverlappingViews.findOverlappingViews: transformed bbox intersects the block expanded by ``expand`` (2; the
+    non-rigid fusion's viewsToFuse use 50, J/SparkNonRigidFusion.java:333-340)."""
+    lo = np.asarray(block_min, dtype=np.int64) - int(expand)
+    hi = np.asarray(block_max, dtype=np.int64) + int(expand)
     out = []
     for vid in (view_ids if view_ids is not None else sorted(registrations)):
         bmin, bmax = transformed_bounding_box(view_dims[vid], registrations[vid])

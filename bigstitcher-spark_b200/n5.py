@@ -239,6 +239,22 @@ class N5Store:
                 out[j * bs[1]:j * bs[1] + b.shape[0]] = b
         return out
 
+    def read_correspondences(self, group):
+        """Correspondences of one label of one view in interestpoints.n5 (``group`` = `tpId_{t}_viewSetupId_{s}/{label}`):
+        the uint64 dataset `correspondences/data` {3, M} of (detectionId, correspondingDetectionId, idMap index) rows and
+        the group attribute idMap {"tp,setup,label": index}.  Returns a list of (detection id, (tp, setup), label,
+        corresponding detection id); [] when the view has no correspondences (dataset {0} or absent)."""
+        path = group.rstrip("/") + "/correspondences"
+        attrs = self.get_attributes(path)
+        if "idMap" not in attrs or "dimensions" not in self.get_attributes(path + "/data"):
+            return []
+        keys = {}
+        for k, idx in attrs["idMap"].items():
+            tp, setup, label = k.split(",", 2)
+            keys[int(idx)] = ((int(tp), int(setup)), label)
+        rows = self.read_list(path + "/data")
+        return [(int(a), keys[int(c)][0], keys[int(c)][1], int(b)) for a, b, c in rows]
+
     def write_volume(self, path, volume: np.ndarray, block_size, compression="raw"):
         self.create_dataset(path, volume.shape[::-1], block_size, volume.dtype, compression)
         self.save_block(path, volume, (0, 0, 0))

@@ -54,6 +54,11 @@ class ViewC(C.Structure):
                 ("blend_range", C.c_float * 3), ("full_dims", C.c_longlong * 3), ("window_min", C.c_longlong * 3)]
 
 
+class NonrigidViewC(C.Structure):
+    _fields_ = [("view", ViewC), ("n_points", C.c_int), ("pad", C.c_int),
+                ("target_world_xyz", C.POINTER(C.c_double)), ("local_xyz", C.POINTER(C.c_double))]
+
+
 class DogParamsC(C.Structure):
     _fields_ = [("sigma", C.c_double), ("threshold", C.c_double), ("min_intensity", C.c_double),
                 ("max_intensity", C.c_double), ("find_max", C.c_int), ("find_min", C.c_int),
@@ -108,8 +113,11 @@ SYMBOLS = [
     "bs_content_weights", "bs_volume_info", "bs_volume_download", "bs_volume_devptr", "bs_downsample", "bs_fuse_block", "bs_fuse_blocks",
     "bs_fuse_block_to_volume", "bs_fuse_accumulate", "bs_fuse_finish", "bs_mask_blocks", "bs_dog_default_params", "bs_dog_detect",
     "bs_dog_debug_dog", "bs_comm_unique_id", "bs_comm_init", "bs_comm_destroy", "bs_fuse_allreduce",
-    "bs_downsample_float", "bs_median_divide", "bs_sample_nlinear",
+    "bs_downsample_float", "bs_median_divide", "bs_sample_nlinear", "bs_nonrigid_fuse_blocks", "bs_nonrigid_debug_grid",
 ]
+
+#: fixed parameters of the reference's non-rigid fusion (J/SparkNonRigidFusion.java:373-383): control-point distance
+NONRIGID_CP_DISTANCE = 10
 
 #: largest --medianFilter radius bs_median_divide accepts (BS_MEDIAN_MAX_RADIUS in include/bsgpu.h)
 MEDIAN_MAX_RADIUS = 32
@@ -178,6 +186,8 @@ def load_library():
     lib.bs_downsample_float.argtypes = [vp, ull, P(ip), P(ull)]
     lib.bs_median_divide.argtypes = [vp, ull, ip, P(ull)]
     lib.bs_sample_nlinear.argtypes = [vp, ull, ip, P(dbl), vp]
+    lib.bs_nonrigid_fuse_blocks.argtypes = [vp, P(NonrigidViewC), ip, ip, P(ll), P(ll), P(ll), P(FuseParamsC), P(vp), ip]
+    lib.bs_nonrigid_debug_grid.argtypes = [vp, P(NonrigidViewC), P(ll), P(ll), P(ll), P(dbl), P(ll)]
     _lib = lib
     return lib
 
@@ -624,6 +634,68 @@ class Context:
         if not (d1 and d2):
             raise ValueError("accumulators must be device buffers")
         self._check(self.lib.bs_fuse_accumulate(self.h, arr, n, bmin, bsz, C.byref(params), p1, p2))
+
+    # -- nonrigid-fusion
+    @staticmethod
+    def make_nonrigid_views(views):
+        """views: iterable of make_views dicts plus target_world_xyz and local_xyz ((n, 3) float64 each).  Returns the
+        ctypes array, its length and the point arrays that must stay alive for the call."""
+        views = list(views)
+        base, n = Context.make_views(views)
+        arr = (NonrigidViewC * max(1, n))()
+        keep = []
+        for i, v in enumerate(views):
+            t = np.ascontiguousarray(np.asarray(v.get("target_world_xyz", np.zeros((0, 3))), dtype=np.float64).reshape(-1, 3))
+            l = np.ascontiguousarray(np.asarray(v.get("local_xyz", np.zeros((0, 3))), dtype=np.float64).reshape(-1, 3))
+            if t.shape != l.shape:
+                raise ValueError("target_world_xyz and local_xyz must have the same shape")
+            keep += [t, l]
+            arr[i].view = base[i]
+            arr[i].n_points = len(t)
+            arr[i].target_world_xyz = t.ctypes.data_as(C.POINTER(C.c_double))
+            arr[i].local_xyz = l.ctypes.data_as(C.POINTER(C.c_double))
+        return arr, n, keep
+
+    def nonrigid_fuse_blocks(self, views, block_mins_xyz, block_sizes_xyz, params: FuseParamsC | None = None,
+                             cp_distance=(NONRIGID_CP_DISTANCE,) * 3, outs=None):
+        """Non-rigid AVG_BLEND fusion of a list of blocks (include/bsgpu.h bs_nonrigid_fuse_blocks).  ``views``: dicts
+        as for make_nonrigid_views; ``outs``: numpy arrays or device tensors / pointers, allocated when None."""
+        params = params or self.fuse_params()
+        arr, n, keep = self.make_nonrigid_views(views)
+        nb = len(block_mins_xyz)
+        bmin = (C.c_longlong * (3 * max(nb, 1)))()
+        bsz = (C.c_longlong * (3 * max(nb, 1)))()
+        for i in range(nb):
+            bmin[3 * i:3 * i + 3] = [int(v) for v in block_mins_xyz[i]]
+            bsz[3 * i:3 * i + 3] = [int(v) for v in block_sizes_xyz[i]]
+        if outs is None:
+            outs = [np.empty(tuple(int(v) for v in s)[::-1], dtype=_out_dtype(params)) for s in block_sizes_xyz]
+        ptrs = (C.c_void_p * max(nb, 1))()
+        on_dev = None
+        for i, o in enumerate(outs):
+            p, d, k = _ptr_of(o)
+            if on_dev is not None and d != on_dev:
+                raise ValueError("all outputs must live on the same side (host or device)")
+            on_dev = d
+            ptrs[i] = p
+            keep.append(k)
+        cpd = (C.c_longlong * 3)(*[int(v) for v in cp_distance])
+        self._check(self.lib.bs_nonrigid_fuse_blocks(self.h, arr, n, nb, bmin, bsz, cpd, C.byref(params), ptrs,
+                                                     1 if on_dev else 0))
+        return outs
+
+    def nonrigid_debug_grid(self, view, block_min_xyz, block_size_xyz, cp_distance=(NONRIGID_CP_DISTANCE,) * 3):
+        """The mapped source coordinate of every control point of one view for one block: float64
+        [gz, gy, gx, 3] ({x, y, z} last); control point (i, j, k) sits at world block_min + ((i, j, k) - 1) * cpd."""
+        arr, _, keep = self.make_nonrigid_views([view])
+        bmin = (C.c_longlong * 3)(*[int(v) for v in block_min_xyz])
+        bsz = (C.c_longlong * 3)(*[int(v) for v in block_size_xyz])
+        cpd = (C.c_longlong * 3)(*[int(v) for v in cp_distance])
+        gd = (C.c_longlong * 3)()
+        self._check(self.lib.bs_nonrigid_debug_grid(self.h, arr, bmin, bsz, cpd, None, gd))
+        out = np.empty((gd[2], gd[1], gd[0], 3), dtype=np.float64)
+        self._check(self.lib.bs_nonrigid_debug_grid(self.h, arr, bmin, bsz, cpd, out.ctypes.data_as(C.POINTER(C.c_double)), gd))
+        return out
 
     @staticmethod
     def comm_unique_id() -> bytes:

@@ -68,7 +68,8 @@ long long bs_launch_count(bs_ctx* ctx);
 /* per-kernel device timing with CUDA events on the context's stream.  Enabling inserts an
  * event pair around every kernel launch; bs_profile_get returns the accumulated milliseconds
  * and launch count for a kernel tag ("fft_x_r2c", "fft_y", "fft_z_xpower", "fft_y_inv",
- * "fft_x_c2r", "peaks", "pearson", "fuse", "content_gauss", "downsample", "median", "sample"). */
+ * "fft_x_c2r", "peaks", "pearson", "fuse", "content_gauss", "downsample", "median", "sample", "mls_grid",
+ * "nonrigid_fuse"). */
 int bs_profile_enable(bs_ctx* ctx, int on);
 int bs_profile_reset(bs_ctx* ctx);
 int bs_profile_get(bs_ctx* ctx, const char* tag, double* ms_total, long long* launches);
@@ -336,6 +337,37 @@ int bs_median_divide(bs_ctx* ctx, unsigned long long vol_handle, int radius, uns
  * imglib2's NLinearInterpolator on FloatType: double weights, each corner term rounded to float and summed in float.
  * out: n floats on the host.  Profile tag "sample". */
 int bs_sample_nlinear(bs_ctx* ctx, unsigned long long vol_handle, int n, const double* loc_xyz, float* out);
+
+/* ---------------------------------------------------------------- nonrigid-fusion (ABI 107)
+ * NonRigidTools.fuseVirtualInterpolatedNonRigid on one super-block (J/SparkNonRigidFusion.java:387-401): per view a
+ * moving-least-squares affine model from target WORLD to local PIXEL coordinates, weights w_i = 1 / |x - t_i|^2
+ * (alpha = 1), evaluated in double at the control points block_min + (k - 1) * cp_distance, k = 0 .. grid_dims - 1,
+ * grid_dims[d] = ceil((block_size[d] - 1) / cp_distance[d]) + 3 (the block plus one cell on every side).  A control
+ * point on a target returns its local point; a view with fewer than 4 points, or a singular fit
+ * (det P <= 1e-10 (trace P / 3)^3 for the weighted, centred second moments P of the targets), uses the inverse of
+ * src_to_world.  Every output voxel trilinearly interpolates the mapped source coordinate of its 8 surrounding control
+ * points, samples the view n-linearly (border extension), weights it with the cosine blending of the view's
+ * blend_border / blend_range at that coordinate and is sum(w I) / sum(w) over the views (0 where sum(w) = 0): AVG_BLEND
+ * with n-linear interpolation only.  Profile tags "mls_grid" and "nonrigid_fuse". */
+typedef struct {
+    bs_view view;                      /* src_to_world: the full-resolution registration; windows as in bs_fuse_blocks */
+    int n_points;
+    int pad;
+    const double* target_world_xyz;    /* n_points x 3: corresponding-point targets, world coordinates */
+    const double* local_xyz;           /* n_points x 3: the same points in the view's full-resolution pixels */
+} bs_nonrigid_view;
+
+/* same block-list form and output conventions as bs_fuse_blocks (out_big_endian included); views in ascending ViewId
+ * order.  BS_ERR_ARG for a fusion_type other than AVG_BLEND, interpolation != 1 or a cp_distance < 1. */
+int bs_nonrigid_fuse_blocks(bs_ctx* ctx, const bs_nonrigid_view* views, int n_views, int n_blocks,
+                            const long long* block_min, const long long* block_size, const long long cp_distance[3],
+                            const bs_fuse_params* params, void* const* outs, int out_on_device);
+
+/* diagnostic: the mapped source coordinate of every control point of one view for one block, host float64
+ * [grid_dims z][y][x][3] ({x, y, z} last), computed by the launch bs_nonrigid_fuse_blocks uses.  grid_dims receives
+ * {gx, gy, gz}; out may be NULL to query the dims.  The view's vol_handle is not used. */
+int bs_nonrigid_debug_grid(bs_ctx* ctx, const bs_nonrigid_view* view, const long long block_min[3],
+                           const long long block_size[3], const long long cp_distance[3], double* out, long long* grid_dims);
 
 #ifdef __cplusplus
 }

@@ -553,3 +553,77 @@ JF(void, sampleNlinear)(JNIEnv* env, jclass, jlong ctx, jlong handle, jdoubleArr
     }
     failed(env, ctx, rc);
 }
+
+// ---------------------------------------------------------------------------------------- nonrigid-fusion
+// views as for fuseBlocks plus nPoints int[n], targets / locals double[3 * sum(nPoints)] (the views' points one after
+// the other, {x, y, z} each); replaces NonRigidTools.fuseVirtualInterpolatedNonRigid (J/SparkNonRigidFusion.java:387-401)
+namespace {
+std::vector<bs_nonrigid_view> unpack_nonrigid(JNIEnv* env, jint n, const std::vector<bs_view>& v, const std::vector<jint>& np,
+                                              jdoubleArray targets, jdoubleArray locals, std::vector<jdouble>& t,
+                                              std::vector<jdouble>& l) {
+    std::vector<bs_nonrigid_view> nv((size_t)n);
+    size_t total = 0;
+    for (jint i = 0; i < n; ++i) total += (size_t)np[(size_t)i];
+    t.assign(total * 3, 0.0);
+    l.assign(total * 3, 0.0);
+    if (total) {
+        env->GetDoubleArrayRegion(targets, 0, (jsize)(total * 3), t.data());
+        env->GetDoubleArrayRegion(locals, 0, (jsize)(total * 3), l.data());
+    }
+    size_t at = 0;
+    for (jint i = 0; i < n; ++i) {
+        memset(&nv[(size_t)i], 0, sizeof(bs_nonrigid_view));
+        nv[(size_t)i].view = v[(size_t)i];
+        nv[(size_t)i].n_points = np[(size_t)i];
+        nv[(size_t)i].target_world_xyz = t.data() + at * 3;
+        nv[(size_t)i].local_xyz = l.data() + at * 3;
+        at += (size_t)np[(size_t)i];
+    }
+    return nv;
+}
+}  // namespace
+
+// cpDistance long[3] (the reference passes 10, 10, 10); dests: Object[] of direct ByteBuffers, one per block
+JF(void, nonrigidFuseBlocks)(JNIEnv* env, jclass, jlong ctx, jint nViews, jdoubleArray models, jlongArray handles,
+                             jfloatArray blend, jlongArray windows, jintArray nPoints, jdoubleArray targets, jdoubleArray locals,
+                             jlongArray blockMins, jlongArray blockSizes, jlongArray cpDistance, jintArray iparams,
+                             jdoubleArray dparams, jobjectArray dests) {
+    std::vector<bs_view> v = unpack_views(env, nViews, models, handles, blend, windows);
+    std::vector<jint> np((size_t)nViews, 0);
+    if (nViews > 0) env->GetIntArrayRegion(nPoints, 0, nViews, np.data());
+    std::vector<jdouble> t, l;
+    std::vector<bs_nonrigid_view> nv = unpack_nonrigid(env, nViews, v, np, targets, locals, t, l);
+    const jsize n = env->GetArrayLength(dests);
+    std::vector<jlong> mnj((size_t)n * 3), szj((size_t)n * 3);
+    env->GetLongArrayRegion(blockMins, 0, n * 3, mnj.data());
+    env->GetLongArrayRegion(blockSizes, 0, n * 3, szj.data());
+    std::vector<long long> mn(mnj.begin(), mnj.end()), sz(szj.begin(), szj.end());
+    std::vector<void*> outs((size_t)n);
+    for (jsize i = 0; i < n; ++i) outs[(size_t)i] = env->GetDirectBufferAddress(env->GetObjectArrayElement(dests, i));
+    long long cpd[3];
+    get3(env, cpDistance, cpd);
+    const bs_fuse_params p = fuse_params(env, iparams, dparams);
+    failed(env, ctx, bs_nonrigid_fuse_blocks(C(ctx), nv.data(), nViews, n, mn.data(), sz.data(), cpd, &p, outs.data(), 0));
+}
+
+// one view: the mapped source coordinate of every control point, double[gz][gy][gx][3]; gridDims (long[3]) receives
+// {gx, gy, gz}
+JF(jdoubleArray, nonrigidDebugGrid)(JNIEnv* env, jclass, jlong ctx, jdoubleArray model, jint nPoints, jdoubleArray targets,
+                                    jdoubleArray locals, jlongArray blockMin, jlongArray blockSize, jlongArray cpDistance,
+                                    jlongArray gridDims) {
+    std::vector<bs_view> v = unpack_views(env, 1, model, nullptr, nullptr, nullptr);
+    std::vector<jdouble> t, l;
+    std::vector<bs_nonrigid_view> nv = unpack_nonrigid(env, 1, v, std::vector<jint>(1, nPoints), targets, locals, t, l);
+    long long mn[3], sz[3], cpd[3], gd[3];
+    get3(env, blockMin, mn);
+    get3(env, blockSize, sz);
+    get3(env, cpDistance, cpd);
+    if (failed(env, ctx, bs_nonrigid_debug_grid(C(ctx), nv.data(), mn, sz, cpd, nullptr, gd))) return nullptr;
+    std::vector<jdouble> out((size_t)gd[0] * gd[1] * gd[2] * 3);
+    if (failed(env, ctx, bs_nonrigid_debug_grid(C(ctx), nv.data(), mn, sz, cpd, out.data(), gd))) return nullptr;
+    jlong g[3] = {gd[0], gd[1], gd[2]};
+    env->SetLongArrayRegion(gridDims, 0, 3, g);
+    jdoubleArray r = env->NewDoubleArray((jsize)out.size());
+    env->SetDoubleArrayRegion(r, 0, (jsize)out.size(), out.data());
+    return r;
+}

@@ -93,4 +93,14 @@ public final class BsNative
 	public static native long medianDivide( long ctx, long handle, int radius );
 	/** n-linear intensities (border extension) at loc = n x {x, y, z} into out: float[n] or a direct ByteBuffer */
 	public static native void sampleNlinear( long ctx, long handle, double[] loc, Object out );
+
+	/** nonrigid-fusion (replaces NonRigidTools.fuseVirtualInterpolatedNonRigid): views as for fuseBlocks plus nPoints[n] and
+	 *  targets / locals = 3 * sum(nPoints) doubles (world targets, full-resolution pixel locations); iparams / dparams as for
+	 *  fuseBlock with fusionType AVG_BLEND and interpolation 1; cpDistance {10, 10, 10} in the reference */
+	public static native void nonrigidFuseBlocks( long ctx, int nViews, double[] models, long[] handles, float[] blend, long[] windows,
+			int[] nPoints, double[] targets, double[] locals, long[] blockMins, long[] blockSizes, long[] cpDistance,
+			int[] iparams, double[] dparams, Object[] dests );
+	/** the MLS-mapped source coordinate of every control point of one view for one block: double[gz][gy][gx][3]; gridDims receives {gx, gy, gz} */
+	public static native double[] nonrigidDebugGrid( long ctx, double[] model, int nPoints, double[] targets, double[] locals,
+			long[] blockMin, long[] blockSize, long[] cpDistance, long[] gridDims );
 }
