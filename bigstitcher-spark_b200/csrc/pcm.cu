@@ -12,6 +12,8 @@
 //   k_fft_col540     forward y FFT of the product
 //                    (other padded y / z sizes than 540: k_fft_strided_pipe / k_fft_xpower_pipe / k_fft_strided)
 //   k_fft_x_c2r      conj + C2R along x, in place -> real PCM (row pitch 2*pitch floats)
+//                    (Px = 540 with at least one tile per SM: k_fft_x_r2c_col540 / k_fft_x_c2r_col540, two lines per
+//                    complex transform)
 //   k_peaks          periodic 6-neighbour local maxima, per-CTA top-K
 //   k_gather27       3x3x3 neighbourhoods of the K peaks (sub-pixel fit runs on the host)
 //   k_pearson_u16    exact integer sums (uint64 atomics) for all surviving wrap candidates, slab-staged image 1
@@ -939,6 +941,248 @@ __global__ void __launch_bounds__(COL540_NT, 1) k_fft_xpower_col540(const __grid
         __syncthreads();
         float2* g = a.a + tile_off(t);
         Col540Q::stage2(XA, [&](const float2 (&w)[20], int, int k1, int c) { Col540Q::store(w, g, a.estride, k1, c); });
+    }
+}
+
+// ------------------------------------------------------------------------------------------
+// x passes of the 540-point plan on Col540, two real lines per complex transform.  A tile's 16 columns are 16
+// line pairs, so one RegFft2<20, 27> tile transform does the work of 32 real 540-point lines.  Stage 2 writes the
+// transform in natural order into Y[c * COL540_XLP + k]; COL540_XLP is odd, so the 16 columns a half-warp writes
+// fall on distinct banks, and the rows read back out of Y are contiguous.
+//
+// 448 threads (14 warps), not the 320 of the y / z passes: each thread holds one of the 432 stage-1 items instead of
+// 112 threads holding two while the other 208 wait at the barrier, and the extra warps hide the shared-memory
+// latency of building the points.  113-116 registers, no spills (the 146-register cap of 448 threads).  At 320 threads
+// the r2c pass took 1.06 ms per bench pair, at 448 0.81 (H100 80GB HBM3, 700 W).
+#define COL540_XLP 541
+#define COL540_SP 546   // c2r: float2 between staged row pairs (2 x 272 + 2: pair c starts 2c banks further on)
+#define COL540X_NT 448
+typedef RegFft2<20, 27, COL540_TC, COL540X_NT> Col540X;
+static_assert(Col540X::IT1 == 1 && Col540X::IT2 == 1, "one item per thread in each stage");
+
+// Forward x pass of uint16 crops.  Column c of tile t is the line position L = 16 t + c (L = zp Py + yp) of both
+// images: z[n] = a[n] + i b[n], with a, b the blended mirrored extension of the two crops' row (the same idx / w rule
+// as k_fft_x_r2c_w).  With Z = FFT540(z) the two half spectra are
+//   A[k] = (Z[k] + conj Z[540 - k]) / 2,   B[k] = (Z[k] - conj Z[540 - k]) / 2i,   k = 0..270.
+// A line whose windowed samples are all zero gets an exactly zero spectrum, as it does from a one-line transform,
+// rather than the partner's rounding noise.  The raw rows of tile t+1 are staged by 16-byte cp.async copies (rows
+// 16-byte aligned) while tile t is transformed.
+// Per tile: stage-1 load from the staged rows, stage 1 into X | barrier | stage 2 into Y | barrier (Y complete, the
+// next tile's rows landed) | separation and whole-row stores from Y.
+struct XR2CCol540Args {
+    XR2CArgs x;
+    int row_bytes;    // dx * 2, a multiple of 16
+    int raw_stride;   // bytes between staged rows: row_bytes padded so that 16 rows fall on 8 different banks
+    int n_tiles;      // ceil(Py * Pz / 16)
+};
+
+__global__ void __launch_bounds__(COL540X_NT, 1) k_fft_x_r2c_col540(const __grid_constant__ XR2CCol540Args P) {
+    const XR2CArgs& a = P.x;
+    constexpr int TC = COL540_TC, N = Col540X::N, pitch = 272;
+    float2* X = bs_sm;
+    float2* Y = X + Col540X::XSIZE;
+    float2* tw = Y + TC * COL540_XLP;
+    int2* xw = reinterpret_cast<int2*>(tw + N);   // (idx_x, w_x bits) per padded x position
+    int* nz = reinterpret_cast<int*>(xw + N);     // [buffer][image][16 lines]: the windowed line has a nonzero sample
+    unsigned char* raw = reinterpret_cast<unsigned char*>(nz + 4 * TC);   // [buffer][image][16 lines][raw_stride]
+    const int n_lines = a.Py * a.Pz;
+    const int chunks = P.row_bytes >> 4;
+    // all threads: stage the rows of tile t into raw buffer b.  TPR threads per (image, line) row, so each thread
+    // looks up one source row per tile (the memory clobber of each copy would serialise per-chunk lookups); all-zero
+    // lines are not read, so not copied.
+    constexpr int TPR = COL540X_NT / (2 * TC);
+    static_assert(COL540X_NT % (2 * TC) == 0, "whole rows per thread group");
+    auto stage = [&](int t, int b) {
+        const int im = threadIdx.x / (TPR * TC), l = (threadIdx.x / TPR) % TC;
+        const int L = t * TC + l;
+        const int zp = L / a.Py, yp = L - zp * a.Py;
+        if (L < n_lines && zp < a.Ez && yp < a.Ey) {
+            const size_t row = (size_t)__ldg(a.idx_z + zp) * a.dy + __ldg(a.idx_y + yp);
+            const unsigned char* src = reinterpret_cast<const unsigned char*>(a.img[im]) + row * P.row_bytes;
+            unsigned char* dst = raw + ((size_t)(b * 2 + im) * TC + l) * P.raw_stride;
+            for (int ch = threadIdx.x % TPR; ch < chunks; ch += TPR) cp_async16(dst + ch * 16, src + ch * 16);
+        }
+        cp_async_commit();
+    };
+    for (int i = threadIdx.x; i < N; i += COL540X_NT) {
+        tw[i] = a.tw[i];
+        xw[i] = make_int2(a.idx_x[i], __float_as_int(a.w_x[i]));
+    }
+    if (threadIdx.x < 4 * TC) nz[threadIdx.x] = 0;
+    int t = blockIdx.x;
+    if (t < P.n_tiles) stage(t, 0);
+    cp_async_wait<0>();
+    __syncthreads();
+    const int c = threadIdx.x % TC;   // this thread's column in both of its stage-1 items and its stage-2 item
+    for (int it = 0; t < P.n_tiles; t += gridDim.x, ++it) {
+        const int b = it & 1;
+        const int L = t * TC + c;
+        const int zp = L / a.Py, yp = L - zp * a.Py;
+        const bool live = L < n_lines && zp < a.Ez && yp < a.Ey;
+        const float wy = live ? __ldg(a.w_y + yp) : 0.f, wz = live ? __ldg(a.w_z + zp) : 0.f;
+        if (t + (int)gridDim.x < P.n_tiles) stage(t + gridDim.x, b ^ 1);   // buffer b^1 was read before the last B1
+        const unsigned short* ra = reinterpret_cast<const unsigned short*>(raw + ((size_t)b * 2 * TC + c) * P.raw_stride);
+        const unsigned short* rb = reinterpret_cast<const unsigned short*>(raw + ((size_t)(b * 2 + 1) * TC + c) * P.raw_stride);
+        Col540X::In v;
+        bool nza = false, nzb = false;
+#pragma unroll
+        for (int u = 0; u < Col540X::IT1; ++u) {
+            if (!Col540X::live1(u)) continue;
+            const int n2 = (threadIdx.x + u * COL540X_NT) / TC;
+#pragma unroll
+            for (int n1 = 0; n1 < 20; ++n1) {
+                float2 z = make_float2(0.f, 0.f);
+                if (live) {
+                    const int2 e = xw[27 * n1 + n2];
+                    const float g = (__int_as_float(e.y) * wy) * wz;
+                    if (g != 0.f) z = make_float2((float)ra[e.x] * g, (float)rb[e.x] * g);
+                }
+                nza |= z.x != 0.f;
+                nzb |= z.y != 0.f;
+                v[u][n1] = z;
+            }
+        }
+        if (nza) nz[(b * 2) * TC + c] = 1;
+        if (nzb) nz[(b * 2 + 1) * TC + c] = 1;
+        Col540X::stage1(v, X, tw);
+        __syncthreads();   // B1: X complete; the previous tile's separation has read Y and nz[b ^ 1] out
+        if (threadIdx.x < 2 * TC) nz[(b ^ 1) * 2 * TC + threadIdx.x] = 0;
+        Col540X::stage2(X, [&](const float2 (&w)[27], int, int k1, int cc) {
+            float2* y = Y + cc * COL540_XLP + k1;
+#pragma unroll
+            for (int k2 = 0; k2 < 27; ++k2) y[20 * k2] = w[k2];
+        });
+        cp_async_wait<0>();
+        __syncthreads();   // B2: Y complete (X free again), this thread's and every other thread's next rows landed
+        for (int j = threadIdx.x; j < TC * pitch; j += COL540X_NT) {
+            const int l = j / pitch, k = j - l * pitch;
+            const int Lj = t * TC + l;
+            if (Lj >= n_lines) break;   // j only grows
+            float2 A = make_float2(0.f, 0.f), B = A;
+            if (k <= N / 2) {
+                const float2 Zk = Y[l * COL540_XLP + k], Zm = Y[l * COL540_XLP + (k ? N - k : 0)];
+                if (nz[(b * 2) * TC + l]) A = make_float2(0.5f * (Zk.x + Zm.x), 0.5f * (Zk.y - Zm.y));
+                if (nz[(b * 2 + 1) * TC + l]) B = make_float2(0.5f * (Zk.y + Zm.y), -0.5f * (Zk.x - Zm.x));
+            }
+            __stcg(a.spec[0] + (size_t)Lj * pitch + k, A);
+            __stcg(a.spec[1] + (size_t)Lj * pitch + k, B);
+        }
+    }
+}
+
+// Inverse x pass, in place: a tile is 32 consecutive spectrum rows (16 pairs of lines), staged by one 1-D bulk copy
+// per pair into rows of COL540_SP float2.  Column c transforms
+//   W[n] = S_2c[n] - i S_2c+1[n],   S[n] = s[n] (n <= 270), conj s[540 - n] (n > 270)
+// for the two stored half spectra s, i.e. conj of Z = X_2c + i X_2c+1 with X = conj s the spectra the pass inverts.
+// FFT(W) = conj(540 ifft(Z)), so with R = FFT(W) the real lines are x_2c = R.x / (Px Py Pz) and
+// x_2c+1 = -R.y / (Px Py Pz).  The imaginary parts of bins 0 and 270 are dropped, as a C2R transform does: they
+// would otherwise leak into the partner line.  A line whose (kept) spectrum is all zero is stored as exact zeros.
+// After stage 1 the staged pair rows are free and stage 2 writes R there
+// in natural order, from which whole output rows are stored.
+struct XC2RCol540Args {
+    XC2RArgs x;
+    int n_tiles;   // ceil(Py * Pz / 32)
+};
+
+__global__ void __launch_bounds__(COL540X_NT, 1) k_fft_x_c2r_col540(const __grid_constant__ XC2RCol540Args P) {
+    const XC2RArgs& a = P.x;
+    constexpr int TC = COL540_TC, N = Col540X::N, M = N / 2, pitch = 272;
+    static_assert(TC * COL540_XLP <= TC * COL540_SP && COL540_SP >= 2 * pitch && COL540_SP % 2 == 0, "pair rows");
+    float2* S0 = bs_sm;   // two staging buffers of TC * COL540_SP (bulk-copy targets: first)
+    float2* X = S0 + 2 * TC * COL540_SP;
+    float2* tw = X + Col540X::XSIZE;
+    int* nz = reinterpret_cast<int*>(tw + N);   // [buffer][32 rows]: the row has a nonzero input
+    unsigned long long* bars = reinterpret_cast<unsigned long long*>(nz + 4 * TC);
+    const int n_lines = a.Py * a.Pz;
+    // warp 0: copy the row pairs of tile t into buffer b, one bulk copy per pair (lane c)
+    auto fetch = [&](int t, int b) {
+        const int rows = min(2 * TC, n_lines - t * 2 * TC);
+        const int lane = threadIdx.x;
+        if (lane == 0) mbar_expect_tx(&bars[b], (unsigned int)(rows * pitch * sizeof(float2)));
+        __syncwarp();
+        const int r0 = 2 * lane;
+        if (lane < TC && r0 < rows) {
+            fence_proxy_async_smem();
+            tma_bulk_g2s(S0 + (size_t)(b * TC + lane) * COL540_SP, a.spec + ((size_t)t * 2 * TC + r0) * pitch,
+                         (unsigned int)(min(2, rows - r0) * pitch * sizeof(float2)), &bars[b]);
+        }
+    };
+    if (threadIdx.x == 0) {
+        mbar_init(&bars[0], 1);
+        mbar_init(&bars[1], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    col540_tw(tw, a.tw);
+    if (threadIdx.x < 4 * TC) nz[threadIdx.x] = 0;
+    __syncthreads();
+    int t = blockIdx.x;
+    if (threadIdx.x < 32 && t < P.n_tiles) fetch(t, 0);
+    const int c = threadIdx.x % TC;
+    const float s = 0.5f * a.scale;   // a.scale = 1 / (M Py Pz)
+    unsigned int phase = 0u;
+    for (int it = 0; t < P.n_tiles; t += gridDim.x, ++it) {
+        const int b = it & 1;
+        float2* Sb = S0 + (size_t)b * TC * COL540_SP;
+        mbar_wait(&bars[b], (phase >> b) & 1u);
+        phase ^= 1u << b;
+        const int r = t * 2 * TC + 2 * c;   // this column's first row
+        const bool la = r < n_lines, lb = r + 1 < n_lines;
+        const float2* sa = Sb + c * COL540_SP;
+        const float2* sb = sa + pitch;
+        Col540X::In v;
+        bool nzp = false, nzq = false;
+#pragma unroll
+        for (int u = 0; u < Col540X::IT1; ++u) {
+            if (!Col540X::live1(u)) continue;
+            const int n2 = (threadIdx.x + u * COL540X_NT) / TC;
+#pragma unroll
+            for (int n1 = 0; n1 < 20; ++n1) {
+                // n = 27 n1 + n2 <= 270 exactly for n1 < 10 and for (n1, n2) = (10, 0)
+                float2 p, q;
+                if (n1 < 10) {
+                    p = sa[27 * n1 + n2];
+                    q = sb[27 * n1 + n2];
+                    if (n1 == 0 && n2 == 0) p.y = q.y = 0.f;
+                } else if (n1 == 10) {
+                    const int m = n2 ? M - n2 : M;
+                    p = sa[m];
+                    q = sb[m];
+                    p.y = n2 ? -p.y : 0.f;
+                    q.y = n2 ? -q.y : 0.f;
+                } else {
+                    p = sa[N - 27 * n1 - n2];
+                    q = sb[N - 27 * n1 - n2];
+                    p.y = -p.y;
+                    q.y = -q.y;
+                }
+                if (!la) p = make_float2(0.f, 0.f);
+                if (!lb) q = make_float2(0.f, 0.f);
+                nzp |= p.x != 0.f || p.y != 0.f;
+                nzq |= q.x != 0.f || q.y != 0.f;
+                v[u][n1] = make_float2(p.x + q.y, p.y - q.x);   // p - i q
+            }
+        }
+        if (nzp) nz[b * 2 * TC + 2 * c] = 1;
+        if (nzq) nz[b * 2 * TC + 2 * c + 1] = 1;
+        Col540X::stage1(v, X, tw);
+        __syncthreads();   // B1: X complete, Sb read out; the previous tile's stores have read S[b^1], nz[b^1] out
+        if (threadIdx.x < 32 && t + (int)gridDim.x < P.n_tiles) fetch(t + gridDim.x, b ^ 1);
+        if (threadIdx.x >= 32 && threadIdx.x < 64) nz[(b ^ 1) * 2 * TC + threadIdx.x - 32] = 0;
+        Col540X::stage2(X, [&](const float2 (&w)[27], int, int k1, int cc) {
+            float2* y = Sb + cc * COL540_XLP + k1;
+#pragma unroll
+            for (int k2 = 0; k2 < 27; ++k2) y[20 * k2] = w[k2];
+        });
+        __syncthreads();   // B2: R complete in Sb (X free again)
+        for (int j = threadIdx.x; j < 2 * TC * M; j += COL540X_NT) {
+            const int rr = j / M, q = j - rr * M;   // output row t * 32 + rr, floats 2q, 2q + 1
+            if (t * 2 * TC + rr >= n_lines) break;
+            const float2* y = Sb + (rr >> 1) * COL540_XLP + 2 * q;
+            const float2 r0 = y[0], r1 = y[1];
+            float2 o = (rr & 1) ? make_float2(-r0.y * s, -r1.y * s) : make_float2(r0.x * s, r1.x * s);
+            if (!nz[b * 2 * TC + rr]) o = make_float2(0.f, 0.f);
+            __stcg(a.spec + ((size_t)t * 2 * TC + rr) * pitch + q, o);
+        }
     }
 }
 
@@ -1876,6 +2120,8 @@ static int pcm_kernel_attrs(bs_ctx* ctx) {
     if ((rc = set_smem(ctx, (const void*)k_fft_col540, 0))) return rc;
     if ((rc = set_smem(ctx, (const void*)k_fft_xpower_col540, 0))) return rc;
     if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r<FftX270>, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_col540, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r_col540, 0))) return rc;
     ctx->pcm_attr_done = true;
     return BS_OK;
 }
@@ -1889,6 +2135,15 @@ static void pass_info(char* info, const char* kernel, const FftPlan* plan) {
     int n = snprintf(info, PCM_INFO_LEN, "%s", kernel);
     for (int i = 0; plan && i < plan->nst && n < PCM_INFO_LEN; ++i)
         n += snprintf(info + n, PCM_INFO_LEN - n, "%s%d", i ? "x" : " ", plan->radix[i]);
+}
+
+// The two-for-one Col540 x kernels (k_fft_x_r2c_col540 / k_fft_x_c2r_col540) run one persistent CTA per SM, so they
+// take over from the warp-private kernels only when a pass has at least one tile per SM; below that the warp kernels
+// spread the lines better.  BS_FFT_X_COL540: 1 (default) applies that rule, 0 never uses them, 2 uses them wherever
+// the geometry allows.
+static bool x_col540(bs_ctx* ctx, const PcmGeometry& g, int tiles) {
+    const int mode = env_int("BS_FFT_X_COL540", 1);
+    return mode && g.P[0] == Col540X::N && env_int("BS_FFT_STATIC", 1) && (mode == 2 || tiles >= ctx->sm_count);
 }
 
 // pass 0: both crops -> blended mirrored extension + zero pad -> R2C along x into ws.spec_a / ws.spec_b
@@ -1921,7 +2176,21 @@ static int pcm_pass_x_r2c(bs_ctx* ctx, const void* d1, const void* d2, int dtype
         const int xmode = env_int("BS_FFT_X_WARP", 1);
         const size_t smem_w = ((size_t)g.P[0] + (size_t)(PCM_THREADS / 32) * 2 * g.M) * sizeof(float2) +
                               (tma_ok ? (size_t)(PCM_THREADS / 32) * (2 * (size_t)row_bytes + 16) : 0);
-        if (xmode && g.M <= 32 * XW_MAXV - 1 && smem_w <= PCM_SMEM_MAX && (((size_t)g.P[0] + 16 * (size_t)g.M) * 8) % 16 == 0) {
+        const int col_tiles = (g.P[1] * g.P[2] + COL540_TC - 1) / COL540_TC;
+        int raw_stride = (row_bytes + 15) & ~15;   // 16 staged rows on 8 different banks: 4 words times an odd number
+        while ((raw_stride / 4) % 8 != 4) raw_stride += 16;
+        const size_t smem_col = (Col540X::XSIZE + (size_t)COL540_TC * COL540_XLP + 2 * (size_t)Col540X::N) * sizeof(float2) +
+                                4 * COL540_TC * (sizeof(int) + (size_t)raw_stride);
+        if (x_col540(ctx, g, col_tiles) && dtype == BS_DTYPE_U16 && (row_bytes % 16) == 0 && ((size_t)d1 % 16) == 0 &&
+            ((size_t)d2 % 16) == 0 && smem_col <= PCM_SMEM_MAX) {
+            XR2CCol540Args c;
+            c.x = a;
+            c.row_bytes = row_bytes;
+            c.raw_stride = raw_stride;
+            c.n_tiles = col_tiles;
+            k_fft_x_r2c_col540<<<std::min(col_tiles, ctx->sm_count), COL540X_NT, smem_col, ctx->stream>>>(c);
+            pass_info(info, "k_fft_x_r2c_col540", nullptr);
+        } else if (xmode && g.M <= 32 * XW_MAXV - 1 && smem_w <= PCM_SMEM_MAX && (((size_t)g.P[0] + 16 * (size_t)g.M) * 8) % 16 == 0) {
             XWArgs w;
             w.x = a;
             w.row_bytes = row_bytes;
@@ -2064,7 +2333,16 @@ static int pcm_pass_x_c2r(bs_ctx* ctx, const PcmGeometry& g, PcmDeviceTables* t,
     {
         bs_launch_scope sc(ctx, "fft_x_c2r");
         const size_t smem_w = ((size_t)g.P[0] + (size_t)(PCM_THREADS / 32) * 2 * (g.M + 1)) * sizeof(float2);
-        if (env_int("BS_FFT_X_WARP", 1) && g.M <= 32 * XW_MAXV - 1 && smem_w <= PCM_SMEM_MAX) {
+        const int col_tiles = (g.P[1] * g.P[2] + 2 * COL540_TC - 1) / (2 * COL540_TC);
+        if (x_col540(ctx, g, col_tiles)) {
+            XC2RCol540Args c;
+            c.x = a;
+            c.n_tiles = col_tiles;
+            const size_t smem = (2 * (size_t)COL540_TC * COL540_SP + Col540X::XSIZE + Col540X::N) * sizeof(float2) +
+                                4 * COL540_TC * sizeof(int) + 2 * sizeof(unsigned long long);
+            k_fft_x_c2r_col540<<<std::min(col_tiles, ctx->sm_count), COL540X_NT, smem, ctx->stream>>>(c);
+            pass_info(info, "k_fft_x_c2r_col540", nullptr);
+        } else if (env_int("BS_FFT_X_WARP", 1) && g.M <= 32 * XW_MAXV - 1 && smem_w <= PCM_SMEM_MAX) {
             const long long n_lines = (long long)g.P[1] * g.P[2];
             const int per_sm = std::max(1, std::min(6, (int)(PCM_SMEM_MAX / (smem_w + 1024))));
             const int nctas = (int)std::min<long long>((n_lines + 7) / 8, (long long)ctx->sm_count * per_sm);
