@@ -7,6 +7,7 @@
   affine_fusion           J/SparkAffineFusion.java:179-800       (s0 + multi-resolution pyramid)
   nonrigid_fusion         J/SparkNonRigidFusion.java:124-446     (MLS grids from interest-point correspondences)
   detect_interestpoints   J/SparkInterestPointDetection.java:173-964 (block-wise DoG, interestpoints.n5 + the XML)
+  match_interestpoints    J/SparkGeometricDescriptorMatching.java:161-545 (PRECISE_TRANSLATION, correspondences)
 
 No argument parsing here (the picocli layer is out of scope); keyword names follow the CLI flags.
 """
@@ -22,6 +23,7 @@ import numpy as np
 from . import fusion as bf
 from . import n5 as bn5
 from . import zarr as bzarr
+from . import matching as bm
 from . import native, stitching as bst
 from .native import Context
 from .spimdata import SpimData2
@@ -890,3 +892,173 @@ def _nonrigid_chunk(ctx, src, chunk, bb_min, fuse, nviews, vdims, params, cpd):
     finally:
         for h in staged:
             ctx.volume_free(h)
+
+
+# --------------------------------------------------------------------------------------------- match-interestpoints
+def match_pairs(view_dims, registrations, view_ids, view_reg="OVERLAPPING_ONLY"):
+    """M2: the view pairs (A, B) of one timepoint, A < B in (tp, setup) order; OVERLAPPING_ONLY keeps the pairs whose
+    closed transformed bounding boxes intersect, ALL_AGAINST_ALL keeps every pair."""
+    vr = view_reg.upper()
+    if vr not in ("OVERLAPPING_ONLY", "ALL_AGAINST_ALL"):
+        raise ValueError(f"-vr {view_reg}")
+    views = sorted(view_ids)
+    boxes = {v: bf.transformed_bounding_box(view_dims[v], registrations[v]) for v in views}
+    pairs = []
+    for i, a in enumerate(views):
+        for b in views[i + 1:]:
+            if a[0] != b[0]:
+                continue
+            if vr == "ALL_AGAINST_ALL" or np.all(np.minimum(boxes[a][1], boxes[b][1]) >= np.maximum(boxes[a][0], boxes[b][0])):
+                pairs.append((a, b))
+    return pairs
+
+
+def match_tasks(pairs, labels, match_across_labels=False):
+    """MatcherPairwiseTools.getTasksList: per pair (A, B) the label tasks (l, l), or every (la, lb) with
+    --matchAcrossLabels; tasks are (viewA, labelA, viewB, labelB)."""
+    out = []
+    for a, b in pairs:
+        if match_across_labels:
+            out += [(a, la, b, lb) for la in labels for lb in labels]
+        else:
+            out += [(a, la, b, la) for la in labels]
+    return out
+
+
+def overlap_filter(world, dims_other, reg_other):
+    """M3 (-ipfr OVERLAPPING_ONLY): mask of the world points inside the other view's closed transformed bounding box."""
+    lo, hi = bf.transformed_bounding_box(dims_other, reg_other)
+    return np.all((world >= lo) & (world <= hi), axis=1)
+
+
+def _match_task(ctx, ips, task, vdims, regs, overlapping_only, significance, search_radius, num_neighbors, redundancy,
+                model, ransac_kw):
+    """One task: descriptors of both point sets on the device, the exhaustive search, the ratio test and RANSAC.
+    Returns the inliers as an int64 (K, 2) array of (id in A, id in B)."""
+    va, la, vb, lb = task
+    empty = np.zeros((0, 2), dtype=np.int64)
+    if (va, la) not in ips.world or (vb, lb) not in ips.world:
+        return empty
+    wa, wb = ips.world[(va, la)], ips.world[(vb, lb)]
+    ia, ib = ips.ids[(va, la)], ips.ids[(vb, lb)]
+    if overlapping_only:
+        ka, kb = overlap_filter(wa, vdims[vb], regs[vb]), overlap_filter(wb, vdims[va], regs[va])
+        wa, ia, wb, ib = wa[ka], ia[ka], wb[kb], ib[kb]
+    ha = ctx.descriptors_build(wa, num_neighbors, redundancy)
+    try:
+        hb = ctx.descriptors_build(wb, num_neighbors, redundancy)
+        try:
+            best_b, best, second = ctx.descriptors_match(ha, hb, search_radius)
+        finally:
+            ctx.descriptors_free(hb)
+    finally:
+        ctx.descriptors_free(ha)
+    cand = bm.ratio_test(best_b, best, second, significance)
+    if len(cand) == 0:
+        return empty
+    pb = np.asarray(best_b)[cand].astype(np.int64)
+    inl, _ = bm.ransac(wa[cand], wb[pb], model, **ransac_kw)
+    return np.stack([ia[cand[inl]], ib[pb[inl]]], axis=1).astype(np.int64) if len(inl) else empty
+
+
+class _MatchPoints:
+    """The points of every (view, label) a matching run needs: ids and world positions (M1, as _InterestPoints)."""
+
+    def __init__(self, store: bn5.N5Store, view_ids, labels, registrations):
+        base = _InterestPoints(store, view_ids, labels, registrations)
+        self.world = base.world
+        self.ids = {k: np.array(sorted(base.index[k], key=base.index[k].get), dtype=np.int64) for k in base.index}
+        self.corr = base.corr
+
+
+def match_interestpoints(xml_path, ctx: Context, labels, method, significance=3.0, search_radius=None, redundancy=1,
+                         num_neighbors=3, clear_correspondences=False, match_across_labels=False,
+                         interestpoints_for_reg="ALL", view_reg="OVERLAPPING_ONLY", transformation_model="AFFINE",
+                         regularization_model="RIGID", regularization_lambda=0.1, ransac_iterations=None,
+                         ransac_max_error=None, ransac_min_inlier_ratio=0.1, ransac_min_num_inliers=12,
+                         ransac_multi_consensus=False, registration_tp="TIMEPOINTS_INDIVIDUALLY", group_tiles=False,
+                         group_illums=False, group_channels=False, split_timepoints=False, view_selection=None,
+                         dry_run=False, shard=(0, 1), allgather=None):
+    """`./match-interestpoints -x dataset.xml -l beads -m PRECISE_TRANSLATION [-s 3.0] [-r 1] [-n 3] [--searchRadius r]
+    [--clearCorrespondences] [--matchAcrossLabels] [-ipfr ALL|OVERLAPPING_ONLY] [-vr OVERLAPPING_ONLY|ALL_AGAINST_ALL]
+    [-tm AFFINE] [-rm RIGID] [--lambda 0.1] [-rit 10000] [-rme 5.0] [-rmir 0.1] [-rmni 12]`, the non-grouped branch of
+    J/SparkGeometricDescriptorMatching.java:161-342 and the save at :512-545: for every task (view pair x label pair)
+    the points are read from interestpoints.n5 and mapped to world (M1), optionally filtered to the partner's box (M3);
+    descriptors and the exhaustive A -> B search run on the device (bs_descriptors_build / bs_descriptors_match), the
+    ratio test (M6), RANSAC and its filter (M7, M8) on the host; the inliers become correspondences of both views (M9),
+    written for every selected view x label unless ``dry_run``.  The XML is not touched.
+    Returns {(viewA, labelA, viewB, labelB): int64 (K, 2) id pairs} for every task.
+
+    Multi-GPU: rank r of w (``shard``) takes tasks[r::w]; ``allgather(obj) -> [obj of every rank]`` merges the results
+    and rank 0 writes.  FAST_ROTATION, FAST_TRANSLATION, ICP, grouping, -rtp other than TIMEPOINTS_INDIVIDUALLY and
+    -rmc raise NotImplementedError."""
+    m = method.upper()
+    if m in ("FAST_ROTATION", "FAST_TRANSLATION", "ICP"):
+        raise NotImplementedError(f"match-interestpoints -m {m} is not implemented")
+    if m != "PRECISE_TRANSLATION":
+        raise ValueError(f"-m {method}")
+    for flag, on in (("--groupTiles", group_tiles), ("--groupIllums", group_illums), ("--groupChannels", group_channels),
+                     ("--splitTimepoints", split_timepoints), ("-rmc", ransac_multi_consensus),
+                     (f"-rtp {registration_tp}", registration_tp.upper() != "TIMEPOINTS_INDIVIDUALLY")):
+        if on:
+            raise NotImplementedError(f"match-interestpoints {flag} is not implemented")
+    ipfr = interestpoints_for_reg.upper()
+    if ipfr not in ("ALL", "OVERLAPPING_ONLY"):
+        raise ValueError(f"-ipfr {interestpoints_for_reg}")
+    k = int(num_neighbors) + int(redundancy)
+    if int(num_neighbors) < 3 or int(redundancy) < 0 or k > native.MATCH_MAX_NEIGHBORS:
+        raise ValueError(f"-n {num_neighbors} -r {redundancy}: need n >= 3, r >= 0, n + r <= {native.MATCH_MAX_NEIGHBORS}")
+    labels = list(labels)
+    if not labels:
+        raise ValueError("no interest point labels given")
+    if ransac_iterations is None:                      # J/SparkGeometricDescriptorMatching.java:180-189
+        ransac_iterations = 10000
+    if ransac_max_error is None:
+        ransac_max_error = 5.0
+    model = bm.Model(transformation_model, regularization_model, regularization_lambda)
+    ransac_kw = dict(iterations=int(ransac_iterations), max_error=float(ransac_max_error),
+                     min_inlier_ratio=float(ransac_min_inlier_ratio), min_num_inliers=int(ransac_min_num_inliers))
+
+    data = SpimData2.load(xml_path)
+    views = sorted(data.select_views(**view_selection) if view_selection else data.view_ids())
+    regs = {v: data.model(*v) for v in views}
+    vdims = {v: tuple(int(d) for d in data.setups[v[1]].size) for v in views}
+    tasks = match_tasks(match_pairs(vdims, regs, views, view_reg), labels, match_across_labels)
+    base = os.path.join(os.path.dirname(os.path.abspath(xml_path)), data.root.findtext("BasePath") or ".")
+    store = bn5.N5Store(os.path.join(base, "interestpoints.n5"))
+    ips = _MatchPoints(store, views, labels, regs)
+
+    rank, world = shard
+    results = {}
+    for task in tasks[rank::world]:
+        results[task] = _match_task(ctx, ips, task, vdims, regs, ipfr == "OVERLAPPING_ONLY", float(significance),
+                                    search_radius, int(num_neighbors), int(redundancy), model, ransac_kw)
+    if world > 1:
+        merged = {}
+        for part in allgather(results):
+            merged.update(part)
+        results = {t: merged[t] for t in tasks if t in merged}
+        if rank != 0:
+            return results
+    if dry_run:
+        return results
+    write_match_correspondences(store, ips, views, labels, results, clear_correspondences)
+    return results
+
+
+def write_match_correspondences(store, ips, views, labels, results, clear=False):
+    """M9: each inlier (idA, idB) of task (A, la, B, lb) adds (idA, B, lb, idB) to (A, la) and (idB, A, la, idA) to
+    (B, lb), appended to the stored rows (replacing them with ``clear``) without duplicates, sorted by (id, partner tp,
+    partner setup, partner label, partner id); every selected view x label that has points is written."""
+    rows = {}
+    for v in views:
+        for lab in labels:
+            if (v, lab) in ips.world:
+                rows[(v, lab)] = set() if clear else {(int(a), tuple(pv), pl, int(b)) for a, pv, pl, b in ips.corr[(v, lab)]}
+    for (va, la, vb, lb), pairs in results.items():
+        for ida, idb in np.asarray(pairs, dtype=np.int64).reshape(-1, 2):
+            rows[(va, la)].add((int(ida), tuple(vb), lb, int(idb)))
+            rows[(vb, lb)].add((int(idb), tuple(va), la, int(ida)))
+    for (v, lab), rs in sorted(rows.items()):
+        ordered = sorted(rs, key=lambda r: (r[0], r[1][0], r[1][1], r[2], r[3]))
+        store.write_correspondences(f"tpId_{v[0]}_viewSetupId_{v[1]}/{lab}", ordered)

@@ -132,6 +132,7 @@ void bs_destroy(bs_ctx* ctx) {
     bs_fuse2_free(ctx);
     bs_dog_free(ctx);
     bs_nonrigid_free(ctx);
+    bs_match_free(ctx);
     bs_comm_free(ctx);
     if (ctx->fuse_ring_dev) cudaFree(ctx->fuse_ring_dev);
     if (ctx->fuse_ring_host) cudaFreeHost(ctx->fuse_ring_host);

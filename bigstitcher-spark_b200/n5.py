@@ -14,6 +14,7 @@ from __future__ import annotations
 import gzip
 import json
 import os
+import shutil
 import struct
 import zlib
 
@@ -254,6 +255,20 @@ class N5Store:
             keys[int(idx)] = ((int(tp), int(setup)), label)
         rows = self.read_list(path + "/data")
         return [(int(a), keys[int(c)][0], keys[int(c)][1], int(b)) for a, b, c in rows]
+
+    def write_correspondences(self, group, rows):
+        """The inverse of read_correspondences: ``rows`` [(detection id, (tp, setup), label, corresponding detection id)]
+        become group attributes correspondences = "1.0.0" and idMap {"tp,setup,label": index} (numbered in sorted key
+        order) and the zstd uint64 dataset `correspondences/data` {3, M} in the given row order; {0} when empty.  An
+        earlier `correspondences` group is replaced."""
+        path = group.rstrip("/") + "/correspondences"
+        keys = sorted({(tuple(int(x) for x in pv), str(pl)) for _, pv, pl, _ in rows})
+        idmap = {f"{pv[0]},{pv[1]},{pl}": i for i, (pv, pl) in enumerate(keys)}
+        shutil.rmtree(os.path.join(self.root, path), ignore_errors=True)
+        self.set_attributes(path, {"correspondences": "1.0.0", "idMap": idmap})
+        data = np.array([(int(a), int(b), idmap[f"{int(pv[0])},{int(pv[1])},{pl}"]) for a, pv, pl, b in rows],
+                        dtype=np.uint64).reshape(-1, 3)
+        self.write_list(path + "/data", data, 300000, "zstd")
 
     def write_volume(self, path, volume: np.ndarray, block_size, compression="raw"):
         self.create_dataset(path, volume.shape[::-1], block_size, volume.dtype, compression)

@@ -114,10 +114,14 @@ SYMBOLS = [
     "bs_fuse_block_to_volume", "bs_fuse_accumulate", "bs_fuse_finish", "bs_mask_blocks", "bs_dog_default_params", "bs_dog_detect",
     "bs_dog_debug_dog", "bs_comm_unique_id", "bs_comm_init", "bs_comm_destroy", "bs_fuse_allreduce",
     "bs_downsample_float", "bs_median_divide", "bs_sample_nlinear", "bs_nonrigid_fuse_blocks", "bs_nonrigid_debug_grid",
+    "bs_descriptors_build", "bs_descriptors_free", "bs_descriptors_neighbors", "bs_descriptors_match",
 ]
 
 #: fixed parameters of the reference's non-rigid fusion (J/SparkNonRigidFusion.java:373-383): control-point distance
 NONRIGID_CP_DISTANCE = 10
+
+#: largest num_neighbors + redundancy bs_descriptors_build accepts (BS_MATCH_MAX_NEIGHBORS in include/bsgpu.h)
+MATCH_MAX_NEIGHBORS = 6
 
 #: largest --medianFilter radius bs_median_divide accepts (BS_MEDIAN_MAX_RADIUS in include/bsgpu.h)
 MEDIAN_MAX_RADIUS = 32
@@ -188,6 +192,10 @@ def load_library():
     lib.bs_sample_nlinear.argtypes = [vp, ull, ip, P(dbl), vp]
     lib.bs_nonrigid_fuse_blocks.argtypes = [vp, P(NonrigidViewC), ip, ip, P(ll), P(ll), P(ll), P(FuseParamsC), P(vp), ip]
     lib.bs_nonrigid_debug_grid.argtypes = [vp, P(NonrigidViewC), P(ll), P(ll), P(ll), P(dbl), P(ll)]
+    lib.bs_descriptors_build.argtypes = [vp, P(dbl), ip, ip, ip, P(ull)]
+    lib.bs_descriptors_free.argtypes = [vp, ull]
+    lib.bs_descriptors_neighbors.argtypes = [vp, ull, P(ip), P(dbl)]
+    lib.bs_descriptors_match.argtypes = [vp, ull, ull, dbl, P(ip), P(dbl), P(dbl)]
     _lib = lib
     return lib
 
@@ -232,6 +240,7 @@ class Context:
             raise BsError(rc, self.lib.bs_last_error(None).decode())
         self.h = h
         self.device = device
+        self._desc_shape = {}      # descriptor handle -> (n, k)
 
     # -- plumbing
     def _check(self, rc):
@@ -696,6 +705,43 @@ class Context:
         out = np.empty((gd[2], gd[1], gd[0], 3), dtype=np.float64)
         self._check(self.lib.bs_nonrigid_debug_grid(self.h, arr, bmin, bsz, cpd, out.ctypes.data_as(C.POINTER(C.c_double)), gd))
         return out
+
+    # -- match-interestpoints
+    def descriptors_build(self, xyz, num_neighbors=3, redundancy=1) -> int:
+        """Resident local descriptors of (n, 3) float64 world points: every point's num_neighbors + redundancy nearest
+        other points in (squared distance, index) order, kept as relative vectors (include/bsgpu.h)."""
+        p = np.ascontiguousarray(np.asarray(xyz, dtype=np.float64).reshape(-1, 3))
+        h = C.c_ulonglong()
+        self._check(self.lib.bs_descriptors_build(self.h, p.ctypes.data_as(C.POINTER(C.c_double)), len(p),
+                                                  int(num_neighbors), int(redundancy), C.byref(h)))
+        self._desc_shape[h.value] = (len(p), int(num_neighbors) + int(redundancy))
+        return h.value
+
+    def descriptors_neighbors(self, handle: int):
+        """(idx int32 (n, k), d2 float64 (n, k)) of a descriptor set; -1 / inf everywhere when n <= k."""
+        n, k = self._desc_shape[handle]
+        idx = np.empty((n, k), dtype=np.int32)
+        d2 = np.empty((n, k), dtype=np.float64)
+        self._check(self.lib.bs_descriptors_neighbors(self.h, handle, idx.ctypes.data_as(C.POINTER(C.c_int)),
+                                                      d2.ctypes.data_as(C.POINTER(C.c_double))))
+        return idx, d2
+
+    def descriptors_match(self, ha: int, hb: int, search_radius=None):
+        """Exhaustive descriptor search A -> B: (best_b int32 (nA,), best float64, second float64); best_b = -1 where no
+        point of B qualifies.  ``search_radius`` None: every point of B."""
+        n = self._desc_shape[ha][0]
+        best_b = np.empty(n, dtype=np.int32)
+        best = np.empty(n, dtype=np.float64)
+        second = np.empty(n, dtype=np.float64)
+        r = -1.0 if search_radius is None else float(search_radius)
+        self._check(self.lib.bs_descriptors_match(self.h, ha, hb, r, best_b.ctypes.data_as(C.POINTER(C.c_int)),
+                                                  best.ctypes.data_as(C.POINTER(C.c_double)),
+                                                  second.ctypes.data_as(C.POINTER(C.c_double))))
+        return best_b, best, second
+
+    def descriptors_free(self, handle: int):
+        self._check(self.lib.bs_descriptors_free(self.h, handle))
+        self._desc_shape.pop(handle, None)
 
     @staticmethod
     def comm_unique_id() -> bytes:

@@ -369,6 +369,28 @@ int bs_nonrigid_fuse_blocks(bs_ctx* ctx, const bs_nonrigid_view* views, int n_vi
 int bs_nonrigid_debug_grid(bs_ctx* ctx, const bs_nonrigid_view* view, const long long block_min[3],
                            const long long block_size[3], const long long cp_distance[3], double* out, long long* grid_dims);
 
+/* ---------------------------------------------------------------- match-interestpoints
+ * The two quadratic steps of PRECISE_TRANSLATION matching, RGLDMPairwise (J/SparkGeometricDescriptorMatching.java:594-605):
+ * the local descriptors of each point set and the exhaustive descriptor search from A to B, both in FP64.  The ratio test,
+ * RANSAC and the model fits stay on the host.  These entry points are additive: the ABI version stays 107. */
+#define BS_MATCH_MAX_NEIGHBORS 6   /* num_neighbors + redundancy */
+
+/* resident local descriptors of one point set (world coordinates, n x 3 doubles {x,y,z}): for every point p its
+ * k = num_neighbors + redundancy nearest OTHER points, ordered by (squared distance, index), kept as the relative
+ * vectors q_j - p in double.  3 <= num_neighbors, 0 <= redundancy, k <= BS_MATCH_MAX_NEIGHBORS, else BS_ERR_ARG.
+ * n <= k is legal: the set has no descriptors.  Profile tag "knn". */
+int bs_descriptors_build(bs_ctx* ctx, const double* xyz, int n, int num_neighbors, int redundancy, unsigned long long* handle);
+int bs_descriptors_free(bs_ctx* ctx, unsigned long long handle);
+/* diagnostic: neighbour indices [n][k] and squared distances [n][k] of bs_descriptors_build (-1 / +inf when n <= k) */
+int bs_descriptors_neighbors(bs_ctx* ctx, unsigned long long handle, int* idx, double* d2);
+/* for every point a of A: over the points b of B (only |p_b - p_a| <= search_radius when search_radius >= 0),
+ * D(a, b) = min over the C(k,n)^2 pairs of neighbour subsets (s of a, t of b) of sum_j |u_{s_j} - v_{t_j}|^2;
+ * best_b = argmin (ties -> lower b), best = D(a, best_b), second = min over b != best_b (+inf when none);
+ * best_b = -1 when no b qualifies.  A and B must share (num_neighbors, redundancy).  Subsets are taken in lexicographic
+ * order of neighbour rank, each in ascending-distance order.  Profile tag "desc_match". */
+int bs_descriptors_match(bs_ctx* ctx, unsigned long long ha, unsigned long long hb, double search_radius,
+                         int* best_b, double* best, double* second);
+
 #ifdef __cplusplus
 }
 #endif

@@ -627,3 +627,44 @@ JF(jdoubleArray, nonrigidDebugGrid)(JNIEnv* env, jclass, jlong ctx, jdoubleArray
     env->SetDoubleArrayRegion(r, 0, (jsize)out.size(), out.data());
     return r;
 }
+
+// ---------------------------------------------------------------------------------------- match-interestpoints
+// the two quadratic steps of RGLDMPairwise (J/SparkGeometricDescriptorMatching.java:594-605); xyz: double[3n] world
+// coordinates {x, y, z} per point
+JF(jlong, descriptorsBuild)(JNIEnv* env, jclass, jlong ctx, jdoubleArray xyz, jint numNeighbors, jint redundancy) {
+    const jint n = env->GetArrayLength(xyz) / 3;
+    std::vector<jdouble> p((size_t)n * 3);
+    if (n > 0) env->GetDoubleArrayRegion(xyz, 0, n * 3, p.data());
+    unsigned long long h = 0;
+    return failed(env, ctx, bs_descriptors_build(C(ctx), p.data(), n, numNeighbors, redundancy, &h)) ? 0 : (jlong)h;
+}
+
+JF(void, descriptorsFree)(JNIEnv* env, jclass, jlong ctx, jlong handle) {
+    failed(env, ctx, bs_descriptors_free(C(ctx), (unsigned long long)handle));
+}
+
+// idx: long[n * k], d2: double[n * k] (k = numNeighbors + redundancy of the set)
+JF(void, descriptorsNeighbors)(JNIEnv* env, jclass, jlong ctx, jlong handle, jlongArray idx, jdoubleArray d2) {
+    const jsize m = env->GetArrayLength(idx);
+    std::vector<int> i((size_t)m);
+    std::vector<jdouble> d((size_t)m);
+    if (failed(env, ctx, bs_descriptors_neighbors(C(ctx), (unsigned long long)handle, i.data(), d.data()))) return;
+    const std::vector<jlong> il(i.begin(), i.end());
+    env->SetLongArrayRegion(idx, 0, m, il.data());
+    env->SetDoubleArrayRegion(d2, 0, m, d.data());
+}
+
+// per point of A: bestB long[nA], best / second double[nA]; searchRadius < 0: unlimited
+JF(void, descriptorsMatch)(JNIEnv* env, jclass, jlong ctx, jlong ha, jlong hb, jdouble searchRadius, jlongArray bestB,
+                           jdoubleArray best, jdoubleArray second) {
+    const jsize n = env->GetArrayLength(bestB);
+    std::vector<int> bi((size_t)n);
+    std::vector<jdouble> b((size_t)n), s((size_t)n);
+    if (failed(env, ctx, bs_descriptors_match(C(ctx), (unsigned long long)ha, (unsigned long long)hb, searchRadius, bi.data(),
+                                              b.data(), s.data())))
+        return;
+    const std::vector<jlong> bl(bi.begin(), bi.end());
+    env->SetLongArrayRegion(bestB, 0, n, bl.data());
+    env->SetDoubleArrayRegion(best, 0, n, b.data());
+    env->SetDoubleArrayRegion(second, 0, n, s.data());
+}

@@ -103,4 +103,14 @@ public final class BsNative
 	/** the MLS-mapped source coordinate of every control point of one view for one block: double[gz][gy][gx][3]; gridDims receives {gx, gy, gz} */
 	public static native double[] nonrigidDebugGrid( long ctx, double[] model, int nPoints, double[] targets, double[] locals,
 			long[] blockMin, long[] blockSize, long[] cpDistance, long[] gridDims );
+
+	/** match-interestpoints (replaces the descriptor steps of RGLDMPairwise): resident local descriptors of n world points
+	 *  xyz = n x {x, y, z}; k = numNeighbors + redundancy <= 6 nearest other points per point */
+	public static native long descriptorsBuild( long ctx, double[] xyz, int numNeighbors, int redundancy );
+	public static native void descriptorsFree( long ctx, long handle );
+	/** neighbour indices idx[n * k] and squared distances d2[n * k] of a descriptor set (-1 / +inf when n <= k) */
+	public static native void descriptorsNeighbors( long ctx, long handle, long[] idx, double[] d2 );
+	/** exhaustive search A -> B: per point of A the best B index (-1: none), its descriptor distance and the second best;
+	 *  searchRadius < 0: unlimited */
+	public static native void descriptorsMatch( long ctx, long ha, long hb, double searchRadius, long[] bestB, double[] best, double[] second );
 }
