@@ -1467,35 +1467,79 @@ __device__ __forceinline__ void prs_stage(const PearsonU16Args& a, int s, long l
     if (lane < 16 && e < (lane < 8 ? min(b0, e1) : e1)) buf[PRS_PAD + (e - a0)] = a.img1[e];
 }
 
-__device__ __forceinline__ void prs_acc(const unsigned int A[4], const unsigned int B[4], unsigned int& sa, unsigned int& sb,
-                                        unsigned long long& saa, unsigned long long& sbb, unsigned long long& sab) {
+// One lane's exact sums of one candidate.  The products go through the 2-way dot product IDP.2A (16-bit x 8-bit
+// pairs into 32 bits): with b = b_lo + 256 b_hi, a * b = a * b_lo + 256 a * b_hi, so each product sum is kept as two
+// uint32 partials p_lo + 256 p_hi.  One IDP adds at most 2 * 65535 * 255 = 33,422,850, so a partial holds 128 of
+// them (4,278,124,800 < 2^32): 32 chunks of 8 elements (4 IDPs per partial each) between folds into uint64.
+// sa / sb take one IDP against 0x0101 per word (bounded in prs_flush).
+struct PrsAcc {
+    unsigned int sa, sb;
+    unsigned int aal, aah, bbl, bbh, abl, abh;
+};
+#define PRS_FOLD_CHUNKS 32        // chunks per lane between folds of the uint32 partials
+
+__device__ __forceinline__ void prs_acc(const unsigned int A[4], const unsigned int B[4], PrsAcc& s) {
 #pragma unroll
     for (int m = 0; m < 4; ++m) {
-        const unsigned int a0 = A[m] & 0xffffu, a1 = A[m] >> 16, b0 = B[m] & 0xffffu, b1 = B[m] >> 16;
-        sa += a0 + a1;
-        sb += b0 + b1;
-        saa += (unsigned long long)a0 * a0;   // IMAD.WIDE.U32 with 64-bit accumulate each
-        saa += (unsigned long long)a1 * a1;
-        sbb += (unsigned long long)b0 * b0;
-        sbb += (unsigned long long)b1 * b1;
-        sab += (unsigned long long)a0 * b0;
-        sab += (unsigned long long)a1 * b1;
+        // [x0 | x1] (two uint16) -> bytes [x0 lo, x1 lo, x0 hi, x1 hi]: _lo pairs with the low bytes, _hi the high
+        const unsigned int Ap = __byte_perm(A[m], 0u, 0x3120), Bp = __byte_perm(B[m], 0u, 0x3120);
+        s.sa = __dp2a_lo(A[m], 0x0101u, s.sa);
+        s.sb = __dp2a_lo(B[m], 0x0101u, s.sb);
+        s.aal = __dp2a_lo(A[m], Ap, s.aal);
+        s.aah = __dp2a_hi(A[m], Ap, s.aah);
+        s.bbl = __dp2a_lo(B[m], Bp, s.bbl);
+        s.bbh = __dp2a_hi(B[m], Bp, s.bbh);
+        s.abl = __dp2a_lo(A[m], Bp, s.abl);
+        s.abh = __dp2a_hi(A[m], Bp, s.abh);
     }
+}
+
+// Fold the lanes' partials into uint64, add the warp's total to the candidate's shared-memory sums and restart the
+// partials (warp-uniform).  Between flushes the warp covers at most 32 * PRS_FOLD_CHUNKS chunks (see prs_row), so its
+// sa / sb stay below 8192 elements * 65535 < 2^32.
+__device__ __forceinline__ void prs_flush(PrsAcc& s, unsigned long long* acc, int lane) {
+    unsigned int sa = s.sa, sb = s.sb;
+    unsigned long long saa = s.aal + ((unsigned long long)s.aah << 8), sbb = s.bbl + ((unsigned long long)s.bbh << 8),
+                       sab = s.abl + ((unsigned long long)s.abh << 8);
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        sa += __shfl_xor_sync(0xffffffffu, sa, off);
+        sb += __shfl_xor_sync(0xffffffffu, sb, off);
+        saa += __shfl_xor_sync(0xffffffffu, saa, off);
+        sbb += __shfl_xor_sync(0xffffffffu, sbb, off);
+        sab += __shfl_xor_sync(0xffffffffu, sab, off);
+    }
+    if (lane == 0) {
+        if (sa) atomicAdd(acc + 0, (unsigned long long)sa);
+        if (sb) atomicAdd(acc + 1, (unsigned long long)sb);
+        if (saa) atomicAdd(acc + 2, saa);
+        if (sbb) atomicAdd(acc + 3, sbb);
+        if (sab) atomicAdd(acc + 4, sab);
+    }
+    s = PrsAcc{0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
 }
 
 // One image-2 row segment of one candidate, owned by a warp.  Chunk k covers image-2 elements g + 8k .. g + 8k + 7
 // (g 16-byte aligned); elements lo .. hi - 1 of the chunk sequence belong to the segment.  s1 points at the staged
 // image-1 element paired with chunk 0's first element, rounded down to 16 bytes; SH is the rounding (0..7).
 // Chunks k >= kvec reach past the end of image 2 and are loaded element by element.
+// A round takes one chunk per lane, and the row's last round up to two (its loads in flight before the arithmetic),
+// so a segment of up to 64 chunks costs one round trip to image 2.  A lane takes ceil(nch / 32) chunks of the row.
+// Segments of more than 32 * PRS_FOLD_CHUNKS = 1024 chunks (hi > 8192) fold every PRS_FOLD_CHUNKS - 1 rounds, which
+// with a last round of two leaves at most PRS_FOLD_CHUNKS chunks per lane between folds.  Their rows are over 8185
+// elements wide, so a slab holds at most 2 rows (slab_rows = PRS_STAGE_ELEMS / dx) and the warp owns only this one:
+// the partials enter it at zero and leave it with at most PRS_FOLD_CHUNKS chunks per lane.  Everything else folds once per candidate in the caller:
+// with slab_rows <= 8 a warp owns one row of <= 1024 chunks, with 9-16 two rows of <= 1820 elements and with 17-32
+// four rows of <= 963 elements, <= 32 chunks per lane in every case.
 template <int SH>
 __device__ __forceinline__ void prs_row(const unsigned short* __restrict__ g, const unsigned short* s1, int lo, int hi,
-                                        int nch, int kvec, int lane, unsigned int& sa, unsigned int& sb,
-                                        unsigned long long& saa, unsigned long long& sbb, unsigned long long& sab) {
-    for (int k0 = lane; k0 < nch; k0 += 64) {
+                                        int nch, int kvec, int lane, PrsAcc& s, unsigned long long* acc) {
+    for (int kb = 0, r = 1; kb < nch; kb += 32, ++r) {   // warp-uniform rounds
+        const bool last = nch - kb <= 64;
         uint4 v[2];
 #pragma unroll
-        for (int u = 0; u < 2; ++u) {        // both chunks' loads in flight before any arithmetic
-            const int k = k0 + 32 * u;
+        for (int u = 0; u < 2; ++u) {
+            const int k = (u == 0 || last) ? kb + lane + 32 * u : nch;
             v[u] = make_uint4(0u, 0u, 0u, 0u);
             if (k < kvec) {
                 v[u] = ldg_stream16(g + 8 * k);
@@ -1511,7 +1555,7 @@ __device__ __forceinline__ void prs_row(const unsigned short* __restrict__ g, co
         }
 #pragma unroll
         for (int u = 0; u < 2; ++u) {
-            const int k = k0 + 32 * u;
+            const int k = (u == 0 || last) ? kb + lane + 32 * u : nch;
             if (k >= nch) break;
             const uint4 p = *reinterpret_cast<const uint4*>(s1 + 8 * k);
             const uint4 q = *reinterpret_cast<const uint4*>(s1 + 8 * k + 8);
@@ -1530,8 +1574,10 @@ __device__ __forceinline__ void prs_row(const unsigned short* __restrict__ g, co
                     B[m] &= mk;
                 }
             }
-            prs_acc(A, B, sa, sb, saa, sbb, sab);
+            prs_acc(A, B, s);
         }
+        if (last) break;
+        if (r % (PRS_FOLD_CHUNKS - 1) == 0) prs_flush(s, acc, lane);
     }
 }
 
@@ -1575,15 +1621,6 @@ __global__ void __launch_bounds__(PCM_THREADS, 3) k_pearson_u16(const __grid_con
         const int nr = (int)min((long long)a.slab_rows, nrows - r0);
         const int z0 = (int)(r0 / a.dy), y0 = (int)(r0 - (long long)z0 * a.dy);
         const int zl = (int)((r0 + nr - 1) / a.dy);
-        // (y, z) of this warp's rows wid, wid + NW, ...
-        int ry[RPW], rz[RPW];
-#pragma unroll
-        for (int j = 0; j < RPW; ++j) {
-            int y = y0 + wid + j * NW, z = z0;
-            while (y >= a.dy) { y -= a.dy; ++z; }
-            ry[j] = y;
-            rz[j] = z;
-        }
         // staged image-1 element e0 + i (e0 = r0 * dx, the slab's first) sits at sbuf[soff + i]
         const unsigned short* sbuf = stage + (size_t)buf * a.stage_elems;
         const int soff = PRS_PAD + (int)((r0 * a.dx) & 7);
@@ -1591,13 +1628,16 @@ __global__ void __launch_bounds__(PCM_THREADS, 3) k_pearson_u16(const __grid_con
         for (int c = 0; c < ncand; ++c) {
             const PearsonCand cd = s_cand[c];
             if (zl < cd.o1[2] || z0 >= cd.o1[2] + cd.sz[2]) continue;   // block-uniform
-            unsigned int sa = 0, sb = 0;
-            unsigned long long saa = 0, sbb = 0, sab = 0;
+            PrsAcc acc = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
             bool any = false;
-#pragma unroll
+            // not unrolled: the 8 alignment cases of prs_row are inlined once each, not once per row (instruction
+            // cache)
+#pragma unroll 1
             for (int j = 0; j < RPW; ++j) {
                 const int rr = wid + j * NW;
-                const int yy = ry[j] - cd.o1[1], zz = rz[j] - cd.o1[2];
+                int y = y0 + rr, z = z0;   // (y, z) of slab row rr
+                while (y >= a.dy) { y -= a.dy; ++z; }
+                const int yy = y - cd.o1[1], zz = z - cd.o1[2];
                 if (rr >= nr || yy < 0 || yy >= cd.sz[1] || zz < 0 || zz >= cd.sz[2]) continue;
                 any = true;
                 const long long g2 = ((long long)(zz + cd.o2[2]) * a.dy + (yy + cd.o2[1])) * a.dx + cd.o2[0];
@@ -1610,34 +1650,17 @@ __global__ void __launch_bounds__(PCM_THREADS, 3) k_pearson_u16(const __grid_con
                 const unsigned short* s1 = sbuf + (t & ~7);
                 const unsigned short* g = a.img2 + c2;
                 switch (t & 7) {
-                    case 0: prs_row<0>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
-                    case 1: prs_row<1>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
-                    case 2: prs_row<2>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
-                    case 3: prs_row<3>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
-                    case 4: prs_row<4>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
-                    case 5: prs_row<5>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
-                    case 6: prs_row<6>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
-                    default: prs_row<7>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
+                    case 0: prs_row<0>(g, s1, lo, hi, nch, kvec, lane, acc, s_acc + 5 * c); break;
+                    case 1: prs_row<1>(g, s1, lo, hi, nch, kvec, lane, acc, s_acc + 5 * c); break;
+                    case 2: prs_row<2>(g, s1, lo, hi, nch, kvec, lane, acc, s_acc + 5 * c); break;
+                    case 3: prs_row<3>(g, s1, lo, hi, nch, kvec, lane, acc, s_acc + 5 * c); break;
+                    case 4: prs_row<4>(g, s1, lo, hi, nch, kvec, lane, acc, s_acc + 5 * c); break;
+                    case 5: prs_row<5>(g, s1, lo, hi, nch, kvec, lane, acc, s_acc + 5 * c); break;
+                    case 6: prs_row<6>(g, s1, lo, hi, nch, kvec, lane, acc, s_acc + 5 * c); break;
+                    default: prs_row<7>(g, s1, lo, hi, nch, kvec, lane, acc, s_acc + 5 * c); break;
                 }
             }
-            if (!any) continue;  // warp-uniform
-            // per-warp partials: sa, sb < slab elements * 65535 < 2^32
-#pragma unroll
-            for (int off = 16; off > 0; off >>= 1) {
-                sa += __shfl_xor_sync(0xffffffffu, sa, off);
-                sb += __shfl_xor_sync(0xffffffffu, sb, off);
-                saa += __shfl_xor_sync(0xffffffffu, saa, off);
-                sbb += __shfl_xor_sync(0xffffffffu, sbb, off);
-                sab += __shfl_xor_sync(0xffffffffu, sab, off);
-            }
-            if (lane == 0) {
-                unsigned long long* acc = s_acc + 5 * c;
-                if (sa) atomicAdd(acc + 0, (unsigned long long)sa);
-                if (sb) atomicAdd(acc + 1, (unsigned long long)sb);
-                if (saa) atomicAdd(acc + 2, saa);
-                if (sbb) atomicAdd(acc + 3, sbb);
-                if (sab) atomicAdd(acc + 4, sab);
-            }
+            if (any) prs_flush(acc, s_acc + 5 * c, lane);   // warp-uniform
         }
         __syncthreads();   // every warp is done with this buffer before it is refilled
     }

@@ -5,16 +5,22 @@
 //   (r) a plain 16-byte read of both volumes (the card's streaming-read bandwidth);
 //   (a) the previous traversal (k_pearson's old uint16 path);
 //   (b) the slab-staged traversal of k_pearson_u16 with the arithmetic replaced by one XOR per word;
-//   (c) (b) plus the exact sums, i.e. k_pearson_u16 itself, at several slab heights and chunks per lane per round.
+//   (c) (b) plus the exact sums taken the previous way (three 64-bit multiply-accumulates per element);
+//   (d) (b) plus the exact sums from packed 16 x 8-bit dot products (IDP.2A) into 32-bit partials;
+//   (e) (d) with the loop over a warp's rows not unrolled, and optionally one more chunk per lane in a row's last
+//       round; "as built" is k_pearson_u16 itself.
+// (c) and (d) at several slab heights and chunks per lane per round (U).
 // "DRAM" bytes are the slab design's traffic: image 1 once plus image 2 once per candidate box (2 n + 2 sum npx).
-// (c)'s sums are checked against (a)'s.  (b) / (c) are a copy of k_pearson_u16 from csrc/pcm.cu with the arithmetic
-// and the chunks per lane as template parameters; keep them in step when the kernel changes.
+// (c) - (e)'s sums are checked against (a)'s.  (b) - (e) are a copy of k_pearson_u16 from csrc/pcm.cu with the
+// arithmetic, the chunks per lane and the row loop's unrolling as template parameters; keep them in step when the
+// kernel changes.
 //   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a pearson_probe.cu -o pearson_probe && ./pearson_probe
 #include <cuda_runtime.h>
 #include <algorithm>
 #include <cstdio>
 #include <cstring>
 #include <random>
+#include <type_traits>
 #include <vector>
 
 #define NT 256
@@ -155,8 +161,8 @@ __global__ void __launch_bounds__(NT) k_old(const __grid_constant__ PearsonArgs 
         if (s_u[i]) atomicAdd(sums + i, s_u[i]);
 }
 
-// (b) / (c): the slab-staged traversal of k_pearson_u16 (csrc/pcm.cu), with the arithmetic switchable (SUMS) and
-// U chunks per lane per round
+// (b) - (d): the slab-staged traversal of k_pearson_u16 (csrc/pcm.cu), with the arithmetic switchable (MODE 0 / 1 / 2
+// for (b) / (c) / (d)) and U chunks per lane per round
 __device__ __forceinline__ unsigned int smem_u32(const void* p) { return (unsigned int)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned int count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -224,35 +230,92 @@ __device__ __forceinline__ void prs_stage(const PearsonU16Args& a, int s, long l
     if (lane < 16 && e < (lane < 8 ? min(b0, e1) : e1)) buf[PRS_PAD + (e - a0)] = a.img1[e];
 }
 
-__device__ __forceinline__ void prs_acc(const unsigned int A[4], const unsigned int B[4], unsigned int& sa, unsigned int& sb,
-                                        unsigned long long& saa, unsigned long long& sbb, unsigned long long& sab) {
+// (c): 64-bit multiply-accumulates
+struct Acc64 {
+    unsigned int sa, sb;
+    unsigned long long saa, sbb, sab;
+};
+__device__ __forceinline__ void prs_acc(const unsigned int A[4], const unsigned int B[4], Acc64& s) {
 #pragma unroll
     for (int m = 0; m < 4; ++m) {
         const unsigned int a0 = A[m] & 0xffffu, a1 = A[m] >> 16, b0 = B[m] & 0xffffu, b1 = B[m] >> 16;
-        sa += a0 + a1;
-        sb += b0 + b1;
-        saa += (unsigned long long)a0 * a0;   // IMAD.WIDE.U32 with 64-bit accumulate each
-        saa += (unsigned long long)a1 * a1;
-        sbb += (unsigned long long)b0 * b0;
-        sbb += (unsigned long long)b1 * b1;
-        sab += (unsigned long long)a0 * b0;
-        sab += (unsigned long long)a1 * b1;
+        s.sa += a0 + a1;
+        s.sb += b0 + b1;
+        s.saa += (unsigned long long)a0 * a0;   // IMAD.WIDE.U32 with 64-bit accumulate each
+        s.saa += (unsigned long long)a1 * a1;
+        s.sbb += (unsigned long long)b0 * b0;
+        s.sbb += (unsigned long long)b1 * b1;
+        s.sab += (unsigned long long)a0 * b0;
+        s.sab += (unsigned long long)a1 * b1;
     }
+}
+
+// (d): IDP.2A into uint32 partials p_lo + 256 p_hi, 128 IDPs (32 chunks) per partial between folds
+struct PrsAcc {
+    unsigned int sa, sb;
+    unsigned int aal, aah, bbl, bbh, abl, abh;
+};
+#define PRS_FOLD_CHUNKS 32
+__device__ __forceinline__ void prs_acc(const unsigned int A[4], const unsigned int B[4], PrsAcc& s) {
+#pragma unroll
+    for (int m = 0; m < 4; ++m) {
+        const unsigned int Ap = __byte_perm(A[m], 0u, 0x3120), Bp = __byte_perm(B[m], 0u, 0x3120);
+        s.sa = __dp2a_lo(A[m], 0x0101u, s.sa);
+        s.sb = __dp2a_lo(B[m], 0x0101u, s.sb);
+        s.aal = __dp2a_lo(A[m], Ap, s.aal);
+        s.aah = __dp2a_hi(A[m], Ap, s.aah);
+        s.bbl = __dp2a_lo(B[m], Bp, s.bbl);
+        s.bbh = __dp2a_hi(B[m], Bp, s.bbh);
+        s.abl = __dp2a_lo(A[m], Bp, s.abl);
+        s.abh = __dp2a_hi(A[m], Bp, s.abh);
+    }
+}
+
+__device__ __forceinline__ void prs_add(unsigned int sa, unsigned int sb, unsigned long long saa, unsigned long long sbb,
+                                        unsigned long long sab, unsigned long long* acc, int lane) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        sa += __shfl_xor_sync(0xffffffffu, sa, off);
+        sb += __shfl_xor_sync(0xffffffffu, sb, off);
+        saa += __shfl_xor_sync(0xffffffffu, saa, off);
+        sbb += __shfl_xor_sync(0xffffffffu, sbb, off);
+        sab += __shfl_xor_sync(0xffffffffu, sab, off);
+    }
+    if (lane == 0) {
+        if (sa) atomicAdd(acc + 0, (unsigned long long)sa);
+        if (sb) atomicAdd(acc + 1, (unsigned long long)sb);
+        if (saa) atomicAdd(acc + 2, saa);
+        if (sbb) atomicAdd(acc + 3, sbb);
+        if (sab) atomicAdd(acc + 4, sab);
+    }
+}
+__device__ __forceinline__ void prs_flush(Acc64& s, unsigned long long* acc, int lane) {
+    prs_add(s.sa, s.sb, s.saa, s.sbb, s.sab, acc, lane);
+    s = Acc64{0u, 0u, 0ull, 0ull, 0ull};
+}
+__device__ __forceinline__ void prs_flush(PrsAcc& s, unsigned long long* acc, int lane) {
+    prs_add(s.sa, s.sb, s.aal + ((unsigned long long)s.aah << 8), s.bbl + ((unsigned long long)s.bbh << 8),
+            s.abl + ((unsigned long long)s.abh << 8), acc, lane);
+    s = PrsAcc{0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
 }
 
 // One image-2 row segment of one candidate, owned by a warp.  Chunk k covers image-2 elements g + 8k .. g + 8k + 7
 // (g 16-byte aligned); elements lo .. hi - 1 of the chunk sequence belong to the segment.  s1 points at the staged
 // image-1 element paired with chunk 0's first element, rounded down to 16 bytes; SH is the rounding (0..7).
-// Chunks k >= kvec reach past the end of image 2 and are loaded element by element.
-template <bool SUMS, int U, int SH>
+// Chunks k >= kvec reach past the end of image 2 and are loaded element by element.  (d) folds every
+// PRS_FOLD_CHUNKS / U rounds of segments longer than 32 * PRS_FOLD_CHUNKS chunks (never at the probe's dx = 512).
+// TAIL: the row's last round takes up to U + 1 chunks per lane (k_pearson_u16: U = 1, TAIL).
+template <int MODE, int U, bool TAIL, int SH, typename ACC>
 __device__ __forceinline__ void prs_row(const unsigned short* __restrict__ g, const unsigned short* s1, int lo, int hi,
-                                        int nch, int kvec, int lane, unsigned int& sa, unsigned int& sb,
-                                        unsigned long long& saa, unsigned long long& sbb, unsigned long long& sab) {
-    for (int k0 = lane; k0 < nch; k0 += 32 * U) {
-        uint4 v[U];
+                                        int nch, int kvec, int lane, ACC& s, unsigned long long* acc) {
+    constexpr int UM = U + (TAIL ? 1 : 0);
+    constexpr int FOLD_ROUNDS = (PRS_FOLD_CHUNKS - (TAIL ? 1 : 0)) / U;
+    for (int kb = 0, r = 1; kb < nch; kb += 32 * U, ++r) {   // warp-uniform rounds
+        const bool last = TAIL && nch - kb <= 32 * UM;
+        uint4 v[UM];
 #pragma unroll
-        for (int u = 0; u < U; ++u) {        // both chunks' loads in flight before any arithmetic
-            const int k = k0 + 32 * u;
+        for (int u = 0; u < UM; ++u) {        // all chunks' loads in flight before any arithmetic
+            const int k = (u < U || last) ? kb + lane + 32 * u : nch;
             v[u] = make_uint4(0u, 0u, 0u, 0u);
             if (k < kvec) {
                 v[u] = ldg_stream16(g + 8 * k);
@@ -267,8 +330,8 @@ __device__ __forceinline__ void prs_row(const unsigned short* __restrict__ g, co
             }
         }
 #pragma unroll
-        for (int u = 0; u < U; ++u) {
-            const int k = k0 + 32 * u;
+        for (int u = 0; u < UM; ++u) {
+            const int k = (u < U || last) ? kb + lane + 32 * u : nch;
             if (k >= nch) break;
             const uint4 p = *reinterpret_cast<const uint4*>(s1 + 8 * k);
             const uint4 q = *reinterpret_cast<const uint4*>(s1 + 8 * k + 8);
@@ -287,14 +350,17 @@ __device__ __forceinline__ void prs_row(const unsigned short* __restrict__ g, co
                     B[m] &= mk;
                 }
             }
-            if (SUMS) prs_acc(A, B, sa, sb, saa, sbb, sab);
-            else sa ^= A[0] ^ A[1] ^ A[2] ^ A[3] ^ B[0] ^ B[1] ^ B[2] ^ B[3];
+            if (MODE) prs_acc(A, B, s);
+            else s.sa ^= A[0] ^ A[1] ^ A[2] ^ A[3] ^ B[0] ^ B[1] ^ B[2] ^ B[3];
         }
+        if (last) break;
+        if (MODE == 2 && r % FOLD_ROUNDS == 0 && kb + 32 * U < nch) prs_flush(s, acc, lane);
     }
 }
 
-// dynamic smem: 2 stage buffers, the candidate list, 5 accumulators per candidate
-template <bool SUMS, int U>
+// dynamic smem: 2 stage buffers, the candidate list, 5 accumulators per candidate.  UNR: unrolling of the loop over a
+// warp's rows (k_pearson_u16: 1, so that the 8 alignment cases of prs_row are inlined once each).
+template <int MODE, int U, bool TAIL = false, int UNR = PRS_ROWS / (NT / 32)>
 __global__ void __launch_bounds__(NT, 3) k_new(const __grid_constant__ PearsonU16Args a) {
     extern __shared__ __align__(16) unsigned char dyn_sm[];
     const int ncand = *a.ncand;   // written by k_pcm_select (no host round trip between peaks and Pearson)
@@ -335,15 +401,6 @@ __global__ void __launch_bounds__(NT, 3) k_new(const __grid_constant__ PearsonU1
         const int nr = (int)min((long long)a.slab_rows, nrows - r0);
         const int z0 = (int)(r0 / a.dy), y0 = (int)(r0 - (long long)z0 * a.dy);
         const int zl = (int)((r0 + nr - 1) / a.dy);
-        // (y, z) of this warp's rows wid, wid + NW, ...
-        int ry[RPW], rz[RPW];
-#pragma unroll
-        for (int j = 0; j < RPW; ++j) {
-            int y = y0 + wid + j * NW, z = z0;
-            while (y >= a.dy) { y -= a.dy; ++z; }
-            ry[j] = y;
-            rz[j] = z;
-        }
         // staged image-1 element e0 + i (e0 = r0 * dx, the slab's first) sits at sbuf[soff + i]
         const unsigned short* sbuf = stage + (size_t)buf * a.stage_elems;
         const int soff = PRS_PAD + (int)((r0 * a.dx) & 7);
@@ -351,13 +408,14 @@ __global__ void __launch_bounds__(NT, 3) k_new(const __grid_constant__ PearsonU1
         for (int c = 0; c < ncand; ++c) {
             const PearsonCand cd = s_cand[c];
             if (zl < cd.o1[2] || z0 >= cd.o1[2] + cd.sz[2]) continue;   // block-uniform
-            unsigned int sa = 0, sb = 0;
-            unsigned long long saa = 0, sbb = 0, sab = 0;
+            typename std::conditional<MODE == 1, Acc64, PrsAcc>::type acc = {};
             bool any = false;
-#pragma unroll
+#pragma unroll UNR
             for (int j = 0; j < RPW; ++j) {
                 const int rr = wid + j * NW;
-                const int yy = ry[j] - cd.o1[1], zz = rz[j] - cd.o1[2];
+                int y = y0 + rr, z = z0;   // (y, z) of slab row rr
+                while (y >= a.dy) { y -= a.dy; ++z; }
+                const int yy = y - cd.o1[1], zz = z - cd.o1[2];
                 if (rr >= nr || yy < 0 || yy >= cd.sz[1] || zz < 0 || zz >= cd.sz[2]) continue;
                 any = true;
                 const long long g2 = ((long long)(zz + cd.o2[2]) * a.dy + (yy + cd.o2[1])) * a.dx + cd.o2[0];
@@ -370,34 +428,17 @@ __global__ void __launch_bounds__(NT, 3) k_new(const __grid_constant__ PearsonU1
                 const unsigned short* s1 = sbuf + (t & ~7);
                 const unsigned short* g = a.img2 + c2;
                 switch (t & 7) {
-                    case 0: prs_row<SUMS, U, 0>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
-                    case 1: prs_row<SUMS, U, 1>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
-                    case 2: prs_row<SUMS, U, 2>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
-                    case 3: prs_row<SUMS, U, 3>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
-                    case 4: prs_row<SUMS, U, 4>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
-                    case 5: prs_row<SUMS, U, 5>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
-                    case 6: prs_row<SUMS, U, 6>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
-                    default: prs_row<SUMS, U, 7>(g, s1, lo, hi, nch, kvec, lane, sa, sb, saa, sbb, sab); break;
+                    case 0: prs_row<MODE, U, TAIL, 0>(g, s1, lo, hi, nch, kvec, lane, acc, s_acc + 5 * c); break;
+                    case 1: prs_row<MODE, U, TAIL, 1>(g, s1, lo, hi, nch, kvec, lane, acc, s_acc + 5 * c); break;
+                    case 2: prs_row<MODE, U, TAIL, 2>(g, s1, lo, hi, nch, kvec, lane, acc, s_acc + 5 * c); break;
+                    case 3: prs_row<MODE, U, TAIL, 3>(g, s1, lo, hi, nch, kvec, lane, acc, s_acc + 5 * c); break;
+                    case 4: prs_row<MODE, U, TAIL, 4>(g, s1, lo, hi, nch, kvec, lane, acc, s_acc + 5 * c); break;
+                    case 5: prs_row<MODE, U, TAIL, 5>(g, s1, lo, hi, nch, kvec, lane, acc, s_acc + 5 * c); break;
+                    case 6: prs_row<MODE, U, TAIL, 6>(g, s1, lo, hi, nch, kvec, lane, acc, s_acc + 5 * c); break;
+                    default: prs_row<MODE, U, TAIL, 7>(g, s1, lo, hi, nch, kvec, lane, acc, s_acc + 5 * c); break;
                 }
             }
-            if (!any) continue;  // warp-uniform
-            // per-warp partials: sa, sb < slab elements * 65535 < 2^32
-#pragma unroll
-            for (int off = 16; off > 0; off >>= 1) {
-                sa += __shfl_xor_sync(0xffffffffu, sa, off);
-                sb += __shfl_xor_sync(0xffffffffu, sb, off);
-                saa += __shfl_xor_sync(0xffffffffu, saa, off);
-                sbb += __shfl_xor_sync(0xffffffffu, sbb, off);
-                sab += __shfl_xor_sync(0xffffffffu, sab, off);
-            }
-            if (lane == 0) {
-                unsigned long long* acc = s_acc + 5 * c;
-                if (sa) atomicAdd(acc + 0, (unsigned long long)sa);
-                if (sb) atomicAdd(acc + 1, (unsigned long long)sb);
-                if (saa) atomicAdd(acc + 2, saa);
-                if (sbb) atomicAdd(acc + 3, sbb);
-                if (sab) atomicAdd(acc + 4, sab);
-            }
+            if (any) prs_flush(acc, s_acc + 5 * c, lane);   // warp-uniform
         }
         __syncthreads();   // every warp is done with this buffer before it is refilled
     }
@@ -513,7 +554,8 @@ int main() {
                L ? "all shifts within +-4" : "true peak + 4 seeded noise peaks, wrap candidates", nc, px / 1e6, dram / 1e9, alg / 1e9);
         CK(cudaMemcpy(dc, cl.data(), sizeof(PearsonCand) * nc, cudaMemcpyHostToDevice));
         std::vector<unsigned long long> ref(5 * nc), got(5 * nc);
-        auto run = [&](const char* name, int variant, int slab_rows) -> int {
+        typedef void (*KNew)(PearsonU16Args);   // nullptr: (a)
+        auto run = [&](const char* name, KNew kn, bool check, int slab_rows) -> int {
             PearsonArgs oa;
             oa.img1 = i1; oa.img2 = i2; oa.dtype = 0; oa.dx = D; oa.dy = D; oa.dz = D; oa.cands = dc;
             PearsonU16Args a;
@@ -523,25 +565,19 @@ int main() {
             a.nslabs = (int)(((long long)D * D + slab_rows - 1) / slab_rows);
             a.cands = dc; a.sums = dsum; a.ncand = dcnt; a.counter = dcnt + 1;
             const size_t smem = 2 * 2 * (size_t)a.stage_elems + 80 * nc;
-            auto setup = [&](const void* f, int& ctas) -> cudaError_t {
-                cudaError_t e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            int ctas = prop.multiProcessorCount * 8;
+            if (kn) {
+                CK(cudaFuncSetAttribute((const void*)kn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
                 int occ = 0;
-                if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, f, NT, smem);
+                CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, (const void*)kn, NT, smem));
                 ctas = std::min(a.nslabs, prop.multiProcessorCount * std::max(occ, 1));
-                return e;
-            };
-            int ctas = 0;
-            if (variant == 1) CK(setup((const void*)k_new<false, 2>, ctas));
-            if (variant == 2) CK(setup((const void*)k_new<true, 2>, ctas));
-            if (variant == 3) CK(setup((const void*)k_new<true, 3>, ctas));
+            }
             const int cnt[2] = {nc, 0};
             auto launch = [&]() {
                 cudaMemsetAsync(dsum, 0, 8 * 5 * nc);
                 cudaMemcpyAsync(dcnt, cnt, 8, cudaMemcpyHostToDevice);
-                if (variant == 0) k_old<<<prop.multiProcessorCount * 8, NT, 8 * 5 * nc>>>(oa, dcnt, dsum);
-                else if (variant == 1) k_new<false, 2><<<ctas, NT, smem>>>(a);
-                else if (variant == 2) k_new<true, 2><<<ctas, NT, smem>>>(a);
-                else k_new<true, 3><<<ctas, NT, smem>>>(a);
+                if (!kn) k_old<<<ctas, NT, 8 * 5 * nc>>>(oa, dcnt, dsum);
+                else kn<<<ctas, NT, smem>>>(a);
             };
             for (int w = 0; w < 3; ++w) launch();
             CK(cudaEventRecord(e0));
@@ -553,18 +589,28 @@ int main() {
             ms /= iters;
             CK(cudaMemcpy(got.data(), dsum, 8 * 5 * nc, cudaMemcpyDeviceToHost));
             const char* chk = "";
-            if (variant == 0) ref = got;
-            else if (variant >= 2) chk = got == ref ? "  sums == (a)" : "  SUMS DIFFER from (a)";
+            if (!kn) ref = got;
+            else if (check) chk = got == ref ? "  sums == (a)" : "  SUMS DIFFER from (a)";
             printf("  %-44s %7.3f ms  DRAM model %7.1f GB/s (%.2f of 3.35 TB/s)  4 B/voxel frac %.2f  CTAs %d%s\n", name, ms,
-                   dram / (ms * 1e-3) / 1e9, dram / (ms * 1e-3) / 3.35e12, alg / (ms * 1e-3) / 3.35e12, variant ? ctas : prop.multiProcessorCount * 8, chk);
+                   dram / (ms * 1e-3) / 1e9, dram / (ms * 1e-3) / 3.35e12, alg / (ms * 1e-3) / 3.35e12, ctas, chk);
             return 0;
         };
-        if (run("(a) previous traversal", 0, 32)) return 1;
-        if (run("(b) slabs of 32 rows, no arithmetic, U=2", 1, 32)) return 1;
-        if (run("(c) slabs of 32 rows, sums, U=2", 2, 32)) return 1;
-        if (run("(c) slabs of 16 rows, sums, U=2", 2, 16)) return 1;
-        if (run("(c) slabs of 32 rows, sums, U=3", 3, 32)) return 1;
-        if (run("(c) slabs of 16 rows, sums, U=3", 3, 16)) return 1;
+        if (run("(a) previous traversal", nullptr, true, 32)) return 1;
+        if (run("(b) slabs of 32 rows, no arithmetic, U=2", k_new<0, 2>, false, 32)) return 1;
+        if (run("(c) slabs of 32 rows, 64-bit sums, U=2", k_new<1, 2>, true, 32)) return 1;
+        if (run("(c) slabs of 16 rows, 64-bit sums, U=2", k_new<1, 2>, true, 16)) return 1;
+        if (run("(c) slabs of 32 rows, 64-bit sums, U=3", k_new<1, 3>, true, 32)) return 1;
+        if (run("(c) slabs of 16 rows, 64-bit sums, U=3", k_new<1, 3>, true, 16)) return 1;
+        if (run("(d) slabs of 32 rows, IDP sums, U=1", k_new<2, 1>, true, 32)) return 1;
+        if (run("(d) slabs of 16 rows, IDP sums, U=1", k_new<2, 1>, true, 16)) return 1;
+        if (run("(d) slabs of 32 rows, IDP sums, U=2", k_new<2, 2>, true, 32)) return 1;
+        if (run("(d) slabs of 16 rows, IDP sums, U=2", k_new<2, 2>, true, 16)) return 1;
+        if (run("(d) slabs of 32 rows, IDP sums, U=3", k_new<2, 3>, true, 32)) return 1;
+        if (run("(d) slabs of 16 rows, IDP sums, U=3", k_new<2, 3>, true, 16)) return 1;
+        if (run("(e) (d) rows not unrolled, U=2", k_new<2, 2, false, 1>, true, 32)) return 1;
+        if (run("(e) (d) rows not unrolled, U=1", k_new<2, 1, false, 1>, true, 32)) return 1;
+        if (run("(e) U=1, last round of 2 (as built)", k_new<2, 1, true, 1>, true, 32)) return 1;
+        if (run("(e) U=2, last round of 3", k_new<2, 2, true, 1>, true, 32)) return 1;
     }
     return 0;
 }
