@@ -55,6 +55,8 @@ struct bs_pcm_workspace {
     void* small = nullptr;       // device scratch for peaks / pearson sums
     size_t small_bytes = 0;
     void* small_host = nullptr;  // pinned mirror
+    void* sync = nullptr;        // int: hand-off error word, then the per-plane counters of the fused FFT kernels
+    size_t sync_bytes = 0;
     cudaEvent_t crop_ready[2] = {nullptr, nullptr};
     cudaEvent_t crop_free[2] = {nullptr, nullptr};
 };

@@ -816,6 +816,120 @@ __device__ __forceinline__ void col540_tw(float2* tw, const float2* __restrict__
     for (int i = threadIdx.x; i < Col540::N; i += blockDim.x) tw[i] = g[i];
 }
 
+// ------------------------------------------------------------------------------------------
+// Plane hand-off between the two roles of the fused kernel k_fft_xy_col540.  One role (the producer) stores z-planes
+// of the spectra, the other (the consumer) transforms them along y as soon as each plane is complete, while the plane
+// is still in L2.  Two counters per plane, zeroed before the launch: ready[z] counts the units the producer has stored
+// into plane z, done[z] the units the consumer has taken out of it.  The producer stores into plane z only once plane
+// z - window is taken, which bounds the data waiting in L2 to about `window` planes whatever the split of the CTAs
+// between the roles.  done[] only bounds that residency: the producer never stores into a plane again once it is
+// complete, so the consumer may count a unit as soon as it has loaded it.
+// Every wait is bounded: when a wait expires, its thread records the kernel's code in *err and the CTA stops
+// without writing; the other CTAs see *err and stop as well, and the host turns the code into an error.
+#define PCM_HANDOFF_POLLS (1u << 24)
+struct Handoff {
+    int* ready = nullptr;   // [Pz]; nullptr in the standalone kernels, where every hook below is a no-op
+    int* done = nullptr;    // [Pz]
+    int* err = nullptr;
+    int code = 0;
+    int ready_full = 0, done_full = 0;   // units of a whole plane on each counter
+    int window = 0;                      // >= 2: a tile's stores may reach into the plane after the one it waits for
+};
+
+__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
+    int v;
+    asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+// one thread: poll *c until it reaches `full`; false when the poll budget is spent or another wait has expired
+__device__ __forceinline__ bool handoff_wait(const int* c, int full, const Handoff& h) {
+    unsigned int ns = 32;
+    for (unsigned int i = 0; i < PCM_HANDOFF_POLLS; ++i) {
+        if (ld_acquire_gpu(c) >= full) {
+            __threadfence();   // the whole CTA reads the plane after the barrier that follows
+            return true;
+        }
+        if (*(volatile int*)h.err) return false;
+        __nanosleep(ns);
+        ns = min(2 * ns, 256u);
+    }
+    atomicCAS(h.err, 0, h.code);
+    return false;
+}
+// consumer: plane z is complete
+__device__ __forceinline__ bool handoff_ready(const Handoff& h, int z) {
+    return !h.ready || handoff_wait(h.ready + z, h.ready_full, h);
+}
+// producer: plane z may be stored into (plane z - window has been read out)
+__device__ __forceinline__ bool handoff_window(const Handoff& h, int z) {
+    return !h.ready || z < h.window || handoff_wait(h.done + z - h.window, h.done_full, h);
+}
+// one thread, after a barrier that follows the CTA's stores into plane z: n more units of it are complete
+__device__ __forceinline__ void handoff_publish(const Handoff& h, int z, int n) {
+    if (!h.ready) return;
+    __threadfence();
+    atomicAdd(h.ready + z, n);
+}
+// one thread, once the CTA has loaded n units of plane z
+__device__ __forceinline__ void handoff_consume(const Handoff& h, int z, int n) {
+    if (h.ready) atomicAdd(h.done + z, n);
+}
+// f(z, n) for each plane z of Py lines that lines [l0, l1) touch, with the n lines that fall into it
+template <class Fn>
+__device__ __forceinline__ void for_planes(int l0, int l1, int Py, Fn&& f) {
+    for (int z = l0 / Py; z * Py < l1; ++z) f(z, min(l1, (z + 1) * Py) - max(l0, z * Py));
+}
+
+// Forward y FFT, in place, of tiles t, t + stride, ... < n_tiles on F (RegFft2<20, 27>), ptr(t) the tile's first
+// element.  X0 holds two exchange buffers (one barrier per tile); the next tile's loads go out into the stage-1
+// registers once stage 1 has written them out (in the fused roles after the barrier, which carries the hand-off
+// wait), and are in flight under stage 2 and the stores.
+//   Y_ALONE     k_fft_col540
+//   Y_CONSUMER  y role of k_fft_xy_col540: a tile's loads wait for its plane; thread 0 counts a tile as taken
+//               after its own stage 1, before it waits for the next tile's plane, so a tile's count never waits on
+//               a later plane; the spectra go to DRAM as streaming (evict-first) stores so as not to push the x
+//               output that is still waiting out of L2
+enum { Y_ALONE, Y_CONSUMER };
+template <class F, int MODE, class Ptr>
+__device__ __forceinline__ void col540_y_tiles(float2* X0, float2* tw, const float2* __restrict__ tw_g, int t, int stride,
+                                               int n_tiles, long long estride, int tiles_per_plane, Ptr ptr,
+                                               const Handoff& h) {
+    static_assert(F::N == 540, "RegFft2<20, 27>");
+    bool ok = true;
+    if (MODE == Y_CONSUMER && threadIdx.x == 0 && t < n_tiles) ok = handoff_ready(h, t / tiles_per_plane);
+    if (MODE == Y_CONSUMER && __syncthreads_or(!ok)) return;
+    typename F::In v;
+    if (t < n_tiles) F::load(v, ptr(t), estride);
+    col540_tw(tw, tw_g);
+    __syncthreads();
+    for (int it = 0; t < n_tiles; t += stride, ++it) {
+        float2* x = X0 + (it & 1) * F::XSIZE;
+        F::stage1(v, x, tw);
+        const int tn = t + stride;
+        if (MODE == Y_ALONE) {
+            if (tn < n_tiles) F::load(v, ptr(tn), estride);
+            __syncthreads();
+        } else {
+            if (threadIdx.x == 0) {
+                handoff_consume(h, t / tiles_per_plane, 1);
+                if (tn < n_tiles) ok = handoff_ready(h, tn / tiles_per_plane);
+            }
+            if (__syncthreads_or(!ok)) return;
+            if (tn < n_tiles) F::load(v, ptr(tn), estride);   // the next tile's plane is complete from here on
+        }
+        F::stage2(x, [&](const float2 (&w)[27], int, int k1, int c) {
+            float2* g = ptr(t);
+            if (MODE == Y_CONSUMER) {
+                float2* p = g + (long long)k1 * estride + c;
+#pragma unroll
+                for (int k2 = 0; k2 < 27; ++k2) __stcs(p + (long long)(20 * k2) * estride, w[k2]);
+            } else {
+                F::store(w, g, estride, k1, c);
+            }
+        });
+    }
+}
+
 // forward y FFT in place, tiles of both spectra (p.n_tiles = tiles_x * n_other * n_img)
 __global__ void __launch_bounds__(COL540_NT, 1) k_fft_col540(const __grid_constant__ StridedPipeArgs p) {
     const StridedArgs& a = p.s;
@@ -825,19 +939,8 @@ __global__ void __launch_bounds__(COL540_NT, 1) k_fft_col540(const __grid_consta
         const int o = r % p.n_other, im = r / p.n_other;
         return (im ? a.b : a.a) + (size_t)o * a.ostride + (size_t)tx * COL540_TC;
     };
-    Col540::In v;
-    int t = blockIdx.x;
-    if (t < p.n_tiles) Col540::load(v, tile_ptr(t), a.estride);
-    col540_tw(tw, a.tw);
-    __syncthreads();
-    for (int it = 0; t < p.n_tiles; t += gridDim.x, ++it) {
-        float2* x = bs_sm + Col540::N + (it & 1) * Col540::XSIZE;   // two exchange buffers: one barrier per tile
-        Col540::stage1(v, x, tw);
-        const int tn = t + gridDim.x;
-        if (tn < p.n_tiles) Col540::load(v, tile_ptr(tn), a.estride);
-        __syncthreads();
-        Col540::stage2(x, [&](const float2 (&w)[27], int, int k1, int c) { Col540::store(w, tile_ptr(t), a.estride, k1, c); });
-    }
+    col540_y_tiles<Col540, Y_ALONE>(bs_sm + Col540::N, tw, a.tw, blockIdx.x, gridDim.x, p.n_tiles, a.estride, 1, tile_ptr,
+                                    Handoff());
 }
 
 // z cross-power: forward z FFT of A and B, unit-magnitude normalisation and conj(A) * B, then the forward FFT of
@@ -976,7 +1079,10 @@ struct XR2CCol540Args {
     int n_tiles;      // ceil(Py * Pz / 16)
 };
 
-__global__ void __launch_bounds__(COL540X_NT, 1) k_fft_x_r2c_col540(const __grid_constant__ XR2CCol540Args P) {
+// Tiles t, t + stride, ... of the pass.  As the producer of k_fft_xy_col540, a tile's stores wait for the window of
+// the last plane they reach, and the tile's lines are published per plane at the next tile's B1 (the last tile's
+// after a barrier of its own).
+__device__ __forceinline__ void x_r2c_col540_tiles(const XR2CCol540Args& P, int t, int stride, const Handoff& h) {
     const XR2CArgs& a = P.x;
     constexpr int TC = COL540_TC, N = Col540X::N, pitch = 272;
     float2* X = bs_sm;
@@ -1009,18 +1115,21 @@ __global__ void __launch_bounds__(COL540X_NT, 1) k_fft_x_r2c_col540(const __grid
         xw[i] = make_int2(a.idx_x[i], __float_as_int(a.w_x[i]));
     }
     if (threadIdx.x < 4 * TC) nz[threadIdx.x] = 0;
-    int t = blockIdx.x;
     if (t < P.n_tiles) stage(t, 0);
     cp_async_wait<0>();
     __syncthreads();
     const int c = threadIdx.x % TC;   // this thread's column in both of its stage-1 items and its stage-2 item
-    for (int it = 0; t < P.n_tiles; t += gridDim.x, ++it) {
+    auto publish = [&](int tp) {      // thread 0, after a barrier that follows tile tp's stores
+        for_planes(tp * TC, min(tp * TC + TC, n_lines), a.Py, [&](int z, int n) { handoff_publish(h, z, n); });
+    };
+    int it = 0;
+    for (; t < P.n_tiles; t += stride, ++it) {
         const int b = it & 1;
         const int L = t * TC + c;
         const int zp = L / a.Py, yp = L - zp * a.Py;
         const bool live = L < n_lines && zp < a.Ez && yp < a.Ey;
         const float wy = live ? __ldg(a.w_y + yp) : 0.f, wz = live ? __ldg(a.w_z + zp) : 0.f;
-        if (t + (int)gridDim.x < P.n_tiles) stage(t + gridDim.x, b ^ 1);   // buffer b^1 was read before the last B1
+        if (t + stride < P.n_tiles) stage(t + stride, b ^ 1);   // buffer b^1 was read before the last B1
         const unsigned short* ra = reinterpret_cast<const unsigned short*>(raw + ((size_t)b * 2 * TC + c) * P.raw_stride);
         const unsigned short* rb = reinterpret_cast<const unsigned short*>(raw + ((size_t)(b * 2 + 1) * TC + c) * P.raw_stride);
         Col540X::In v;
@@ -1046,6 +1155,7 @@ __global__ void __launch_bounds__(COL540X_NT, 1) k_fft_x_r2c_col540(const __grid
         if (nzb) nz[(b * 2 + 1) * TC + c] = 1;
         Col540X::stage1(v, X, tw);
         __syncthreads();   // B1: X complete; the previous tile's separation has read Y and nz[b ^ 1] out
+        if (threadIdx.x == 0 && it) publish(t - stride);
         if (threadIdx.x < 2 * TC) nz[(b ^ 1) * 2 * TC + threadIdx.x] = 0;
         Col540X::stage2(X, [&](const float2 (&w)[27], int, int k1, int cc) {
             float2* y = Y + cc * COL540_XLP + k1;
@@ -1053,7 +1163,10 @@ __global__ void __launch_bounds__(COL540X_NT, 1) k_fft_x_r2c_col540(const __grid
             for (int k2 = 0; k2 < 27; ++k2) y[20 * k2] = w[k2];
         });
         cp_async_wait<0>();
-        __syncthreads();   // B2: Y complete (X free again), this thread's and every other thread's next rows landed
+        bool ok = true;
+        if (threadIdx.x == 0) ok = handoff_window(h, (min(t * TC + TC, n_lines) - 1) / a.Py);
+        // B2: Y complete (X free again), this thread's and every other thread's next rows landed
+        if (__syncthreads_or(!ok)) return;
         for (int j = threadIdx.x; j < TC * pitch; j += COL540X_NT) {
             const int l = j / pitch, k = j - l * pitch;
             const int Lj = t * TC + l;
@@ -1068,6 +1181,14 @@ __global__ void __launch_bounds__(COL540X_NT, 1) k_fft_x_r2c_col540(const __grid
             __stcg(a.spec[1] + (size_t)Lj * pitch + k, B);
         }
     }
+    if (h.ready && it) {
+        __syncthreads();
+        if (threadIdx.x == 0) publish(t - stride);
+    }
+}
+
+__global__ void __launch_bounds__(COL540X_NT, 1) k_fft_x_r2c_col540(const __grid_constant__ XR2CCol540Args P) {
+    x_r2c_col540_tiles(P, blockIdx.x, gridDim.x, Handoff());
 }
 
 // Inverse x pass, in place: a tile is 32 consecutive spectrum rows (16 pairs of lines), staged by one 1-D bulk copy
@@ -1185,6 +1306,50 @@ __global__ void __launch_bounds__(COL540X_NT, 1) k_fft_x_c2r_col540(const __grid
         }
     }
 }
+
+// ------------------------------------------------------------------------------------------
+// The forward x and y passes in one persistent kernel, for Px = Py = 540.  The y transform of a z-plane needs only
+// that plane's x output, so instead of one kernel per axis, with a round trip of both spectra through DRAM in
+// between, the CTAs split into two roles that run concurrently and hand each plane over through L2 (Handoff above):
+// CTAs [0, kx) run k_fft_x_r2c_col540's tiles (16 lines each, ascending line order, which is plane order) and publish
+// the lines each tile stores per plane; the others run y tiles (540 rows x 16 columns) plane-major: the 17 column
+// tiles of A and of B of plane z, then plane z + 1.  A y tile waits until its plane has all Py lines.
+// The y role runs Col540X (RegFft2<20, 27> on 448 threads, one stage-1 item per thread): each item computes what
+// k_fft_col540's does, so the spectra are bit-identical to the five-pass chain's.  It uses the x role's largest
+// shared-memory regions as its two exchange buffers.
+// Forward progress: all CTAs are co-resident (cooperative launch, one CTA per SM).  Each role takes its tiles in
+// ascending plane order.  A y tile waits only on x tiles of its own plane (its count in done[] waits on nothing), and
+// an x tile waits only on y tiles `window` >= 2 planes behind the last plane it stores into.  So the lowest plane p
+// that is not yet taken can always proceed: the x tiles that reach into p (at most into p + 1) wait on planes below p,
+// and every earlier tile of each CTA is in a plane no higher.
+// The inverse pair (y, then x C2R) fused the same way measured slower than the two kernels (DESIGN.md), so it
+// stays two launches.
+struct XYCol540Args {
+    XR2CCol540Args x;
+    const float2* tw_y;
+    int kx;   // CTAs of the x role
+    Handoff h;
+};
+
+__global__ void __launch_bounds__(COL540X_NT, 1) k_fft_xy_col540(const __grid_constant__ XYCol540Args P) {
+    if ((int)blockIdx.x < P.kx) {
+        x_r2c_col540_tiles(P.x, blockIdx.x, P.kx, P.h);
+        return;
+    }
+    const XR2CArgs& a = P.x.x;
+    float2* X0 = bs_sm;                                           // r2c's X and Y regions
+    float2* tw = X0 + Col540X::XSIZE + COL540_TC * COL540_XLP;   // r2c's twiddle region
+    static_assert(COL540_TC * COL540_XLP >= Col540X::XSIZE, "exchange buffers");
+    const int tiles_x = a.pitch / COL540_TC, per_plane = 2 * tiles_x;
+    const long long ostride = (long long)a.Py * a.pitch;
+    auto ptr = [&](int u) -> float2* {
+        const int z = u / per_plane, j = u - z * per_plane, im = j / tiles_x;
+        return a.spec[im] + z * ostride + (j - im * tiles_x) * COL540_TC;
+    };
+    col540_y_tiles<Col540X, Y_CONSUMER>(X0, tw, P.tw_y, blockIdx.x - P.kx, gridDim.x - P.kx, a.Pz * per_plane, a.pitch,
+                                        per_plane, ptr, P.h);
+}
+
 
 // ------------------------------------------------------------------------------------------
 // x pass, complex -> real, in place
@@ -1964,6 +2129,7 @@ void bs_pcm_workspace_free(bs_ctx* ctx) {
             if (ws.crop[i][j]) cudaFree(ws.crop[i][j]);
     if (ws.small) cudaFree(ws.small);
     if (ws.small_host) cudaFreeHost(ws.small_host);
+    if (ws.sync) cudaFree(ws.sync);
     for (int i = 0; i < 2; ++i) {
         if (ws.crop_ready[i]) cudaEventDestroy(ws.crop_ready[i]);
         if (ws.crop_free[i]) cudaEventDestroy(ws.crop_free[i]);
@@ -2060,6 +2226,11 @@ static int pcm_tables(bs_ctx* ctx, const PcmGeometry& g, PcmDeviceTables** out) 
     return BS_OK;
 }
 
+// ws.sync: the error word of k_fft_xy_col540's hand-off waits (PCM_HANDOFF_XY once one expired, else 0), reset once
+// per pair, then [ready Pz][done Pz] counters, zeroed before each launch
+#define PCM_SYNC_COUNTERS 32   // ints ahead of the counters (the error word on a line of its own)
+enum { PCM_HANDOFF_OK = 0, PCM_HANDOFF_XY = 1 };
+
 static int pcm_workspace(bs_ctx* ctx, const PcmGeometry& g) {
     bs_pcm_workspace& ws = ctx->ws;
     const size_t need = (size_t)g.P[2] * g.P[1] * g.pitch * sizeof(float2);
@@ -2079,7 +2250,33 @@ static int pcm_workspace(bs_ctx* ctx, const PcmGeometry& g) {
         BS_CUDA(ctx, cudaHostAlloc(&ws.small_host, small_need, cudaHostAllocDefault));
         ws.small_bytes = small_need;
     }
+    const size_t sync_need = sizeof(int) * (PCM_SYNC_COUNTERS + 2 * (size_t)g.P[2]);
+    if (ws.sync_bytes < sync_need) {
+        BS_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        if (ws.sync) cudaFree(ws.sync);
+        ws.sync = nullptr;
+        ws.sync_bytes = 0;
+        BS_CUDA(ctx, cudaMalloc(&ws.sync, sync_need));
+        BS_CUDA(ctx, cudaMemset(ws.sync, 0, sync_need));
+        ws.sync_bytes = sync_need;
+    }
     return BS_OK;
+}
+
+static int pcm_reset_handoff(bs_ctx* ctx) {
+    BS_CUDA(ctx, cudaMemsetAsync(ctx->ws.sync, 0, sizeof(int), ctx->stream));
+    return BS_OK;
+}
+static int pcm_handoff_error(bs_ctx* ctx, int code) {
+    if (code == PCM_HANDOFF_OK) return BS_OK;
+    return bs_set_error(ctx, BS_ERR_CUDA, "pcm: k_fft_xy_col540: a plane hand-off wait expired (code %d)", code);
+}
+// wait for the stream, then check the error word
+static int pcm_sync_handoff(bs_ctx* ctx) {
+    int code = 0;
+    BS_CUDA(ctx, cudaMemcpyAsync(&code, ctx->ws.sync, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    BS_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return pcm_handoff_error(ctx, code);
 }
 
 static int set_smem(bs_ctx* ctx, const void* fn, size_t bytes) {
@@ -2145,6 +2342,7 @@ static int pcm_kernel_attrs(bs_ctx* ctx) {
     if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r<FftX270>, 0))) return rc;
     if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_col540, 0))) return rc;
     if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r_col540, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_xy_col540, 0))) return rc;
     ctx->pcm_attr_done = true;
     return BS_OK;
 }
@@ -2169,9 +2367,8 @@ static bool x_col540(bs_ctx* ctx, const PcmGeometry& g, int tiles) {
     return mode && g.P[0] == Col540X::N && env_int("BS_FFT_STATIC", 1) && (mode == 2 || tiles >= ctx->sm_count);
 }
 
-// pass 0: both crops -> blended mirrored extension + zero pad -> R2C along x into ws.spec_a / ws.spec_b
-static int pcm_pass_x_r2c(bs_ctx* ctx, const void* d1, const void* d2, int dtype, const PcmGeometry& g,
-                          PcmDeviceTables* t, char* info) {
+static XR2CArgs r2c_args(bs_ctx* ctx, const void* d1, const void* d2, int dtype, const PcmGeometry& g,
+                         PcmDeviceTables* t) {
     bs_pcm_workspace& ws = ctx->ws;
     XR2CArgs a;
     a.img[0] = d1; a.img[1] = d2;
@@ -2187,6 +2384,30 @@ static int pcm_pass_x_r2c(bs_ctx* ctx, const void* d1, const void* d2, int dtype
     a.tw = t->tw[0];
     a.plan = g.plan_x;
     a.lshift = g.lshift_r2c;
+    return a;
+}
+
+// k_fft_x_r2c_col540's arguments and dynamic shared memory; false when pass 0 does not take that kernel
+static bool r2c_col540(bs_ctx* ctx, const XR2CArgs& a, int dtype, const PcmGeometry& g, XR2CCol540Args* c,
+                       size_t* smem) {
+    const int row_bytes = g.d[0] * (dtype == BS_DTYPE_U16 ? 2 : dtype == BS_DTYPE_F32 ? 4 : 1);
+    const int col_tiles = (g.P[1] * g.P[2] + COL540_TC - 1) / COL540_TC;
+    int raw_stride = (row_bytes + 15) & ~15;   // 16 staged rows on 8 different banks: 4 words times an odd number
+    while ((raw_stride / 4) % 8 != 4) raw_stride += 16;
+    *smem = (Col540X::XSIZE + (size_t)COL540_TC * COL540_XLP + 2 * (size_t)Col540X::N) * sizeof(float2) +
+            4 * COL540_TC * (sizeof(int) + (size_t)raw_stride);
+    c->x = a;
+    c->row_bytes = row_bytes;
+    c->raw_stride = raw_stride;
+    c->n_tiles = col_tiles;
+    return x_col540(ctx, g, col_tiles) && dtype == BS_DTYPE_U16 && (row_bytes % 16) == 0 && ((size_t)a.img[0] % 16) == 0 &&
+           ((size_t)a.img[1] % 16) == 0 && *smem <= PCM_SMEM_MAX;
+}
+
+// pass 0: both crops -> blended mirrored extension + zero pad -> R2C along x into ws.spec_a / ws.spec_b
+static int pcm_pass_x_r2c(bs_ctx* ctx, const void* d1, const void* d2, int dtype, const PcmGeometry& g,
+                          PcmDeviceTables* t, char* info) {
+    const XR2CArgs a = r2c_args(ctx, d1, d2, dtype, g, t);
     const int LB = 1 << g.lshift_r2c;
     dim3 grid((g.P[1] + LB - 1) / LB, g.P[2], 2);
     {
@@ -2199,19 +2420,10 @@ static int pcm_pass_x_r2c(bs_ctx* ctx, const void* d1, const void* d2, int dtype
         const int xmode = env_int("BS_FFT_X_WARP", 1);
         const size_t smem_w = ((size_t)g.P[0] + (size_t)(PCM_THREADS / 32) * 2 * g.M) * sizeof(float2) +
                               (tma_ok ? (size_t)(PCM_THREADS / 32) * (2 * (size_t)row_bytes + 16) : 0);
-        const int col_tiles = (g.P[1] * g.P[2] + COL540_TC - 1) / COL540_TC;
-        int raw_stride = (row_bytes + 15) & ~15;   // 16 staged rows on 8 different banks: 4 words times an odd number
-        while ((raw_stride / 4) % 8 != 4) raw_stride += 16;
-        const size_t smem_col = (Col540X::XSIZE + (size_t)COL540_TC * COL540_XLP + 2 * (size_t)Col540X::N) * sizeof(float2) +
-                                4 * COL540_TC * (sizeof(int) + (size_t)raw_stride);
-        if (x_col540(ctx, g, col_tiles) && dtype == BS_DTYPE_U16 && (row_bytes % 16) == 0 && ((size_t)d1 % 16) == 0 &&
-            ((size_t)d2 % 16) == 0 && smem_col <= PCM_SMEM_MAX) {
-            XR2CCol540Args c;
-            c.x = a;
-            c.row_bytes = row_bytes;
-            c.raw_stride = raw_stride;
-            c.n_tiles = col_tiles;
-            k_fft_x_r2c_col540<<<std::min(col_tiles, ctx->sm_count), COL540X_NT, smem_col, ctx->stream>>>(c);
+        XR2CCol540Args c;
+        size_t smem_col;
+        if (r2c_col540(ctx, a, dtype, g, &c, &smem_col)) {
+            k_fft_x_r2c_col540<<<std::min(c.n_tiles, ctx->sm_count), COL540X_NT, smem_col, ctx->stream>>>(c);
             pass_info(info, "k_fft_x_r2c_col540", nullptr);
         } else if (xmode && g.M <= 32 * XW_MAXV - 1 && smem_w <= PCM_SMEM_MAX && (((size_t)g.P[0] + 16 * (size_t)g.M) * 8) % 16 == 0) {
             XWArgs w;
@@ -2391,13 +2603,97 @@ static int pcm_pass_x_c2r(bs_ctx* ctx, const PcmGeometry& g, PcmDeviceTables* t,
     return BS_OK;
 }
 
-// forward pipeline up to the real PCM in ws.spec_a (row pitch 2*pitch floats)
+// k_fft_xy_col540 takes over from passes 0 + 1 when k_fft_x_r2c_col540 would run, Py = 540 (static_y) and one CTA
+// of the fused kernel fits on every SM.  BS_FFT_XY_FUSE: 1 (default) applies that rule, 0 keeps the five-pass chain.
+static int xy_fuse(bs_ctx* ctx, const PcmGeometry& g, const void* fn, size_t smem, bool* fuse) {
+    *fuse = false;
+    if (!env_int("BS_FFT_XY_FUSE", 1) || !g.static_y) return BS_OK;
+    int occ = 0;
+    BS_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, COL540X_NT, smem));
+    *fuse = occ >= 1;
+    return BS_OK;
+}
+
+// CTAs of k_fft_xy_col540's x role: 80 of 132 measured best (DESIGN.md), scaled to the SM count;
+// BS_FFT_XY_KX overrides it
+static int xy_split(bs_ctx* ctx) {
+    return std::max(1, std::min(ctx->sm_count - 1, env_int("BS_FFT_XY_KX", (80 * ctx->sm_count + 66) / 132)));
+}
+
+// counters in ws.sync; window: as many planes of plane_bytes as fill half of L2 (BS_FFT_XY_WINDOW overrides)
+static int make_handoff(bs_ctx* ctx, const PcmGeometry& g, int code, int ready_full, int done_full, size_t plane_bytes,
+                        Handoff* h) {
+    int l2 = 0;
+    BS_CUDA(ctx, cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, ctx->device));
+    h->err = (int*)ctx->ws.sync;
+    h->ready = h->err + PCM_SYNC_COUNTERS;
+    h->done = h->ready + g.P[2];
+    h->code = code;
+    h->ready_full = ready_full;
+    h->done_full = done_full;
+    h->window = std::max(2, env_int("BS_FFT_XY_WINDOW", (int)((size_t)l2 / 2 / plane_bytes)));
+    BS_CUDA(ctx, cudaMemsetAsync(h->ready, 0, 2 * sizeof(int) * g.P[2], ctx->stream));
+    return BS_OK;
+}
+
+// one CTA per SM, launched cooperatively: a grid that cannot be co-resident fails to launch instead of waiting on
+// CTAs that never start
+template <class Args>
+static int launch_fused(bs_ctx* ctx, void (*fn)(Args), const Args& args, size_t smem) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(ctx->sm_count);
+    cfg.blockDim = dim3(COL540X_NT);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = ctx->stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeCooperative;
+    attr[0].val.cooperative = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    BS_CUDA(ctx, cudaLaunchKernelEx(&cfg, fn, args));
+    return BS_OK;
+}
+
+static void join_info(char* info, const char* a, const char* b) {
+    if (info) snprintf(info, PCM_INFO_LEN, "%s + %s", a, b);
+}
+
+// passes 0 + 1: k_fft_xy_col540 when the rule above takes them, else the two passes
+static int pcm_pass_xy(bs_ctx* ctx, const void* d1, const void* d2, int dtype, const PcmGeometry& g, PcmDeviceTables* t,
+                       char* info) {
+    XYCol540Args f;
+    size_t smem;
+    bool fuse = false;
+    int rc;
+    if (r2c_col540(ctx, r2c_args(ctx, d1, d2, dtype, g, t), dtype, g, &f.x, &smem) &&
+        (rc = xy_fuse(ctx, g, (const void*)k_fft_xy_col540, smem, &fuse)))
+        return rc;
+    if (!fuse) {
+        char i0[PCM_INFO_LEN] = "", i1[PCM_INFO_LEN] = "";
+        if ((rc = pcm_pass_x_r2c(ctx, d1, d2, dtype, g, t, i0))) return rc;
+        if ((rc = pcm_pass_y_fwd(ctx, g, t, i1))) return rc;
+        join_info(info, i0, i1);
+        return BS_OK;
+    }
+    f.tw_y = t->tw[1];
+    f.kx = xy_split(ctx);
+    bs_launch_scope sc(ctx, "fft_xy");
+    if ((rc = make_handoff(ctx, g, PCM_HANDOFF_XY, g.P[1], 2 * (g.pitch / COL540_TC),
+                           2 * (size_t)g.P[1] * g.pitch * sizeof(float2), &f.h)) ||
+        (rc = launch_fused(ctx, k_fft_xy_col540, f, smem)))
+        return rc;
+    pass_info(info, "k_fft_xy_col540", nullptr);
+    return BS_OK;
+}
+
+
+// forward pipeline up to the real PCM in ws.spec_a (row pitch 2*pitch floats).  The caller resets the hand-off
+// error word (pcm_reset_handoff) before and checks it once the stream has passed the pair.
 static int pcm_compute_pcm(bs_ctx* ctx, const void* d1, const void* d2, int dtype, const PcmGeometry& g,
                            PcmDeviceTables* t) {
     int rc;
     if ((rc = pcm_kernel_attrs(ctx))) return rc;
-    if ((rc = pcm_pass_x_r2c(ctx, d1, d2, dtype, g, t, nullptr))) return rc;
-    if ((rc = pcm_pass_y_fwd(ctx, g, t, nullptr))) return rc;
+    if ((rc = pcm_pass_xy(ctx, d1, d2, dtype, g, t, nullptr))) return rc;
     if ((rc = pcm_pass_z_xpower(ctx, g, t, nullptr))) return rc;
     if ((rc = pcm_pass_y_inv(ctx, g, t, nullptr))) return rc;
     return pcm_pass_x_c2r(ctx, g, t, nullptr);
@@ -2473,7 +2769,7 @@ struct PcmPending {
     bs_pcm_params p;
     int dtype = 0;
     long long min_px = 0;
-    size_t off_sel = 0, off_cands = 0, off_sums = 0, slot_base = 0;
+    size_t off_sel = 0, off_cands = 0, off_sums = 0, off_err = 0, slot_base = 0;
 };
 
 struct PcmSlotState {
@@ -2574,6 +2870,7 @@ static int pcm_enqueue(bs_ctx* ctx, const void* d1, const void* d2, const long l
     PcmDeviceTables* t;
     if ((rc = pcm_tables(ctx, g, &t))) return rc;
     if ((rc = pcm_workspace(ctx, g))) return rc;
+    if ((rc = pcm_reset_handoff(ctx))) return rc;
     if ((rc = pcm_compute_pcm(ctx, d1, d2, dtype, g, t))) return rc;
 
     bs_pcm_workspace& ws = ctx->ws;
@@ -2595,6 +2892,7 @@ static int pcm_enqueue(bs_ctx* ctx, const void* d1, const void* d2, const long l
     pd.off_sums = off;  off += sizeof(unsigned long long) * 5 * 8 * PCM_KMAX;
     const size_t readback = off;
     const size_t off_ncand = off; off += 16;
+    pd.off_err = off;   off += 16;
     const size_t off_peaks = off; off += sizeof(PeakEntry) * (size_t)peak_ctas * K;
     if (off > slot_bytes) return bs_set_error(ctx, BS_ERR_NOMEM, "pcm: scratch too small");
     unsigned char* dsmall = (unsigned char*)ws.small + pd.slot_base;
@@ -2636,6 +2934,7 @@ static int pcm_enqueue(bs_ctx* ctx, const void* d1, const void* d2, const long l
                              dsmall + pd.off_sums, (int*)(dsmall + off_ncand))))
         return rc;
     BS_CUDA(ctx, cudaMemcpyAsync(hsmall, dsmall, readback, cudaMemcpyDeviceToHost, ctx->stream));
+    BS_CUDA(ctx, cudaMemcpyAsync(hsmall + pd.off_err, ws.sync, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     if (!S->done[slot]) BS_CUDA(ctx, cudaEventCreateWithFlags(&S->done[slot], cudaEventDisableTiming));
     BS_CUDA(ctx, cudaEventRecord(S->done[slot], ctx->stream));
     pd.active = true;
@@ -2654,6 +2953,8 @@ static int pcm_finish(bs_ctx* ctx, int slot, bs_pcm_result* out) {
     const PcmGeometry& g = pd.g;
     for (int d = 0; d < 3; ++d) out->pad[d] = g.P[d];
     const unsigned char* hsmall = (const unsigned char*)ctx->ws.small_host + pd.slot_base;
+    int rc = pcm_handoff_error(ctx, *(const int*)(hsmall + pd.off_err));
+    if (rc) return rc;
     const PcmSelect* sel = (const PcmSelect*)(hsmall + pd.off_sel);
     const unsigned long long* hsums = (const unsigned long long*)(hsmall + pd.off_sums);
     const int np = sel->np;
@@ -2932,10 +3233,11 @@ int bs_pcm_debug_pcm(bs_ctx* ctx, const void* img1, const void* img2, const long
     bs_pcm_workspace& ws = ctx->ws;
     BS_CUDA(ctx, cudaMemcpyAsync(ws.crop[0][0], img1, bytes, cudaMemcpyHostToDevice, ctx->stream));
     BS_CUDA(ctx, cudaMemcpyAsync(ws.crop[0][1], img2, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    if ((rc = pcm_reset_handoff(ctx))) return rc;
     if ((rc = pcm_compute_pcm(ctx, ws.crop[0][0], ws.crop[0][1], dtype, g, t))) return rc;
     BS_CUDA(ctx, cudaMemcpy2DAsync(out_pcm, sizeof(float) * g.P[0], ws.spec_a, sizeof(float2) * g.pitch,
                                    sizeof(float) * g.P[0], (size_t)g.P[1] * g.P[2], cudaMemcpyDeviceToHost, ctx->stream));
-    BS_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if ((rc = pcm_sync_handoff(ctx))) return rc;
     if (pad_out) for (int d = 0; d < 3; ++d) pad_out[d] = g.P[d];
     return BS_OK;
 }
@@ -2944,13 +3246,23 @@ int bs_pcm_debug_pass(bs_ctx* ctx, int pass, const long long dims[3], int dtype,
                       const void* in_b, void* out_a, void* out_b, int poison, int pad_out[3], char info[128]) {
     if (!ctx) return BS_ERR_ARG;
     std::lock_guard<std::mutex> lk(ctx->mu);
-    if (pass < 0 || pass > 4) return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_debug_pass: pass %d not in [0,4]", pass);
-    const bool two = pass <= 2;          // passes 0..2 read both spectra / crops
-    if (!dims || !extension || !in_a || (two && !in_b) || !out_a || (pass <= 1 && !out_b))
+    if (pass < 0 || pass > 5) return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_debug_pass: pass %d not in [0,5]", pass);
+    const bool crops = pass == 0 || pass == 5;
+    const bool two = pass <= 2 || pass == 5;    // read both spectra / crops
+    const bool two_out = pass <= 1 || pass == 5;
+    const bool real_out = pass == 4;
+    if (!dims || !extension || !in_a || (two && !in_b) || !out_a || (two_out && !out_b))
         return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_debug_pass: NULL argument");
-    if (pass == 0 && dtype != BS_DTYPE_U16 && dtype != BS_DTYPE_F32 && dtype != BS_DTYPE_U8)
+    if (crops && dtype != BS_DTYPE_U16 && dtype != BS_DTYPE_F32 && dtype != BS_DTYPE_U8)
         return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_debug_pass: bad dtype %d", dtype);
     BS_CUDA(ctx, cudaSetDevice(ctx->device));
+    for (int i = 0; crops && i < 2; ++i) {   // the x kernels read the crops directly
+        cudaPointerAttributes pa;
+        BS_CUDA(ctx, cudaPointerGetAttributes(&pa, i ? in_b : in_a));
+        if (pa.type != cudaMemoryTypeDevice && pa.type != cudaMemoryTypeManaged)
+            return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_debug_pass: pass %d takes device crops (in_%c)", pass,
+                                i ? 'b' : 'a');
+    }
     PcmGeometry g;
     int rc = pcm_geometry(ctx, dims, extension, &g);
     if (rc) return rc;
@@ -2965,7 +3277,8 @@ int bs_pcm_debug_pass(bs_ctx* ctx, int pass, const long long dims[3], int dtype,
     const void* in[2] = {in_a, in_b};
     void* out[2] = {out_a, out_b};
     for (int i = 0; i < 2; ++i) BS_CUDA(ctx, cudaMemsetAsync(spec[i], poison ? 0xff : 0, spec_bytes, ctx->stream));
-    if (pass >= 1)
+    if ((rc = pcm_reset_handoff(ctx))) return rc;
+    if (!crops)
         for (int i = 0; i < (two ? 2 : 1); ++i)
             BS_CUDA(ctx, cudaMemcpy2DAsync(spec[i], sizeof(float2) * g.pitch, in[i], row, row, rows, cudaMemcpyHostToDevice,
                                            ctx->stream));
@@ -2975,18 +3288,19 @@ int bs_pcm_debug_pass(bs_ctx* ctx, int pass, const long long dims[3], int dtype,
         case 1: rc = pcm_pass_y_fwd(ctx, g, t, buf); break;
         case 2: rc = pcm_pass_z_xpower(ctx, g, t, buf); break;
         case 3: rc = pcm_pass_y_inv(ctx, g, t, buf); break;
-        default: rc = pcm_pass_x_c2r(ctx, g, t, buf); break;
+        case 4: rc = pcm_pass_x_c2r(ctx, g, t, buf); break;
+        default: rc = pcm_pass_xy(ctx, in_a, in_b, dtype, g, t, buf); break;
     }
     if (rc) return rc;
-    if (pass == 4) {
+    if (real_out) {
         BS_CUDA(ctx, cudaMemcpy2DAsync(out_a, sizeof(float) * g.P[0], ws.spec_a, sizeof(float2) * g.pitch,
                                        sizeof(float) * g.P[0], rows, cudaMemcpyDeviceToHost, ctx->stream));
     } else {
-        for (int i = 0; i < (pass <= 1 ? 2 : 1); ++i)
+        for (int i = 0; i < (two_out ? 2 : 1); ++i)
             BS_CUDA(ctx, cudaMemcpy2DAsync(out[i], row, spec[i], sizeof(float2) * g.pitch, row, rows,
                                            cudaMemcpyDeviceToHost, ctx->stream));
     }
-    BS_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if ((rc = pcm_sync_handoff(ctx))) return rc;
     if (pad_out) for (int d = 0; d < 3; ++d) pad_out[d] = g.P[d];
     if (info) memcpy(info, buf, PCM_INFO_LEN);
     return BS_OK;

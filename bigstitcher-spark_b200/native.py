@@ -366,20 +366,23 @@ class Context:
 
     def pcm_debug_pass(self, pass_no: int, dims_xyz, in_a, in_b=None, dtype=None, extension=(10, 10, 10), poison=True):
         """Run one FFT pass of the PCM pipeline with the production launch (include/bsgpu.h bs_pcm_debug_pass states
-        what each pass computes).  Pass 0 takes two device crops ([z,y,x] CUDA tensors or int device pointers with
-        ``dtype``); passes 1-4 take host complex64 spectra [Pz, Py, M+1].  Returns (out_a, out_b, info): complex64
-        spectra (out_b is None from pass 2 on), or for pass 4 the float32 PCM [Pz, Py, Px] as out_a."""
+        what each pass computes).  Passes 0 and 5 take two device crops ([z,y,x] CUDA tensors or int device pointers
+        with ``dtype``); passes 1-4 take host complex64 spectra [Pz, Py, M+1].  Returns (out_a, out_b, info):
+        complex64 spectra (out_b is None from pass 2 to 4), or for pass 4 the float32 PCM [Pz, Py, Px] as out_a."""
         dims = (C.c_longlong * 3)(*[int(v) for v in dims_xyz])
         ext = (C.c_int * 3)(*[int(e) for e in extension])
         P = [good_fft_size(d + (2 * d if d < e else 2 * e), i == 0) for i, (d, e) in enumerate(zip(dims_xyz, extension))]
         M = P[0] // 2
         spec_shape = (P[2], P[1], M + 1)
         keep = []
-        if pass_no == 0:
-            (pa, da, _), (pb, db, _) = _ptr_of(in_a), _ptr_of(in_b)
-            if not (da and db):
-                raise ValueError("pass 0 takes device crops")
-            dt = _bs_dtype(in_a, dtype)
+        if pass_no in (0, 5):
+            # the library rejects crops that are not device memory or not of an image dtype
+            (pa, _, ka), (pb, _, kb) = _ptr_of(in_a), _ptr_of(in_b)
+            keep += [ka, kb]
+            try:
+                dt = _bs_dtype(in_a, dtype)
+            except KeyError:
+                dt = -1
         else:
             dt = DTYPE_F32
             ins = [in_a] + ([in_b] if pass_no <= 2 else [])
@@ -391,7 +394,7 @@ class Context:
             pa = keep[0].ctypes.data
             pb = keep[1].ctypes.data if len(keep) > 1 else None
         out_a = np.empty((P[2], P[1], P[0]), np.float32) if pass_no == 4 else np.empty(spec_shape, np.complex64)
-        out_b = np.empty(spec_shape, np.complex64) if pass_no <= 1 else None
+        out_b = np.empty(spec_shape, np.complex64) if pass_no in (0, 1, 5) else None
         pad = (C.c_int * 3)()
         info = C.create_string_buffer(128)
         self._check(self.lib.bs_pcm_debug_pass(self.h, int(pass_no), dims, dt, ext, pa, pb, out_a.ctypes.data,

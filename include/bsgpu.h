@@ -147,8 +147,11 @@ int bs_pcm_debug_pcm(bs_ctx* ctx, const void* img1, const void* img2, const long
  *                    out = irfft(conj(H), P[0]) / (P[1] P[2])   (numpy's irfft, 1 / P[0] normalised; the kernel
  *                    scales its half-length transform by 1 / (M P[1] P[2])).  As in any C2R the imaginary parts of
  *                    bins 0 and M are expected to be 0.
+ *   pass 5  x R2C + y.   As pass 1 after pass 0, from the same inputs to the same outputs, as the pipeline runs the
+ *                    two (one fused kernel, k_fft_xy_col540, where it applies; the two passes otherwise).
  * The conjugations make passes 3 and 4 the inverse transforms: pass4(pass3(pass2(pass1(pass0(a, b))))) is the PCM
  * irfftn(n(rfftn A) conj(n(rfftn B))) of bs_pcm_debug_pcm.
+ * BS_ERR_ARG when the crops of passes 0 and 5 are not device memory.
  * in_b / out_b are ignored (may be NULL) for passes 3 and 4, out_b also for pass 2.  poison != 0 fills the device
  * spectra with NaN bytes first, so anything a pass fails to write shows up as NaN.  info (may be NULL) receives the
  * kernel instantiation launched, and for runtime-planned kernels the radices of the plan, e.g.
