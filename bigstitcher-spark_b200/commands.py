@@ -8,6 +8,7 @@
   nonrigid_fusion         J/SparkNonRigidFusion.java:124-446     (MLS grids from interest-point correspondences)
   detect_interestpoints   J/SparkInterestPointDetection.java:173-964 (block-wise DoG, interestpoints.n5 + the XML)
   match_interestpoints    J/SparkGeometricDescriptorMatching.java:161-545 (PRECISE_TRANSLATION, correspondences)
+  solver                  J/Solver.java:161-432                   (ONE_ROUND_SIMPLE / ONE_ROUND_ITERATIVE, registrations)
 
 No argument parsing here (the picocli layer is out of scope); keyword names follow the CLI flags.
 """
@@ -24,7 +25,7 @@ from . import fusion as bf
 from . import n5 as bn5
 from . import zarr as bzarr
 from . import matching as bm
-from . import native, stitching as bst
+from . import native, solver as bsolver, stitching as bst
 from .native import Context
 from .spimdata import SpimData2
 
@@ -727,9 +728,10 @@ class _InterestPoints:
     """Every selected view's points and correspondences of the `-ip` labels, read once from interestpoints.n5, with
     their world positions (the view's registration applied to the full-resolution pixel location)."""
 
-    def __init__(self, store: bn5.N5Store, view_ids, labels, registrations):
+    def __init__(self, store: bn5.N5Store, view_ids, labels, registrations, tables=False):
+        """``tables``: keep each view's correspondences as arrays (``table``, ``ids``) instead of the row list ``corr``."""
         self.labels = list(labels)
-        self.loc, self.world, self.index, self.corr = {}, {}, {}, {}
+        self.loc, self.world, self.index, self.corr, self.table, self.ids = {}, {}, {}, {}, {}, {}
         for v in view_ids:
             for label in self.labels:
                 group = f"tpId_{v[0]}_viewSetupId_{v[1]}/{label}"
@@ -740,6 +742,10 @@ class _InterestPoints:
                 M = np.asarray(registrations[v], dtype=np.float64).reshape(3, 4)
                 self.loc[(v, label)] = loc
                 self.world[(v, label)] = loc @ M[:, :3].T + M[:, 3]
+                self.ids[(v, label)] = ids
+                if tables:
+                    self.table[(v, label)] = store.read_correspondence_table(group)
+                    continue
                 self.index[(v, label)] = {int(i): k for k, i in enumerate(ids)}
                 self.corr[(v, label)] = store.read_correspondences(group)
 
@@ -1062,3 +1068,26 @@ def write_match_correspondences(store, ips, views, labels, results, clear=False)
     for (v, lab), rs in sorted(rows.items()):
         ordered = sorted(rs, key=lambda r: (r[0], r[1][0], r[1][1], r[2], r[3]))
         store.write_correspondences(f"tpId_{v[0]}_viewSetupId_{v[1]}/{lab}", ordered)
+
+
+# --------------------------------------------------------------------------------------------- solver
+def solver(xml_path, ctx: Context, source, labels=None, label_weights=None, method="ONE_ROUND_SIMPLE",
+           transformation_model="AFFINE", regularization_model="RIGID", regularization_lambda=0.1, max_error=5.0,
+           max_iterations=10000, max_plateau_width=200, relative_threshold=3.5, absolute_threshold=7.0, fixed_views=None,
+           disable_fixed_views=False, group_tiles=None, group_illums=None, group_channels=None, split_timepoints=None,
+           registration_tp="TIMEPOINTS_INDIVIDUALLY", view_selection=None, dry_run=False):
+    """`./solver -x dataset.xml -s STITCHING|IP [-l beads [-lw 1.0]] [--method ONE_ROUND_SIMPLE|ONE_ROUND_ITERATIVE]
+    [-tm AFFINE] [-rm RIGID] [--lambda 0.1] [--maxError 5.0] [--maxIterations 10000] [--maxPlateauwidth 200]
+    [--relativeThreshold 3.5] [--absoluteThreshold 7.0] [-fv 'tp,setup' | --disableFixedViews] [--groupTiles]
+    [--groupIllums] [--groupChannels] [--splitTimepoints] [--dryRun]` (J/Solver.java:161-432): global optimisation of
+    the stored stitching results or interest-point correspondences.  The matches are built and the tiles pre-aligned on
+    the host; the relaxation runs on the device (bs_solve_tiles).  Every view of a solved tile gets the tile's model as
+    a new first <ViewTransform>; the XML is saved (with a ~1 backup) unless ``dry_run``.  Returns dict(models={view:
+    3 x 4}, removed=[(views A, views B)] (ONE_ROUND_ITERATIVE), stats) -- stats holds iterations, the final error,
+    skipped fits, stale stitching results and the views without links, which keep their registration.
+
+    TWO_ROUND_SIMPLE / TWO_ROUND_ITERATIVE and -rtp other than TIMEPOINTS_INDIVIDUALLY raise NotImplementedError."""
+    return bsolver.run(xml_path, ctx, source, labels, label_weights, method, transformation_model, regularization_model,
+                       regularization_lambda, max_error, max_iterations, max_plateau_width, relative_threshold,
+                       absolute_threshold, fixed_views, disable_fixed_views, group_tiles, group_illums, group_channels,
+                       split_timepoints, registration_tp, view_selection, dry_run)

@@ -35,16 +35,19 @@ class Model:
         self.min_matches = MIN_MATCHES[self.tm] if self.rm == "NONE" else max(MIN_MATCHES[self.tm],
                                                                              MIN_MATCHES[self.rm])
 
-    def fit(self, a, b):
-        """Batched fit: a, b (H, m, 3) -> (models (H, 3, 4), ok (H,) bool; False = singular / ill-defined)."""
-        M, ok = _fit(self.tm, a, b)
+    def fit(self, a, b, w=None):
+        """Batched fit: a, b (H, m, 3) -> (models (H, 3, 4), ok (H,) bool; False = singular / ill-defined).
+        ``w`` (H, m): match weights (the solver's fits); None fits every match with weight 1."""
+        M, ok = _fit(self.tm, a, b, w)
         if self.rm == "NONE":
             return M, ok
-        R, okr = _fit(self.rm, a, b)
+        R, okr = _fit(self.rm, a, b, w)
         return (1.0 - self.lam) * M + self.lam * R, ok & okr
 
 
-def _fit(kind, a, b):
+def _fit(kind, a, b, w=None):
+    if w is not None:
+        return _fit_weighted(kind, a, b, np.asarray(w, dtype=np.float64))
     H = a.shape[0]
     ca, cb = a.mean(axis=1), b.mean(axis=1)
     M = np.zeros((H, 3, 4))
@@ -72,10 +75,47 @@ def _fit(kind, a, b):
     return M, ok
 
 
+def _fit_weighted(kind, a, b, w):
+    """The fits of _fit with weighted centroids and moments, as the solver's tiles fit them.  Singular: total weight
+    <= 0; RIGID when the centred points are (numerically) collinear, i.e. the second invariant of P = sum w a_c a_c^T is
+    <= 1e-12 (trace P)^2; AFFINE with _fit's determinant test on P."""
+    H = a.shape[0]
+    W = w.sum(axis=1)
+    ok = W > 0
+    Ws = np.where(ok, W, 1.0)
+    ca = np.einsum("hm,hmi->hi", w, a) / Ws[:, None]
+    cb = np.einsum("hm,hmi->hi", w, b) / Ws[:, None]
+    M = np.zeros((H, 3, 4))
+    if kind in ("IDENTITY", "TRANSLATION"):
+        M[:, :, :3] = np.eye(3)
+        if kind == "TRANSLATION":
+            M[:, :, 3] = cb - ca
+        return M, ok if kind == "TRANSLATION" else np.ones(H, dtype=bool)
+    ac, bc = a - ca[:, None], b - cb[:, None]
+    P = np.einsum("hm,hmi,hmj->hij", w, ac, ac)
+    S = np.einsum("hm,hmi,hmj->hij", w, ac, bc)
+    tr = np.trace(P, axis1=1, axis2=2)
+    if kind == "RIGID":
+        i2 = (P[:, 0, 0] * P[:, 1, 1] - P[:, 0, 1] * P[:, 1, 0] + P[:, 0, 0] * P[:, 2, 2] - P[:, 0, 2] * P[:, 2, 0] +
+              P[:, 1, 1] * P[:, 2, 2] - P[:, 1, 2] * P[:, 2, 1])
+        ok &= i2 > 1e-12 * tr * tr
+        return _rigid_from_cov(S, ca, cb), ok
+    det = np.linalg.det(P)
+    ok &= np.isfinite(det) & (det > 1e-12 * (tr / 3.0) ** 3)
+    Ps = np.where(ok[:, None, None], P, np.eye(3))
+    A = np.swapaxes(np.linalg.solve(Ps, S), 1, 2)
+    M[:, :, :3] = A
+    M[:, :, 3] = cb - np.einsum("hij,hj->hi", A, ca)
+    return M, ok
+
+
 def _fit_rigid(ac, bc, ca, cb):
     """Horn's closed form: the rotation is the quaternion of the largest eigenvalue of the 4 x 4 matrix N of the
     centred cross-covariance S = sum a b^T."""
-    S = np.einsum("hmi,hmj->hij", ac, bc)
+    return _rigid_from_cov(np.einsum("hmi,hmj->hij", ac, bc), ca, cb)
+
+
+def _rigid_from_cov(S, ca, cb):
     xx, xy, xz = S[:, 0, 0], S[:, 0, 1], S[:, 0, 2]
     yx, yy, yz = S[:, 1, 0], S[:, 1, 1], S[:, 1, 2]
     zx, zy, zz = S[:, 2, 0], S[:, 2, 1], S[:, 2, 2]

@@ -245,16 +245,21 @@ class N5Store:
         the uint64 dataset `correspondences/data` {3, M} of (detectionId, correspondingDetectionId, idMap index) rows and
         the group attribute idMap {"tp,setup,label": index}.  Returns a list of (detection id, (tp, setup), label,
         corresponding detection id); [] when the view has no correspondences (dataset {0} or absent)."""
+        rows, keys = self.read_correspondence_table(group)
+        return [(int(a), keys[int(c)][0], keys[int(c)][1], int(b)) for a, b, c in rows]
+
+    def read_correspondence_table(self, group):
+        """The same correspondences as arrays: (uint64 (M, 3) rows of (detection id, corresponding detection id, idMap
+        index), {idMap index: ((tp, setup), label)})."""
         path = group.rstrip("/") + "/correspondences"
         attrs = self.get_attributes(path)
         if "idMap" not in attrs or "dimensions" not in self.get_attributes(path + "/data"):
-            return []
+            return np.zeros((0, 3), dtype=np.uint64), {}
         keys = {}
         for k, idx in attrs["idMap"].items():
             tp, setup, label = k.split(",", 2)
             keys[int(idx)] = ((int(tp), int(setup)), label)
-        rows = self.read_list(path + "/data")
-        return [(int(a), keys[int(c)][0], keys[int(c)][1], int(b)) for a, b, c in rows]
+        return np.asarray(self.read_list(path + "/data"), dtype=np.uint64).reshape(-1, 3), keys
 
     def write_correspondences(self, group, rows):
         """The inverse of read_correspondences: ``rows`` [(detection id, (tp, setup), label, corresponding detection id)]

@@ -70,6 +70,20 @@ class DogPointC(C.Structure):
                 ("pad", C.c_int)]
 
 
+class SolveParamsC(C.Structure):
+    _fields_ = [("transformation", C.c_int), ("regularization", C.c_int), ("lam", C.c_double), ("max_error", C.c_double),
+                ("max_iterations", C.c_int), ("max_plateau_width", C.c_int)]
+
+
+class SolveStatsC(C.Structure):
+    _fields_ = [("iterations", C.c_int), ("stopped", C.c_int), ("skipped_fits", C.c_longlong), ("error", C.c_double),
+                ("blocks", C.c_int), ("models_in_shared", C.c_int)]
+
+
+#: model kinds of bs_solve_params (BS_MODEL_* in include/bsgpu.h)
+SOLVE_MODELS = {"NONE": -1, "IDENTITY": 0, "TRANSLATION": 1, "RIGID": 2, "AFFINE": 3}
+
+
 class PcmJobC(C.Structure):
     _fields_ = [("vol1", C.c_ulonglong), ("vol2", C.c_ulonglong), ("min1", C.c_longlong * 3),
                 ("min2", C.c_longlong * 3), ("dims", C.c_longlong * 3)]
@@ -115,6 +129,7 @@ SYMBOLS = [
     "bs_dog_debug_dog", "bs_comm_unique_id", "bs_comm_init", "bs_comm_destroy", "bs_fuse_allreduce",
     "bs_downsample_float", "bs_median_divide", "bs_sample_nlinear", "bs_nonrigid_fuse_blocks", "bs_nonrigid_debug_grid",
     "bs_descriptors_build", "bs_descriptors_free", "bs_descriptors_neighbors", "bs_descriptors_match",
+    "bs_solve_tiles",
 ]
 
 #: fixed parameters of the reference's non-rigid fusion (J/SparkNonRigidFusion.java:373-383): control-point distance
@@ -196,6 +211,8 @@ def load_library():
     lib.bs_descriptors_free.argtypes = [vp, ull]
     lib.bs_descriptors_neighbors.argtypes = [vp, ull, P(ip), P(dbl)]
     lib.bs_descriptors_match.argtypes = [vp, ull, ull, dbl, P(ip), P(dbl), P(dbl)]
+    lib.bs_solve_tiles.argtypes = [vp, ip, ip, P(ip), P(ip), P(ip), ip, P(ip), P(ll), P(dbl), P(dbl), P(dbl),
+                                   P(SolveParamsC), P(dbl), P(SolveStatsC), P(dbl), P(dbl), P(dbl)]
     _lib = lib
     return lib
 
@@ -745,6 +762,37 @@ class Context:
     def descriptors_free(self, handle: int):
         self._check(self.lib.bs_descriptors_free(self.h, handle))
         self._desc_shape.pop(handle, None)
+
+    # -- solver
+    def solve_tiles(self, colour_offsets, colour_tiles, fixed, links, match_offsets, p, q, w, models,
+                    transformation="AFFINE", regularization="RIGID", lam=0.1, max_error=5.0, max_iterations=10000,
+                    max_plateau_width=200):
+        """The device relaxation of one solve (include/bsgpu.h bs_solve_tiles) from the starting ``models`` (T, 3, 4).
+        Returns (models (T, 3, 4), stats dict, tile_error (T,), link_mean (L,), link_max (L,))."""
+        def arr(x, dt, shape=(-1,)):
+            return np.ascontiguousarray(np.asarray(x, dtype=dt).reshape(shape))
+        co, ct, fx = arr(colour_offsets, np.int32), arr(colour_tiles, np.int32), arr(fixed, np.int32)
+        lk, mo = arr(links, np.int32, (-1, 2)), arr(match_offsets, np.int64)
+        pp, qq, ww = arr(p, np.float64, (-1, 3)), arr(q, np.float64, (-1, 3)), arr(w, np.float64)
+        M = np.array(models, dtype=np.float64).reshape(-1, 3, 4).copy()
+        T, L = len(M), len(lk)
+        if len(co) < 1:
+            raise ValueError("colour_offsets needs at least one entry")
+        prm = SolveParamsC(SOLVE_MODELS[transformation.upper()], SOLVE_MODELS[regularization.upper()], float(lam),
+                           float(max_error), int(max_iterations), int(max_plateau_width))
+        st = SolveStatsC()
+        te, lm, lx = np.zeros(T), np.zeros(max(L, 1)), np.zeros(max(L, 1))
+        I, LL, D = C.POINTER(C.c_int), C.POINTER(C.c_longlong), C.POINTER(C.c_double)
+        if L and len(mo) != L + 1:
+            raise ValueError("match_offsets needs n_links + 1 entries")
+        self._check(self.lib.bs_solve_tiles(self.h, T, len(co) - 1, co.ctypes.data_as(I), ct.ctypes.data_as(I),
+                                            fx.ctypes.data_as(I), L, lk.ctypes.data_as(I), mo.ctypes.data_as(LL),
+                                            pp.ctypes.data_as(D), qq.ctypes.data_as(D), ww.ctypes.data_as(D), C.byref(prm),
+                                            M.ctypes.data_as(D), C.byref(st), te.ctypes.data_as(D), lm.ctypes.data_as(D),
+                                            lx.ctypes.data_as(D)))
+        stats = dict(iterations=st.iterations, error=st.error, skipped_fits=st.skipped_fits, stopped=bool(st.stopped),
+                     blocks=st.blocks, models_in_shared=bool(st.models_in_shared))
+        return M, stats, te, lm[:L], lx[:L]
 
     @staticmethod
     def comm_unique_id() -> bytes:

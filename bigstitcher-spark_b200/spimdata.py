@@ -97,6 +97,20 @@ class SpimData2:
             M = M @ np.vstack([m, [0, 0, 0, 1]])
         return M[:3, :].copy()
 
+    def add_registration(self, view, name, M):
+        """Preconcatenate the 3 x 4 affine ``M``: a new <ViewTransform> at index 0 of the view's list, applied last."""
+        m = np.asarray(M, dtype=np.float64).reshape(3, 4).copy()
+        for vr in self.root.find("ViewRegistrations").findall("ViewRegistration"):
+            if (int(vr.get("timepoint")), int(vr.get("setup"))) == tuple(view):
+                vt = ET.Element("ViewTransform", type="affine")
+                ET.SubElement(vt, "Name").text = name
+                ET.SubElement(vt, "affine").text = _fmt(m.ravel())
+                first = vr.find("ViewTransform")
+                vr.insert(list(vr).index(first) if first is not None else len(vr), vt)
+                self.registrations[tuple(view)].insert(0, (name, m))
+                return
+        raise KeyError(f"no ViewRegistration for {view}")
+
     def view_ids(self):
         return sorted(self.registrations)
 

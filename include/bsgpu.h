@@ -394,6 +394,54 @@ int bs_descriptors_neighbors(bs_ctx* ctx, unsigned long long handle, int* idx, d
 int bs_descriptors_match(bs_ctx* ctx, unsigned long long ha, unsigned long long hb, double search_radius,
                          int* best_b, double* best, double* second);
 
+/* ---------------------------------------------------------------- solver
+ * The relaxation of the global optimisation (TileConfiguration.optimize behind J/Solver.java:352-395) in FP64: tiles
+ * joined by links, each link a list of weighted point matches p (its first tile) <-> q (its second tile), world
+ * coordinates.  Each iteration fits every non-fixed tile, colour by colour, to M_t(own point) ~ M_u(partner point) with
+ * its partners' current models (a multicolour Gauss-Seidel sweep: no link may join two tiles of one colour), then takes
+ * every match's distance d = |M_a p - M_b q|, each tile's error sum w d / sum w over its links' matches and
+ * E = the mean tile error.  After iteration i > max_plateau_width it stops unless E_i > max_error or
+ * |E_i - E_{i-d}| / d > 1e-4 for some d = max_plateau_width, max_plateau_width / 2, ... >= 1.  The model is
+ * transformation, or (1 - lambda) transformation + lambda regularization; fits are weighted.  A tile with fewer matches
+ * than the model needs, zero total weight, or a singular fit (AFFINE: det P <= 1e-12 (trace P / 3)^3; RIGID: second
+ * invariant of P <= 1e-12 trace(P)^2, P the tile's centred weighted second moments) keeps its model and is counted in
+ * skipped_fits.  Bit-identical between runs.  Additive: the ABI version stays 107.  Profile tags "solve_moments",
+ * "solve". */
+#define BS_MODEL_NONE        -1   /* regularization only */
+#define BS_MODEL_IDENTITY     0   /* regularization only */
+#define BS_MODEL_TRANSLATION  1
+#define BS_MODEL_RIGID        2
+#define BS_MODEL_AFFINE       3
+
+typedef struct {
+    int    transformation;      /* BS_MODEL_TRANSLATION / RIGID / AFFINE (-tm) */
+    int    regularization;      /* BS_MODEL_NONE / IDENTITY / TRANSLATION / RIGID / AFFINE (-rm) */
+    double lambda;              /* --lambda, in [0, 1] */
+    double max_error;           /* --maxError; +inf stops on the plateau alone */
+    int    max_iterations;      /* --maxIterations, >= 1 */
+    int    max_plateau_width;   /* --maxPlateauwidth, >= 0 */
+} bs_solve_params;
+
+typedef struct {
+    int       iterations;       /* iterations run */
+    int       stopped;          /* 1: the stopping rule ended the solve; 0: max_iterations did */
+    long long skipped_fits;     /* fits that kept the tile's model, summed over iterations */
+    double    error;            /* E of the last iteration */
+    int       blocks;           /* CTAs of the persistent solve kernel */
+    int       models_in_shared; /* 1: the distance pass read the models from shared memory */
+} bs_solve_stats;
+
+/* n_tiles >= 1 tiles in n_colours colours: colour c holds tiles colour_tiles[colour_offsets[c] .. colour_offsets[c + 1]).
+ * fixed[n_tiles]: non-zero tiles keep their model.  links[2 * n_links]: the two tiles of each link; the matches of link l
+ * are rows match_offsets[l] .. match_offsets[l + 1] of p, q (3 doubles {x, y, z} each) and w (weights >= 0).
+ * models[12 * n_tiles]: row-packed 3 x 4 models, the starting values in and the solution out.  tile_error[n_tiles] and,
+ * per link, link_mean (sum w d / sum w) and link_max (max d) receive the values of the last iteration.  BS_ERR_ARG for a
+ * bad colouring, link, count, parameter or a non-finite input. */
+int bs_solve_tiles(bs_ctx* ctx, int n_tiles, int n_colours, const int* colour_offsets, const int* colour_tiles,
+                   const int* fixed, int n_links, const int* links, const long long* match_offsets, const double* p,
+                   const double* q, const double* w, const bs_solve_params* params, double* models,
+                   bs_solve_stats* stats, double* tile_error, double* link_mean, double* link_max);
+
 #ifdef __cplusplus
 }
 #endif

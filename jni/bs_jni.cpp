@@ -668,3 +668,48 @@ JF(void, descriptorsMatch)(JNIEnv* env, jclass, jlong ctx, jlong ha, jlong hb, j
     env->SetDoubleArrayRegion(best, 0, n, b.data());
     env->SetDoubleArrayRegion(second, 0, n, s.data());
 }
+
+// ---------------------------------------------------------------------------------------------------------------- solver
+// the relaxation of the global optimisation (J/Solver.java:352-395): iparams = {transformation, regularization,
+// maxIterations, maxPlateauwidth} (BS_MODEL_*), dparams = {lambda, maxError}; links int[2 * nLinks], matchOffsets
+// long[nLinks + 1], p / q double[3 * nMatches], w double[nMatches]; models double[12 * nTiles] in and out; returns
+// {iterations, stopped, skippedFits, error}
+JF(jdoubleArray, solveTiles)(JNIEnv* env, jclass, jlong ctx, jintArray colourOffsets, jintArray colourTiles, jintArray fixed,
+                             jintArray links, jlongArray matchOffsets, jdoubleArray p, jdoubleArray q, jdoubleArray w,
+                             jintArray iparams, jdoubleArray dparams, jdoubleArray models, jdoubleArray tileError,
+                             jdoubleArray linkMean, jdoubleArray linkMax) {
+    auto ints = [&](jintArray a) {
+        std::vector<jint> v((size_t)env->GetArrayLength(a));
+        if (!v.empty()) env->GetIntArrayRegion(a, 0, (jsize)v.size(), v.data());
+        return std::vector<int>(v.begin(), v.end());
+    };
+    auto dbls = [&](jdoubleArray a) {
+        std::vector<jdouble> v((size_t)env->GetArrayLength(a));
+        if (!v.empty()) env->GetDoubleArrayRegion(a, 0, (jsize)v.size(), v.data());
+        return v;
+    };
+    const std::vector<int> co = ints(colourOffsets), ct = ints(colourTiles), fx = ints(fixed), lk = ints(links), ip = ints(iparams);
+    std::vector<jlong> mo((size_t)env->GetArrayLength(matchOffsets));
+    if (!mo.empty()) env->GetLongArrayRegion(matchOffsets, 0, (jsize)mo.size(), mo.data());
+    const std::vector<long long> moff(mo.begin(), mo.end());
+    const std::vector<jdouble> pp = dbls(p), qq = dbls(q), ww = dbls(w), dp = dbls(dparams);
+    std::vector<jdouble> m = dbls(models);
+    const int n_tiles = (int)ct.size(), n_links = (int)lk.size() / 2;
+    std::vector<jdouble> te((size_t)n_tiles), lm((size_t)n_links + 1), lx((size_t)n_links + 1);
+    bs_solve_params prm;
+    prm.transformation = ip[0]; prm.regularization = ip[1]; prm.max_iterations = ip[2]; prm.max_plateau_width = ip[3];
+    prm.lambda = dp[0]; prm.max_error = dp[1];
+    bs_solve_stats st;
+    if (failed(env, ctx, bs_solve_tiles(C(ctx), n_tiles, (int)co.size() - 1, co.data(), ct.data(), fx.data(), n_links, lk.data(),
+                                        moff.data(), pp.data(), qq.data(), ww.data(), &prm, m.data(), &st, te.data(), lm.data(),
+                                        lx.data())))
+        return nullptr;
+    env->SetDoubleArrayRegion(models, 0, (jsize)m.size(), m.data());
+    env->SetDoubleArrayRegion(tileError, 0, n_tiles, te.data());
+    env->SetDoubleArrayRegion(linkMean, 0, n_links, lm.data());
+    env->SetDoubleArrayRegion(linkMax, 0, n_links, lx.data());
+    const jdouble out[4] = {(jdouble)st.iterations, (jdouble)st.stopped, (jdouble)st.skipped_fits, st.error};
+    jdoubleArray r = env->NewDoubleArray(4);
+    env->SetDoubleArrayRegion(r, 0, 4, out);
+    return r;
+}

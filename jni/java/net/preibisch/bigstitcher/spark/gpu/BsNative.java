@@ -113,4 +113,12 @@ public final class BsNative
 	/** exhaustive search A -> B: per point of A the best B index (-1: none), its descriptor distance and the second best;
 	 *  searchRadius < 0: unlimited */
 	public static native void descriptorsMatch( long ctx, long ha, long hb, double searchRadius, long[] bestB, double[] best, double[] second );
+
+	/** solver (replaces TileConfiguration.optimize behind Solver): tiles colourOffsets / colourTiles, fixed flags, links
+	 *  int[2 * nLinks], matchOffsets long[nLinks + 1], p / q double[3 * nMatches], w double[nMatches]; iparams =
+	 *  {transformation, regularization, maxIterations, maxPlateauwidth}, dparams = {lambda, maxError}; models double[12 * nTiles]
+	 *  in and out; returns {iterations, stopped, skippedFits, error} */
+	public static native double[] solveTiles( long ctx, int[] colourOffsets, int[] colourTiles, int[] fixed, int[] links,
+			long[] matchOffsets, double[] p, double[] q, double[] w, int[] iparams, double[] dparams, double[] models,
+			double[] tileError, double[] linkMean, double[] linkMax );
 }
