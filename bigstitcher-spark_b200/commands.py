@@ -9,6 +9,9 @@
   detect_interestpoints   J/SparkInterestPointDetection.java:173-964 (block-wise DoG, interestpoints.n5 + the XML)
   match_interestpoints    J/SparkGeometricDescriptorMatching.java:161-545 (PRECISE_TRANSLATION, correspondences)
   solver                  J/Solver.java:161-432                   (ONE_ROUND_SIMPLE / ONE_ROUND_ITERATIVE, registrations)
+  resave                  J/SparkResaveN5.java:80-455             (OME-ZARR or BDV-N5 with the pyramid built on the device)
+
+Every command reads its images through viewsource.py, so `bdv.n5` and `bdv.multimg.zarr` datasets both work.
 
 No argument parsing here (the picocli layer is out of scope); keyword names follow the CLI flags.
 """
@@ -25,13 +28,9 @@ from . import fusion as bf
 from . import n5 as bn5
 from . import zarr as bzarr
 from . import matching as bm
-from . import native, solver as bsolver, stitching as bst
+from . import native, solver as bsolver, stitching as bst, viewsource as bvs
 from .native import Context
 from .spimdata import SpimData2
-
-
-def _load_views(data: SpimData2, store: bn5.N5Store, view_ids, level=0):
-    return {v: store.read_volume(bn5.bdv_dataset(v[1], v[0], level)) for v in view_ids}
 
 
 def stitching(xml_path, ctx: Context, downsampling=(2, 2, 1), peaks_to_check=5, disable_subpixel=False,
@@ -47,16 +46,13 @@ def stitching(xml_path, ctx: Context, downsampling=(2, 2, 1), peaks_to_check=5, 
     collective; ``allgather(obj) -> [obj of every rank]`` (e.g. torch.distributed.all_gather_object) merges the
     20-doubles-per-pair results and rank 0 writes the XML."""
     data = SpimData2.load(xml_path)
-    fmt, n5_path = data.image_loader()
-    if fmt != "bdv.n5":
-        raise NotImplementedError(f"ImageLoader format {fmt}")
-    store = bn5.N5Store(n5_path)
+    src = bvs.open_views(data)
     selected = data.select_views(**view_selection) if view_selection else None
     all_pairs = data.stitching_groups(selected)
     rank, world = shard
     pairs = all_pairs[rank::world]
     needed = sorted({v for p in pairs for g in p for v in g})
-    tiles = _load_views(data, store, needed)
+    tiles = {v: src.read_volume(v, 0) for v in needed}
     models = {v: data.model(*v) for v in needed}
     attributes = {v: data.setups[v[1]].attributes for v in needed}
     params = bst.PairwiseStitchingParameters(peaks_to_check=peaks_to_check, do_subpixel=not disable_subpixel)
@@ -183,13 +179,6 @@ class _Sink:
                     self.save(dataset, np.ascontiguousarray(cur), (gx, gy, gz))
 
 
-def _mipmap_info(src: bn5.N5Store, setup: int):
-    """downsamplingFactors of a BDV-N5 setup and the default mipmap transforms (scale f, shift (f - 1) / 2)."""
-    a = src.get_attributes(f"setup{setup}")
-    factors = [tuple(int(v) for v in f) for f in a.get("downsamplingFactors", [[1, 1, 1]])]
-    return factors, [bzarr.mipmap_transform_default(f) for f in factors]
-
-
 def _compose(reg, mt):
     R = np.vstack([np.asarray(reg, dtype=np.float64).reshape(3, 4), [0, 0, 0, 1]])
     M = np.vstack([np.asarray(mt, dtype=np.float64).reshape(3, 4), [0, 0, 0, 1]])
@@ -240,10 +229,7 @@ def affine_fusion(out_path, ctx: Context, fusion_type="AVG_BLEND", block_scale=(
     is_zarr = os.path.exists(os.path.join(out_path, ".zgroup"))
     store, meta = (bzarr.read_fusion_container_zarr if is_zarr else bn5.read_fusion_container)(out_path)
     data = SpimData2.load(meta["input_xml"])
-    fmt, n5_in = data.image_loader()
-    if fmt != "bdv.n5":
-        raise NotImplementedError(f"ImageLoader format {fmt}")
-    src = bn5.N5Store(n5_in)
+    src = bvs.open_views(data)
     nc, nt = int(meta["num_channels"]), int(meta["num_timepoints"])
     if nc != len(data.channels_ordered()) or nt != len(data.timepoints):
         raise ValueError(f"container says {nc} channel(s) / {nt} timepoint(s), the XML has "
@@ -293,12 +279,11 @@ def _fuse_volume_blockwise(ctx, data, src, sink, meta, levels, view_ids, fusion_
     # ---- per view: mipmap level by the reference's rule, level volume size, source -> world of that level
     info = {}
     for v in view_ids:
-        factors, mts = _mipmap_info(src, v[1])
+        factors, mts = src.mipmap_info(v)
         lvl = bf.best_mipmap_level(regs[v], factors, mts)
-        lvl_dims = src.dataset_attributes(bn5.bdv_dataset(v[1], v[0], lvl))["dimensions"]
         m = _compose(regs[v], mts[lvl])
-        info[v] = dict(level=lvl, dims=tuple(int(d) for d in lvl_dims), model=m, blending=bf.adjust_blending(m),
-                       dtype=src.dataset_attributes(bn5.bdv_dataset(v[1], v[0], lvl))["dataType"])
+        info[v] = dict(level=lvl, dims=src.level_dims(v, lvl), model=m, blending=bf.adjust_blending(m),
+                       dtype=src.level_dtype(v, lvl))
     vdims = {v: info[v]["dims"] for v in view_ids}
     vregs = {v: info[v]["model"] for v in view_ids}
     windowed_ok = (ft in (native.FUSE_AVG, native.FUSE_AVG_BLEND) and interpolation == 1 and
@@ -306,8 +291,7 @@ def _fuse_volume_blockwise(ctx, data, src, sink, meta, levels, view_ids, fusion_
     content = ft in (native.FUSE_AVG_CONTENT, native.FUSE_AVG_BLEND_CONTENT)
 
     # pyramid straight from the resident fused block when every super-block maps onto whole voxels of every level
-    abs_last = [int(v) for v in levels[-1]["absoluteDownsampling"][:3]]
-    fast_pyramid = len(levels) > 1 and all(compute[d] % abs_last[d] == 0 for d in range(3)) and not masks
+    fast_pyramid = len(levels) > 1 and _maps_onto_level(compute, levels[-1]) and not masks
 
     grid = bf.grid_create(dims, compute, bs)
     slabs = {}
@@ -354,18 +338,17 @@ def _fuse_volume_blockwise(ctx, data, src, sink, meta, levels, view_ids, fusion_
             try:
                 for v in vids:
                     border, rng = info[v]["blending"]
-                    ds_name = bn5.bdv_dataset(v[1], v[0], info[v]["level"])
                     if windowed_ok:
                         w = _source_window(info[v]["model"], info[v]["dims"], lo - bf.AFFINE_EXPANSION, hi + bf.AFFINE_EXPANSION)
                         if w is None:
                             continue
                         wmin, wsize = w
-                        staged[v] = ctx.volume_upload(src.read_region(ds_name, wmin, wsize))
+                        staged[v] = ctx.volume_upload(src.read_region(v, info[v]["level"], wmin, wsize))
                         views[v] = dict(src_to_world=info[v]["model"], vol_handle=staged[v], blend_border=border, blend_range=rng,
                                         full_dims=info[v]["dims"], window_min=tuple(int(x) for x in wmin))
                     else:
                         if v not in whole:
-                            h = ctx.volume_upload(src.read_volume(ds_name))
+                            h = ctx.volume_upload(src.read_volume(v, info[v]["level"]))
                             whole[v] = (h, ctx.content_weights(h) if content else 0)
                         views[v] = dict(src_to_world=info[v]["model"], vol_handle=whole[v][0], content_handle=whole[v][1],
                                         blend_border=border, blend_range=rng)
@@ -415,36 +398,9 @@ def _fuse_volume_blockwise(ctx, data, src, sink, meta, levels, view_ids, fusion_
             if ch:
                 ctx.volume_free(ch)
 
-    # ---- pyramid s1 .. sN when super-blocks do not map onto whole voxels of every level: every block of level l is
-    # the 2x average of its region of level l-1 (N5ApiTools.writeDownsampledBlock[5dOMEZARR]), read back from the
-    # container and averaged on the device (bs_downsample)
-    for li in range(1, 1 if fast_pyramid else len(levels)):
-        if barrier is not None:
-            barrier()                                # level l-1 is complete on every rank
-        prev, cur = levels[li - 1], levels[li]
-        rel = [int(v) for v in cur["relativeDownsampling"][:3]]
-        cdims = [int(v) for v in cur["dimensions"][:3]]
-        todo, attempt = bf.grid_create(cdims, compute, bs)[rank::world], 0
-        while todo:
-            attempt += 1
-            if attempt > retries:
-                raise RuntimeError(f"pyramid s{li}: {len(todo)} block(s) still failing after {retries} attempts")
-            failed = []
-            for gb in todo:
-                off, size, gpos = gb
-                h = h2 = None
-                try:
-                    srcblk = sink.read_region(prev["dataset"], [off[d] * rel[d] for d in range(3)], [size[d] * rel[d] for d in range(3)])
-                    h = ctx.volume_upload(np.ascontiguousarray(srcblk))
-                    h2 = ctx.downsample(h, rel)
-                    sink.save(cur["dataset"], ctx.volume_download(h2, size, np_dt), gpos)
-                except native.BsError:
-                    failed.append(gb)
-                finally:
-                    for hh in (h, h2):
-                        if hh is not None:
-                            ctx.volume_free(hh)
-            todo = failed
+    # ---- pyramid s1 .. sN when super-blocks do not map onto whole voxels of every level
+    _pyramid_from_stored(ctx, [(sink, levels, np_dt)], len(levels) if fast_pyramid else 1, compute, bs, shard, retries,
+                         barrier)
 
 
 def _fuse_block_with_pyramid(ctx, gb, bb_min, vdims, vregs, views, params, np_dt, sink, levels, bs):
@@ -452,21 +408,83 @@ def _fuse_block_with_pyramid(ctx, gb, bb_min, vdims, vregs, views, params, np_dt
     wmin = bb_min + np.asarray(off, dtype=np.int64)
     vids = bf.find_overlapping_views(vdims, vregs, wmin, wmin + np.asarray(size) - 1, sorted(views))
     cur_h = ctx.fuse_block_to_volume([views[v] for v in vids], tuple(int(v) for v in wmin), tuple(int(v) for v in size), params)
+    _write_resident_levels(ctx, cur_h, gb, sink, levels, bs, np_dt)
+
+
+# --------------------------------------------------------------------------------------------- pyramid (shared)
+# The multi-resolution pyramid of a container volume, shared by affine-fusion and resave.  A level is the 2x half-pixel
+# average of the level above (N5ApiTools.writeDownsampledBlock[5dOMEZARR], LazyHalfPixelDownsample2x), taken on the
+# device by bs_downsample.  While a compute block is resident, every level it maps onto whole voxels of is derived from
+# it before anything is downloaded; the other levels are built from the stored level l-1 once it is complete.
+def _maps_onto_level(compute, level):
+    """True when compute blocks (at multiples of ``compute``) cover whole voxels of ``level`` (so the chained
+    downsampling of a block equals that of the volume)."""
+    a = [int(v) for v in level["absoluteDownsampling"][:3]]
+    return all(int(compute[d]) % a[d] == 0 for d in range(3))
+
+
+def _write_resident_levels(ctx, cur_h, gb, sink, levels, bs, np_dt):
+    """Write the resident compute block ``cur_h`` (grid block ``gb`` of level 0) to every level of ``levels``, deriving
+    each from the previous one on the device; frees ``cur_h``.  Each level is downloaded and split into storage blocks
+    on the host, read-modify-writing those it covers only partly."""
+    off, size, gpos = gb
     try:
         cur_size, cur_off = [int(v) for v in size], [int(v) for v in off]
-        sink.save(levels[0]["dataset"], ctx.volume_download(cur_h, cur_size, np_dt), gpos)
-        for lv in levels[1:]:
-            rel = [int(v) for v in lv["relativeDownsampling"][:3]]
-            nxt = [cur_size[d] // rel[d] for d in range(3)]
-            if min(nxt) < 1:
-                break        # an edge block thinner than the step: no voxel of this (or any deeper) level
-            nh = ctx.downsample(cur_h, rel)
-            ctx.volume_free(cur_h)
-            cur_h, cur_size, cur_off = nh, nxt, [cur_off[d] // rel[d] for d in range(3)]
-            sink.write_region(lv["dataset"], ctx.volume_download(cur_h, cur_size, np_dt), cur_off,
-                              [int(v) for v in lv["dimensions"][:3]], bs)
+        for li, lv in enumerate(levels):
+            if li > 0:
+                rel = [int(v) for v in lv["relativeDownsampling"][:3]]
+                nxt = [cur_size[d] // rel[d] for d in range(3)]
+                if min(nxt) < 1:
+                    break        # an edge block thinner than the step: no voxel of this (or any deeper) level
+                nh = ctx.downsample(cur_h, rel)
+                ctx.volume_free(cur_h)
+                cur_h, cur_size, cur_off = nh, nxt, [cur_off[d] // rel[d] for d in range(3)]
+            if li == 0:
+                sink.save(lv["dataset"], ctx.volume_download(cur_h, cur_size, np_dt), gpos)
+            else:
+                sink.write_region(lv["dataset"], ctx.volume_download(cur_h, cur_size, np_dt), cur_off,
+                                  [int(v) for v in lv["dimensions"][:3]], bs)
     finally:
         ctx.volume_free(cur_h)
+
+
+def _pyramid_from_stored(ctx, volumes, first, compute, bs, shard=(0, 1), retries=5, barrier=None):
+    """Levels ``first`` .. N of every volume in ``volumes`` ([(sink, levels, numpy dtype)]): every compute block of level
+    l is the 2x average of its region of level l-1, read back from the container and averaged on the device.  Rank r of
+    w takes blocks [r::w] of each level; ``barrier()`` runs before each level so that level l-1 is complete on every
+    rank.  Failed blocks are retried up to ``retries`` times (RetryTrackerSpark)."""
+    rank, world = shard
+    for li in range(first, max(len(lv) for _, lv, _ in volumes)):
+        if barrier is not None:
+            barrier()                                # level l-1 is complete on every rank
+        work = []
+        for sink, levels, np_dt in volumes:
+            if li < len(levels):
+                cdims = [int(v) for v in levels[li]["dimensions"][:3]]
+                work += [(sink, levels, np_dt, gb) for gb in bf.grid_create(cdims, compute, bs)]
+        todo, attempt = work[rank::world], 0
+        while todo:
+            attempt += 1
+            if attempt > retries:
+                raise RuntimeError(f"pyramid s{li}: {len(todo)} block(s) still failing after {retries} attempts")
+            failed = []
+            for item in todo:
+                sink, levels, np_dt, (off, size, gpos) = item
+                prev, cur = levels[li - 1], levels[li]
+                rel = [int(v) for v in cur["relativeDownsampling"][:3]]
+                h = h2 = None
+                try:
+                    srcblk = sink.read_region(prev["dataset"], [off[d] * rel[d] for d in range(3)], [size[d] * rel[d] for d in range(3)])
+                    h = ctx.volume_upload(np.ascontiguousarray(srcblk))
+                    h2 = ctx.downsample(h, rel)
+                    sink.save(cur["dataset"], ctx.volume_download(h2, size, np_dt), gpos)
+                except native.BsError:
+                    failed.append(item)
+                finally:
+                    for hh in (h, h2):
+                        if hh is not None:
+                            ctx.volume_free(hh)
+            todo = failed
 
 
 def _storage_cells(gb, bs):
@@ -589,17 +607,15 @@ def _check_device_memory(ctx, nbytes, what):
 
 def _detect_view(ctx, src, view, level, remaining, mt, sigma, threshold, min_intensity, max_intensity, find_max,
                  find_min, localization, block_size, median_filter, need_intensities):
-    ds_name = bn5.bdv_dataset(view[1], view[0], level)
-    a = src.dataset_attributes(ds_name)
-    ldims = [int(v) for v in a["dimensions"]]
+    ldims = list(src.level_dims(view, level))
     vox = int(np.prod(ldims))
     dvox = int(np.prod([max(ldims[d] // remaining[d], 0) for d in range(3)]))
     blk = int(np.prod([min(int(block_size[d]), ldims[d]) + 64 for d in range(3)]))
-    _check_device_memory(ctx, vox * np.dtype(bn5._DTYPES[a["dataType"]]).itemsize + 4 * (2 * dvox + 4 * blk),
+    _check_device_memory(ctx, vox * np.dtype(src.level_dtype(view, level)).itemsize + 4 * (2 * dvox + 4 * blk),
                          f"view {view} (level s{level}, {ldims[0]}x{ldims[1]}x{ldims[2]})")
     handles = []
     try:
-        h = ctx.volume_upload(src.read_volume(ds_name))
+        h = ctx.volume_upload(src.read_volume(view, level))
         handles.append(h)
         img = h
         if any(v > 1 for v in remaining):
@@ -659,15 +675,12 @@ def detect_interestpoints(xml_path, ctx: Context, label, sigma, threshold, min_i
     if median_filter is not None and not 0 < int(median_filter) <= native.MEDIAN_MAX_RADIUS:
         raise ValueError(f"--medianFilter {median_filter} outside [1, {native.MEDIAN_MAX_RADIUS}]")
     data = SpimData2.load(xml_path)
-    fmt, n5_path = data.image_loader()
-    if fmt != "bdv.n5":
-        raise NotImplementedError(f"ImageLoader format {fmt}")
-    src = bn5.N5Store(n5_path)
+    src = bvs.open_views(data)
     views = data.select_views(**view_selection) if view_selection else data.view_ids()
     rank, world = shard
     results = {}
     for v in views[rank::world]:
-        factors, mts = _mipmap_info(src, v[1])
+        factors, mts = src.mipmap_info(v)
         level, remaining = interestpoint_level(factors, (downsample_xy, downsample_xy, downsample_z))
         loc, inten = _detect_view(ctx, src, v, level, remaining, mts[level], sigma, threshold, min_intensity, max_intensity,
                                   find_max, find_min, localization.upper() == "QUADRATIC", block_size, median_filter,
@@ -800,10 +813,7 @@ def nonrigid_fusion(xml_path, ctx: Context, out_path, n5_dataset, interest_point
         raise ValueError("no interest points defined, exiting.")
     labels = list(interest_points)
     data = SpimData2.load(xml_path)
-    fmt, n5_in = data.image_loader()
-    if fmt != "bdv.n5":
-        raise NotImplementedError(f"ImageLoader format {fmt}")
-    src = bn5.N5Store(n5_in)
+    src = bvs.open_views(data)
     views = sorted(data.select_views(**view_selection) if view_selection else data.view_ids())
     regs = {v: data.model(*v) for v in views}
     vdims = {v: tuple(int(d) for d in data.setups[v[1]].size) for v in views}
@@ -889,7 +899,7 @@ def _nonrigid_chunk(ctx, src, chunk, bb_min, fuse, nviews, vdims, params, cpd):
             whi = np.minimum(np.ceil(ghi).astype(np.int64) + 2, dims - 1)
             if np.any(whi < wlo):
                 continue                                  # the view's grids never reach its pixels in this chunk
-            h = ctx.volume_upload(src.read_region(bn5.bdv_dataset(v[1], v[0], 0), wlo, whi - wlo + 1))
+            h = ctx.volume_upload(src.read_region(v, 0, wlo, whi - wlo + 1))
             staged.append(h)
             gviews.append(dict(nv, vol_handle=h, window_min=tuple(int(x) for x in wlo)))
         if not gviews:
@@ -1091,3 +1101,179 @@ def solver(xml_path, ctx: Context, source, labels=None, label_weights=None, meth
                        regularization_lambda, max_error, max_iterations, max_plateau_width, relative_threshold,
                        absolute_threshold, fixed_views, disable_fixed_views, group_tiles, group_illums, group_channels,
                        split_timepoints, registration_tp, view_selection, dry_run)
+
+
+# --------------------------------------------------------------------------------------------- resave
+RESAVE_COMPRESSION = {"zstd": "zstd", "zstandard": "zstd", "gzip": "gzip", "raw": "raw"}
+
+
+def propose_mipmaps(size_xyz, voxel_size_xyz=(1.0, 1.0, 1.0)):
+    """Resave_HDF5.proposeMipmaps / bdv ProposeMipmaps restated (recalled, PARITY_GAPS R5): starting at (1, 1, 1), while
+    the largest axis of the current level is over 256 pixels, double the factor of every axis whose voxel size is at
+    most twice the smallest one (and that is still over 1 pixel), so anisotropic z catches up.  Absolute factors."""
+    vs = [float(v) for v in voxel_size_xyz]
+    vs = [v / min(vs) for v in vs]
+    size = [int(v) for v in size_xyz]
+    res, out = [1, 1, 1], []
+    while True:
+        out.append(tuple(res))
+        if max(size) <= 256:
+            return out
+        grow = [d for d in range(3) if vs[d] <= 2.0 * min(vs) and size[d] > 1]
+        for d in grow:
+            res[d] *= 2
+            vs[d] *= 2.0
+            size[d] //= 2
+
+
+def parse_downsampling(downsampling):
+    """`-ds "1,1,1; 2,2,1; 4,4,1"` (or a list of triples): absolute factors per level.  The first must be 1,1,1
+    (J/SparkResaveN5.java:211); each level must be 1x or 2x the previous one per axis, the steps bs_downsample takes
+    (PARITY_GAPS R4).  Anything else raises ValueError."""
+    if isinstance(downsampling, str):
+        steps = [tuple(int(v) for v in s.split(",")) for s in downsampling.split(";") if s.strip()]
+    else:
+        steps = [tuple(int(v) for v in s) for s in downsampling]
+    if not steps or any(len(s) != 3 for s in steps):
+        raise ValueError(f"-ds {downsampling}: need x,y,z triples")
+    if steps[0] != (1, 1, 1):
+        raise ValueError("First downsampling step must be full resolution [1,1,...1], stopping.")
+    for a, b in zip(steps, steps[1:]):
+        if any(b[d] not in (a[d], 2 * a[d]) for d in range(3)):
+            raise ValueError(f"-ds {downsampling}: step {b} after {a} is not 1x or 2x per axis")
+    return steps
+
+
+def _voxel_size(data, setup):
+    for vs in data.root.find("SequenceDescription").find("ViewSetups").findall("ViewSetup"):
+        if int(vs.findtext("id")) == int(setup):
+            txt = vs.findtext("voxelSize/size")
+            return tuple(float(v) for v in txt.split()) if txt else (1.0, 1.0, 1.0)
+    return (1.0, 1.0, 1.0)
+
+
+def resave(xml_path, ctx: Context, xml_out=None, n5=False, out_path=None, block_size=(128, 128, 64),
+           block_scale=(16, 16, 1), downsampling=None, compression="zstd", compression_level=None, dry_run=False,
+           shard=(0, 1), barrier=None, retries=5):
+    """`./resave -x dataset.xml [-xo out.xml] [--N5] [-o dataset.ome.zarr] [--blockSize 128,128,64]
+    [--blockScale 16,16,1] [-ds "1,1,1; 2,2,1; 4,4,1"] [-c Zstandard] [-cl 3] [--dryRun]` (J/SparkResaveN5.java:80-455):
+    copy every view of the XML, through whichever loader it has, into a new OME-ZARR container (default
+    `dataset.ome.zarr` next to ``xml_out``) or, with ``n5``, a BDV-N5 one (`dataset.n5`), with a multi-resolution
+    pyramid, and point the XML's ImageLoader at it (``xml_out``, default the input XML, saved with a ~1 backup).
+
+    Work is cut into compute blocks of ``block_size * block_scale`` on storage-block boundaries (Grid.create).  Each
+    block's s0 is read once and uploaded; the leading pyramid levels it lies on whole storage blocks of (block_scale a
+    multiple of the level's factors) are derived on the device (bs_downsample) while it is resident, so no rank ever
+    writes part of a storage block.  The other levels are built from the stored level l-1 after ``barrier()``; with the
+    default block_scale (16, 16, 1) that is every level of a pyramid that halves z.  ``downsampling``: absolute factors
+    (parse_downsampling); default propose_mipmaps of the first view's setup.
+
+    The output container must not be, contain or lie inside the input one (ValueError): re-saving a dataset next to its
+    own XML in the format it already has would overwrite the data being read.
+
+    Multi-GPU: rank 0 creates every dataset and writes all metadata, then ``barrier()`` (required when w > 1) lets the
+    other ranks in; rank r of w takes compute blocks [r::w]; rank 0 writes the XML after a last ``barrier()``.
+    ``dry_run`` stops after planning and writes nothing.  Returns dict(out_path, xml_out, downsamplings,
+    compute_blocks)."""
+    comp = RESAVE_COMPRESSION.get(str(compression).lower())
+    if comp is None:
+        raise NotImplementedError(f"compression {compression} (writable: Zstandard, Gzip, Raw)")
+    rank, world = shard
+    if world > 1 and barrier is None:
+        raise ValueError("resave with more than one rank needs barrier(): rank 0 creates the datasets first")
+    data = SpimData2.load(xml_path)
+    src = bvs.open_views(data)
+    views = data.view_ids()
+    if not views:
+        raise ValueError("No views to resave.")
+    xml_out = xml_out or xml_path
+    if out_path is None:
+        out_path = os.path.join(os.path.dirname(os.path.abspath(xml_out)), "dataset.n5" if n5 else "dataset.ome.zarr")
+    a, b = os.path.realpath(out_path), os.path.realpath(src.store.root)
+    if a == b or a.startswith(b + os.sep) or b.startswith(a + os.sep):
+        raise ValueError(f"resave output {out_path} overlaps the input container {src.store.root}; choose another -o / -xo")
+    bs = [int(v) for v in block_size]
+    compute = [bs[d] * int(block_scale[d]) for d in range(3)]
+    if downsampling is None:     # N5ApiTools.mipMapInfoToDownsamplings(proposeMipmaps(...)): one pyramid for all views
+        first = views[0]
+        downsampling = propose_mipmaps(src.level_dims(first, 0), _voxel_size(data, first[1]))
+    steps = parse_downsampling(downsampling)
+    # every view is checked before anything is created
+    meta = {}
+    for v in views:
+        dims0, dt = src.level_dims(v, 0), src.level_dtype(v, 0)
+        if dt not in ("uint8", "uint16", "float32"):
+            raise NotImplementedError(f"resave of {dt} view {v} (bs_downsample takes uint8, uint16, float32)")
+        if any(int(dims0[d]) // steps[-1][d] < 1 for d in range(3)):
+            raise ValueError(f"view {v} of {tuple(dims0)} voxels is too small for the downsampling {steps[-1]}")
+        meta[v] = (dims0, dt)
+    grid = [(v, gb) for v in views for gb in bf.grid_create(list(meta[v][0]), compute, bs)]
+    plan = dict(out_path=out_path, xml_out=xml_out, downsamplings=steps, compute_blocks=len(grid))
+    if dry_run:
+        return plan
+
+    # ---- datasets and metadata of every view, created once by rank 0 (setupBdvDatasetsN5 / setupBdvDatasetsOMEZARR,
+    # on the driver before any worker runs, J/SparkResaveN5.java:222-262)
+    if rank == 0:
+        store = bn5.N5Store(out_path, create=True) if n5 else bzarr.ZarrStore(out_path, create=True)
+        for v in views:
+            dims0, dt = meta[v]
+            if n5:
+                store.set_attributes(f"setup{v[1]}", {"downsamplingFactors": [list(s) for s in steps], "dataType": dt})
+                store.set_attributes(f"setup{v[1]}/timepoint{v[0]}", {"resolution": [1.0, 1.0, 1.0], "multiScale": True})
+                for li, f in enumerate(steps):
+                    store.create_dataset(bn5.bdv_dataset(v[1], v[0], li), [int(dims0[d]) // f[d] for d in range(3)], bs,
+                                         np.dtype(dt), comp, compression_level)
+            else:
+                bzarr.create_multiscale_group(store, _resave_group(v), dims0, dt, bs, steps, comp, compression_level)
+    if world > 1:
+        barrier()                                    # the container exists on every rank
+    store = bn5.N5Store(out_path) if n5 else bzarr.ZarrStore(out_path)
+    vols = {}
+    for v in views:
+        dims0, dt = meta[v]
+        levels = [dict(dataset=bn5.bdv_dataset(v[1], v[0], li) if n5 else f"{_resave_group(v)}/{li}",
+                       dimensions=[int(dims0[d]) // f[d] for d in range(3)], absoluteDownsampling=list(f),
+                       relativeDownsampling=[f[d] // (steps[li - 1][d] if li else 1) for d in range(3)])
+                  for li, f in enumerate(steps)]
+        vols[v] = (_Sink(store, not n5, 0, 0), levels, np.dtype(dt))
+
+    # levels kept resident: the leading ones every compute block lies on whole storage blocks of
+    n_res = 1
+    while n_res < len(steps) and all(compute[d] % (steps[n_res][d] * bs[d]) == 0 for d in range(3)):
+        n_res += 1
+
+    # ---- s0 (+ resident levels), compute blocks [r::w], RetryTrackerSpark policy
+    todo, attempt = grid[rank::world], 0
+    while todo:
+        attempt += 1
+        if attempt > retries:
+            raise RuntimeError(f"resave: {len(todo)} block(s) still failing after {retries} attempts")
+        failed = []
+        for v, gb in todo:
+            sink, levels, dt = vols[v]
+            off, size, _ = gb
+            try:
+                h = ctx.volume_upload(src.read_region(v, 0, off, size))
+            except native.BsError:
+                failed.append((v, gb))
+                continue
+            try:
+                _write_resident_levels(ctx, h, gb, sink, levels[:n_res], bs, dt)
+            except native.BsError:
+                failed.append((v, gb))
+        todo = failed
+    _pyramid_from_stored(ctx, [vols[v] for v in views], n_res, compute, bs, shard, retries, barrier)
+
+    if world > 1:
+        barrier()                                    # every rank has written its blocks
+    if rank == 0:
+        data.set_image_loader("bdv.n5" if n5 else "bdv.multimg.zarr", out_path, xml_out,
+                              {v: (_resave_group(v), 0, 0) for v in views} if not n5 else None)
+        data.save(xml_out)
+    return plan
+
+
+def _resave_group(view):
+    """The OME-ZARR group of a resaved view (PARITY_GAPS R3)."""
+    return f"s{view[1]}-t{view[0]}.zarr"

@@ -87,12 +87,14 @@ class N5Store:
             json.dump(cur, f)
 
     # -- datasets
-    def create_dataset(self, path, dimensions, block_size, dtype, compression="raw"):
+    def create_dataset(self, path, dimensions, block_size, dtype, compression="raw", level=None):
         comp = {"type": compression}
         if compression == "gzip":
             comp["level"] = 1  # reference default, J/util/N5Util.java:82-105
         elif compression == "zstd":
             comp["level"] = 3  # reference default (J/CreateFusionContainer.java:71-76, J/util/N5Util.java:91-92)
+        if compression != "raw" and level is not None:
+            comp["level"] = int(level)
         self.set_attributes(path, {"dimensions": [int(d) for d in dimensions],
                                    "blockSize": [int(b) for b in block_size],
                                    "dataType": _dtype_name(dtype), "compression": comp})
@@ -119,7 +121,7 @@ class N5Store:
         if ctype == "gzip":
             payload = gzip.compress(payload, compresslevel=a["compression"].get("level", 1))
         elif ctype == "zstd":
-            payload = bzstd.compress(payload)
+            payload = bzstd.compress(payload, a["compression"].get("level", bzstd.DEFAULT_LEVEL))
         elif ctype != "raw":
             raise NotImplementedError(f"compression {ctype} (not available in this image)")
         p = self._block_path(path, grid_pos)

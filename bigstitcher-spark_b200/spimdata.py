@@ -5,7 +5,8 @@ extensions) -- the fields the two hot paths consume and produce:
     grouping at J/SparkPairwiseStitching.java:147-160)
   * ViewRegistrations: ordered <ViewTransform type="affine"> lists; list index 0 is applied LAST
     (J/ClearRegistrations.java:80-99), so model = T0 * T1 * ... * Tn
-  * ImageLoader format="bdv.n5" path (J/SparkResaveN5.java:424-433)
+  * ImageLoader format="bdv.n5" path (J/SparkResaveN5.java:424-433), or format="bdv.multimg.zarr" (AllenOMEZarrLoader,
+    :434-445): the container root plus one <zgroup> per view with its group path and (channel, timepoint) indices
   * <StitchingResults><PairwiseResult view_setup_a/b tp_a/b> shift (12 doubles), correlation, hash,
     overlap_boundingbox (6 doubles)                                   (J/SparkPairwiseStitching.java:284-301,328-390)
   * <ViewInterestPoints><ViewInterestPointsFile timepoint setup label params>path of the label's group in
@@ -81,6 +82,40 @@ class SpimData2:
             base = self.root.findtext("BasePath") or "."
             p = os.path.normpath(os.path.join(os.path.dirname(os.path.abspath(self.path)), base, p))
         return fmt, p
+
+    def zarr_groups(self):
+        """The views of a `bdv.multimg.zarr` loader: {(tp, setup): (group path, channel index, timepoint index)}.
+        Element and attribute names are recalled from XmlIoAllenOMEZarrLoader (PARITY_GAPS R1)."""
+        il = self.root.find("SequenceDescription").find("ImageLoader")
+        out = {}
+        zg = il.find("zgroups")
+        for g in (zg.findall("zgroup") if zg is not None else []):
+            c, t = (int(v) for v in g.get("indicies", "[0, 0]").strip("[] ").split(","))
+            out[(int(g.get("tp")), int(g.get("setup")))] = (g.get("path"), c, t)
+        return out
+
+    def _loader_path(self, container, xml_path):
+        base = os.path.join(os.path.dirname(os.path.abspath(xml_path or self.path)), self.root.findtext("BasePath") or ".")
+        return os.path.relpath(os.path.abspath(container), os.path.normpath(base))
+
+    def set_image_loader(self, fmt, container, xml_path=None, zgroups=None):
+        """Replace the ImageLoader: ``fmt`` "bdv.n5" (<n5>) or "bdv.multimg.zarr" (<zarr> and <zgroups>, ``zgroups`` =
+        {(tp, setup): (group path, channel index, timepoint index)}).  The container path is written relative to the
+        BasePath of the XML at ``xml_path`` (default: where it was loaded from)."""
+        seq = self.root.find("SequenceDescription")
+        old = seq.find("ImageLoader")
+        il = ET.Element("ImageLoader", format=fmt, version="1.0")
+        tag = "n5" if fmt == "bdv.n5" else "zarr"
+        ET.SubElement(il, tag, type="relative").text = self._loader_path(container, xml_path)
+        if fmt == "bdv.multimg.zarr":
+            zg = ET.SubElement(il, "zgroups")
+            for (tp, setup), (gpath, c, t) in sorted(zgroups.items()):
+                ET.SubElement(zg, "zgroup", setup=str(setup), tp=str(tp), path=gpath, indicies=f"[{int(c)}, {int(t)}]")
+        elif fmt != "bdv.n5":
+            raise ValueError(f"ImageLoader format {fmt}")
+        seq.insert(list(seq).index(old) if old is not None else 0, il)
+        if old is not None:
+            seq.remove(old)
 
     def save(self, path: str | None = None, backup: bool = True):
         path = path or self.path

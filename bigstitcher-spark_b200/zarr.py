@@ -4,13 +4,20 @@ axis order x,y,z,c,t == Zarr array order t,c,z,y,x, chunks {1,1,bz,by,bx}, level
 (:346), `multiscales` v0.4 metadata (:374-388), grid offsets {gx,gy,gz,c,t} at write time
 (J/SparkAffineFusion.java:630-643).  Little-endian C-order chunks, always full chunk shape (edge
 chunks padded with fill_value 0), dimension_separator "/"; compressor null (raw), gzip or zstd (the reference default,
-through zstd.py).  Host-side plumbing only.
+through zstd.py).
+
+The reader also takes 5-D arrays written by other tools (the `bdv.multimg.zarr` input of every command): dtypes in
+any byte order ('<', '>', '|'), both dimension separators ('/' and '.', the Zarr v2 default), compressors null, zstd,
+gzip and zlib, and a missing chunk reads as the array's fill_value.  Any other codec (blosc, ...) raises
+NotImplementedError naming it.  ``read_multiscales`` turns an OME-NGFF 0.4 `multiscales` group into integer mipmap
+factors.  Host-side plumbing only.
 """
 from __future__ import annotations
 
 import gzip
 import json
 import os
+import zlib
 
 import numpy as np
 
@@ -18,7 +25,27 @@ from . import zstd as bzstd
 from .n5 import bs_attrs, parse_fusion_metadata, BS_KEY
 
 _ZDT = {"uint8": "|u1", "uint16": "<u2", "float32": "<f4"}
-_NPDT = {"|u1": np.uint8, "<u2": np.uint16, "<f4": np.float32}
+
+
+def _np_dtype(meta):
+    """Native-order numpy dtype of an array's elements (the stored byte order is handled by the chunk codec)."""
+    return np.dtype(meta["dtype"]).newbyteorder("=")
+
+
+def _decode(meta, payload: bytes) -> bytes:
+    comp = meta.get("compressor")
+    if meta.get("filters"):
+        raise NotImplementedError(f"Zarr filters {[f.get('id') for f in meta['filters']]}")
+    if comp is None:
+        return payload
+    cid = comp.get("id")
+    if cid == "zstd":
+        return bzstd.decompress(payload)
+    if cid == "gzip":
+        return gzip.decompress(payload)
+    if cid == "zlib":
+        return zlib.decompress(payload)
+    raise NotImplementedError(f"Zarr compressor {cid!r} (readable: null, zstd, gzip, zlib)")
 
 
 class ZarrStore:
@@ -55,11 +82,13 @@ class ZarrStore:
                 cur[k] = v
         self._write_json(group, ".zattrs", cur)
 
-    def create_array(self, path, shape_tczyx, chunks_tczyx, dtype: str, compression="raw"):
+    def create_array(self, path, shape_tczyx, chunks_tczyx, dtype: str, compression="raw", level=None):
         if compression not in ("raw", "gzip", "zstd"):
             raise NotImplementedError(f"compression {compression} (not available in this image)")
         # numcodecs ids; zstd level 3 = the reference default (J/util/N5Util.java:91-92)
         comp = {"raw": None, "gzip": {"id": "gzip", "level": 1}, "zstd": {"id": "zstd", "level": 3}}[compression]
+        if comp is not None and level is not None:
+            comp["level"] = int(level)
         self._write_json(path, ".zarray", {"zarr_format": 2, "shape": [int(v) for v in shape_tczyx],
                                            "chunks": [int(v) for v in chunks_tczyx], "dtype": _ZDT[dtype],
                                            "compressor": comp, "fill_value": 0, "order": "C", "filters": None,
@@ -71,40 +100,46 @@ class ZarrStore:
             raise KeyError(f"{path} is not a Zarr array")
         return m
 
-    def _chunk_path(self, path, idx_tczyx):
-        return os.path.join(self.root, path.strip("/"), *[str(int(i)) for i in idx_tczyx])
+    def _chunk_path(self, path, idx_tczyx, meta=None):
+        sep = (meta or self.array_meta(path)).get("dimension_separator") or "."
+        key = sep.join(str(int(i)) for i in idx_tczyx)
+        return os.path.join(self.root, path.strip("/"), *key.split("/"))
 
     def write_chunk(self, path, idx_tczyx, block_zyx: np.ndarray):
-        """block_zyx: the valid [z,y,x] part of one chunk; padded to the full chunk shape."""
+        """block_zyx: the valid [z,y,x] part of one chunk; padded to the full chunk shape.  A full chunk already in
+        the array's byte order is written as it is."""
         m = self.array_meta(path)
         cz, cy, cx = m["chunks"][2:]
-        dt = np.dtype(_NPDT[m["dtype"]])
-        full = np.zeros((cz, cy, cx), dtype=dt)
-        z, y, x = block_zyx.shape
-        full[:z, :y, :x] = block_zyx
-        payload = full.astype(dt.newbyteorder("<"), copy=False).tobytes()
+        sdt = np.dtype(m["dtype"])
+        if block_zyx.shape == (cz, cy, cx) and block_zyx.dtype == sdt and block_zyx.flags["C_CONTIGUOUS"]:
+            payload = block_zyx.tobytes()
+        else:
+            full = np.zeros((cz, cy, cx), dtype=sdt)
+            z, y, x = block_zyx.shape
+            full[:z, :y, :x] = block_zyx
+            payload = full.tobytes()
         if m["compressor"] is not None:
             if m["compressor"]["id"] == "zstd":
                 payload = bzstd.compress(payload, m["compressor"].get("level", 3))
             else:
                 payload = gzip.compress(payload, compresslevel=m["compressor"].get("level", 1))
-        p = self._chunk_path(path, idx_tczyx)
+        p = self._chunk_path(path, idx_tczyx, m)
         os.makedirs(os.path.dirname(p), exist_ok=True)
         with open(p, "wb") as f:
             f.write(payload)
 
     def read_chunk(self, path, idx_tczyx):
         m = self.array_meta(path)
-        p = self._chunk_path(path, idx_tczyx)
+        if m.get("order", "C") != "C":
+            raise NotImplementedError(f"Zarr order {m['order']!r} of {path}")
+        p = self._chunk_path(path, idx_tczyx, m)
         cz, cy, cx = m["chunks"][2:]
-        dt = np.dtype(_NPDT[m["dtype"]])
+        dt = _np_dtype(m)
         if not os.path.exists(p):
-            return np.zeros((cz, cy, cx), dtype=dt)
+            return np.full((cz, cy, cx), m.get("fill_value") or 0, dtype=dt)
         with open(p, "rb") as f:
-            payload = f.read()
-        if m["compressor"] is not None:
-            payload = bzstd.decompress(payload) if m["compressor"]["id"] == "zstd" else gzip.decompress(payload)
-        return np.frombuffer(payload, dtype=dt.newbyteorder("<")).astype(dt).reshape(cz, cy, cx)
+            payload = _decode(m, f.read())
+        return np.frombuffer(payload, dtype=np.dtype(m["dtype"]), count=cz * cy * cx).astype(dt).reshape(cz, cy, cx)
 
     def save_block(self, path, volume_zyx: np.ndarray, grid_offset_xyzct):
         """N5Utils.saveBlock on the 5-D view (J/SparkAffineFusion.java:630-643,670): split a
@@ -131,7 +166,7 @@ class ZarrStore:
         cz, cy, cx = m["chunks"][2:]
         mn = [int(v) for v in min_xyz]
         n = [int(v) for v in size_xyz]
-        out = np.zeros(n[::-1], dtype=_NPDT[m["dtype"]])
+        out = np.zeros(n[::-1], dtype=_np_dtype(m))
         lo = [max(0, mn[d]) for d in range(3)]
         hi = [min((sx, sy, sz)[d], mn[d] + n[d]) for d in range(3)]
         if any(hi[d] <= lo[d] for d in range(3)):
@@ -151,7 +186,7 @@ class ZarrStore:
         m = self.array_meta(path)
         sz, sy, sx = m["shape"][2:]
         cz, cy, cx = m["chunks"][2:]
-        out = np.zeros((sz, sy, sx), dtype=_NPDT[m["dtype"]])
+        out = np.zeros((sz, sy, sx), dtype=_np_dtype(m))
         for iz in range(-(-sz // cz)):
             for iy in range(-(-sy // cy)):
                 for ix in range(-(-sx // cx)):
@@ -166,6 +201,61 @@ def mipmap_transform_default(abs_ds):
     (example at J/SparkInterestPointDetection.java:1073-1080)."""
     f = [float(v) for v in abs_ds]
     return [[f[0], 0, 0, (f[0] - 1) / 2], [0, f[1], 0, (f[1] - 1) / 2], [0, 0, f[2], (f[2] - 1) / 2]]
+
+
+def read_multiscales(store: ZarrStore, group=""):
+    """The levels of an OME-NGFF 0.4 multiscale group: [dict(path, factors (x, y, z) ints, dims (x, y, z))], level 0
+    first.  A level's mipmap factors are its `scale` transformation divided by that of level 0, per spatial axis; they
+    must be integers and the level's array must be floor or ceil of level 0's dims over them (ValueError otherwise)."""
+    ms = store.get_attributes(group).get("multiscales")
+    if not ms:
+        raise KeyError(f"{os.path.join(store.root, group)} has no OME-NGFF multiscales attribute")
+    ms = ms[0]
+    names = [a["name"] if isinstance(a, dict) else str(a) for a in ms.get("axes", [])]
+    ax = [names.index(n) for n in "xyz"] if all(n in names for n in "xyz") else [-1, -2, -3]
+    levels = []
+    for d in ms["datasets"]:
+        scale = next((t["scale"] for t in d.get("coordinateTransformations", []) if t.get("type") == "scale"), None)
+        path = (group.strip("/") + "/" + d["path"]).strip("/")
+        shape = store.array_meta(path)["shape"]
+        levels.append(dict(path=path, scale=[float(scale[a]) if scale else 1.0 for a in ax],
+                           dims=tuple(int(shape[a]) for a in ax)))
+    s0, d0 = levels[0]["scale"], levels[0]["dims"]
+    for lv in levels:
+        f = [lv["scale"][k] / s0[k] for k in range(3)]
+        fi = [int(round(v)) for v in f]
+        if any(abs(f[k] - fi[k]) > 1e-6 * max(1.0, f[k]) or fi[k] < 1 for k in range(3)):
+            raise ValueError(f"{lv['path']}: mipmap factors {f} relative to level 0 are not integers")
+        if any(lv["dims"][k] not in (d0[k] // fi[k], -(-d0[k] // fi[k])) for k in range(3)):
+            raise ValueError(f"{lv['path']}: dims {lv['dims']} do not match level 0 dims {d0} over factors {fi}")
+        lv["factors"] = tuple(fi)
+        del lv["scale"]
+    return levels
+
+
+def create_multiscale_group(store: ZarrStore, group, dims_xyz, dtype, block_size, abs_factors, compression="zstd",
+                            level=None):
+    """One resaved view (J/SparkResaveN5.java:246-256, setupBdvDatasetsOMEZARR; layout recalled, PARITY_GAPS R3):
+    the group holds one 5-D (1, 1, z, y, x) array per level, "0", "1", ..., chunks {1, 1, bz, by, bx}, dims
+    floor(dims / factor), and `multiscales` v0.4 with scale = the absolute factors (pixel units) and the half-pixel
+    translation (f - 1) / 2 of mipmap_transform_default."""
+    datasets = []
+    for lvl, f in enumerate(abs_factors):
+        dims = [int(dims_xyz[d]) // int(f[d]) for d in range(3)]
+        path = f"{group}/{lvl}"
+        store.create_array(path, (1, 1, dims[2], dims[1], dims[0]), (1, 1, block_size[2], block_size[1], block_size[0]),
+                           dtype, compression, level)
+        mt = mipmap_transform_default(f)
+        datasets.append({"path": str(lvl), "coordinateTransformations": [
+            {"type": "scale", "scale": [1.0, 1.0, float(f[2]), float(f[1]), float(f[0])]},
+            {"type": "translation", "translation": [0.0, 0.0, mt[2][3], mt[1][3], mt[0][3]]}]})
+    store.set_attributes(group, {"multiscales": [{
+        "version": "0.4", "name": group,
+        "axes": [{"name": "t", "type": "time", "unit": "second"}, {"name": "c", "type": "channel"},
+                 {"name": "z", "type": "space", "unit": "micrometer"}, {"name": "y", "type": "space", "unit": "micrometer"},
+                 {"name": "x", "type": "space", "unit": "micrometer"}],
+        "datasets": datasets}]})
+    store._write_json(group, ".zgroup", {"zarr_format": 2})
 
 
 def create_fusion_container_zarr(root, input_xml, bb_min, bb_max, block_size=(128, 128, 128), dtype="float32",
