@@ -62,13 +62,12 @@ __device__ __forceinline__ float load_voxel(const void* p, int dtype, size_t i) 
 // One warp owns a line at a time: the row's y/z profile is warp-uniform, interior samples are
 // read as aligned ushort2 pairs, and each lane keeps XR_UNROLL independent loads in flight.
 #define XR_UNROLL 5
-template <class F>
 __global__ void __launch_bounds__(PCM_THREADS) k_fft_x_r2c(const __grid_constant__ XR2CArgs a) {
-    const int M = F::kStatic ? F::N : a.M;
-    const int lshift = F::kStatic ? F::LSHIFT : a.lshift;
+    const int M = a.M;
+    const int lshift = a.lshift;
     const int LB = 1 << lshift, ls = LB + 1;
     const int Px = 2 * M;
-    const int pitch = F::kStatic ? ((F::N + 1 + 15) / 16) * 16 : a.pitch;
+    const int pitch = a.pitch;
     float2* tw = bs_sm;
     float2* b0 = bs_sm + Px;
     float2* b1 = b0 + M * ls;
@@ -148,7 +147,7 @@ __global__ void __launch_bounds__(PCM_THREADS) k_fft_x_r2c(const __grid_constant
         }
     }
     __syncthreads();
-    const float2* res = F::run(b0, b1, tw, a.plan, lshift, ls, 2);
+    const float2* res = fft_tile(b0, b1, tw, a.plan, lshift, ls, 2);
     // untangle the packed half-length transform into the real-input spectrum X[0..M]
     for (int l = wid; l < nlines; l += NW) {
         float2* srow = spec + rowbase + (size_t)l * pitch;
@@ -209,14 +208,13 @@ struct XR2CTmaArgs {
     int esize;
 };
 
-template <class F>
 __global__ void __launch_bounds__(PCM_THREADS) k_fft_x_r2c_tma(const __grid_constant__ XR2CTmaArgs t) {
     const XR2CArgs& a = t.x;
-    const int M = F::kStatic ? F::N : a.M;
-    const int lshift = F::kStatic ? F::LSHIFT : a.lshift;
+    const int M = a.M;
+    const int lshift = a.lshift;
     const int LB = 1 << lshift, ls = LB + 1;
     const int Px = 2 * M;
-    const int pitch = F::kStatic ? ((F::N + 1 + 15) / 16) * 16 : a.pitch;
+    const int pitch = a.pitch;
     float2* tw = bs_sm;
     float2* b0 = bs_sm + Px;
     float2* b1 = b0 + M * ls;
@@ -326,7 +324,7 @@ __global__ void __launch_bounds__(PCM_THREADS) k_fft_x_r2c_tma(const __grid_cons
             }
         }
         __syncthreads();
-        const float2* res = F::run(b0, b1, tw, a.plan, lshift, ls, 2);
+        const float2* res = fft_tile(b0, b1, tw, a.plan, lshift, ls, 2);
         for (int l = wid; l < nlines; l += NW) {
             float2* srow = spec + rowbase + (size_t)l * pitch;
             for (int k = lane; k < pitch; k += 32) {
@@ -651,10 +649,9 @@ __device__ __forceinline__ float2 unit_or_zero(float2 x, float thresh) {
 }
 
 // forward FFT in place on (blockIdx.z ? b : a), one tile per CTA (y lengths whose pipelined tiles do not fit)
-template <class F>
 __global__ void __launch_bounds__(PCM_THREADS, 3) k_fft_strided(const __grid_constant__ StridedArgs a) {
-    const int tshift = F::kStatic ? F::LSHIFT : a.tshift;
-    const int TW = 1 << tshift, N = F::kStatic ? F::N : a.plan.n;
+    const int tshift = a.tshift;
+    const int TW = 1 << tshift, N = a.plan.n;
     const int twpad = (N + 1) & ~1;
     float2* tw = bs_sm;
     float2* B0 = bs_sm + twpad;
@@ -664,7 +661,7 @@ __global__ void __launch_bounds__(PCM_THREADS, 3) k_fft_strided(const __grid_con
     float2* g = (blockIdx.z ? a.b : a.a) + base;
     tile_load<9>(B0, g, a.estride, N, tshift);
     __syncthreads();
-    const float2* res = F::run(B0, B1, tw, a.plan, tshift, TW, 1);
+    const float2* res = fft_tile(B0, B1, tw, a.plan, tshift, TW, 1);
     tile_store(g, res, a.estride, N, tshift);
 }
 
@@ -685,11 +682,10 @@ struct StridedPipeArgs {
     int n_tiles;     // tiles_x * n_other * n_img
 };
 
-template <class F>
 __global__ void __launch_bounds__(PCM_THREADS, 2) k_fft_strided_pipe(const __grid_constant__ StridedPipeArgs p) {
     const StridedArgs& a = p.s;
-    const int tshift = F::kStatic ? F::LSHIFT : a.tshift;
-    const int TW = 1 << tshift, N = F::kStatic ? F::N : a.plan.n;
+    const int tshift = a.tshift;
+    const int TW = 1 << tshift, N = a.plan.n;
     const int twpad = (N + 1) & ~1;
     float2* tw = bs_sm;
     float2* B[3];
@@ -727,7 +723,7 @@ __global__ void __launch_bounds__(PCM_THREADS, 2) k_fft_strided_pipe(const __gri
             cp_async_wait<0>();
         }
         __syncthreads();
-        const float2* res = F::run(cur, pong, tw, a.plan, tshift, TW, 1);
+        const float2* res = fft_tile(cur, pong, tw, a.plan, tshift, TW, 1);
         tile_store(tile_ptr(t), res, a.estride, N, tshift);
         __syncthreads();   // res / cur may be overwritten by the next iteration's prefetch and FFT
     }
@@ -739,11 +735,10 @@ __global__ void __launch_bounds__(PCM_THREADS, 2) k_fft_strided_pipe(const __gri
 //   B(t) lands -> FFT B -> normalise, conj(A) * B
 //   B's buffer is free    -> prefetch A(t+1) under the transform of the product
 //   the transform's scratch buffer is free -> prefetch B(t+1) under the store and FFT A(t+1)
-template <class F>
 __global__ void __launch_bounds__(PCM_THREADS, 2) k_fft_xpower_pipe(const __grid_constant__ StridedPipeArgs p) {
     const StridedArgs& a = p.s;
-    const int tshift = F::kStatic ? F::LSHIFT : a.tshift;
-    const int TW = 1 << tshift, N = F::kStatic ? F::N : a.plan.n;
+    const int tshift = a.tshift;
+    const int TW = 1 << tshift, N = a.plan.n;
     const int twpad = (N + 1) & ~1;
     float2* tw = bs_sm;
     float2* bufA = bs_sm + twpad;
@@ -771,11 +766,11 @@ __global__ void __launch_bounds__(PCM_THREADS, 2) k_fft_xpower_pipe(const __grid
         const bool has_next = tn < p.n_tiles;
         cp_async_wait<1>();            // A(t) landed (B(t) is the newest group)
         __syncthreads();
-        float2* rA = F::run(bufA, pong, tw, a.plan, tshift, TW, 1);
+        float2* rA = fft_tile(bufA, pong, tw, a.plan, tshift, TW, 1);
         float2* freeA = (rA == bufA) ? pong : bufA;
         cp_async_wait<0>();            // B(t) landed
         __syncthreads();
-        float2* rB = F::run(bufB, freeA, tw, a.plan, tshift, TW, 1);
+        float2* rB = fft_tile(bufB, freeA, tw, a.plan, tshift, TW, 1);
         float2* free2 = (rB == bufB) ? freeA : bufB;
         const int tot = N * TW;
         for (int i = threadIdx.x; i < tot; i += blockDim.x) {
@@ -785,7 +780,7 @@ __global__ void __launch_bounds__(PCM_THREADS, 2) k_fft_xpower_pipe(const __grid
         }
         __syncthreads();
         if (has_next) prefetch(a.a + tile_off(tn), rB);          // rB's buffer is free from here on
-        float2* rQ = F::run(rA, free2, tw, a.plan, tshift, TW, 1);
+        float2* rQ = fft_tile(rA, free2, tw, a.plan, tshift, TW, 1);
         float2* otherQ = (rQ == rA) ? free2 : rA;
         if (has_next) prefetch(a.b + tile_off(tn), otherQ);      // scratch of the last transform is free
         tile_store(a.a + tile_off(t), rQ, a.estride, N, tshift);
@@ -1354,13 +1349,12 @@ __global__ void __launch_bounds__(COL540X_NT, 1) k_fft_xy_col540(const __grid_co
 // ------------------------------------------------------------------------------------------
 // x pass, complex -> real, in place
 
-template <class F>
 __global__ void __launch_bounds__(PCM_THREADS) k_fft_x_c2r(const __grid_constant__ XC2RArgs a) {
-    const int M = F::kStatic ? F::N : a.M;
-    const int lshift = F::kStatic ? F::LSHIFT : a.lshift;
+    const int M = a.M;
+    const int lshift = a.lshift;
     const int LB = 1 << lshift, ls = LB + 1;
     const int Px = 2 * M;
-    const int pitch = F::kStatic ? ((F::N + 1 + 15) / 16) * 16 : a.pitch;
+    const int pitch = a.pitch;
     float2* tw = bs_sm;
     float2* T0 = bs_sm + Px;                 // (M+1) * ls
     float2* T1 = T0 + (size_t)(M + 1) * ls;  // M * ls
@@ -1403,7 +1397,7 @@ __global__ void __launch_bounds__(PCM_THREADS) k_fft_x_c2r(const __grid_constant
         T1[k * ls + l] = make_float2(E.x - O.y, -(E.y + O.x));
     }
     __syncthreads();
-    const float2* res = F::run(T1, T0, tw, a.plan, lshift, ls, 2);
+    const float2* res = fft_tile(T1, T0, tw, a.plan, lshift, ls, 2);
     for (int l = wid; l < nlines; l += NW) {
         float2* row = a.spec + rowbase + (size_t)l * pitch;
         for (int n = lane; n < M; n += 32) {
@@ -1542,10 +1536,6 @@ __global__ void __launch_bounds__(PCM_THREADS) k_peaks(const __grid_constant__ P
         }
     }
 }
-
-// compile-time specialisations: padded 512^3 overlaps -> 540^3 (x half-length 270)
-typedef FftStatic<270, 4, 17, 2, PCM_THREADS, 9, 6, 5> FftX270;
-typedef FftStatic<270, 3, 9, 2, PCM_THREADS, 9, 6, 5> FftX270L8;
 
 // ------------------------------------------------------------------------------------------
 // Pearson sums for all candidate shifts in one launch
@@ -2101,7 +2091,7 @@ struct PcmGeometry {
     int lshift_r2c; // log2 lines per CTA in the r2c kernel (fewer lines -> more CTAs/SM to hide load latency)
     int tshift_y, tshift_z;
     size_t smem_x_r2c, smem_x_c2r, smem_y, smem_z;
-    bool static_x, static_y, static_z;  // compile-time specialised kernels apply
+    bool static_y, static_z;  // compile-time specialised kernels apply
 };
 
 struct PcmDeviceTables {
@@ -2164,18 +2154,17 @@ static int pcm_geometry(bs_ctx* ctx, const long long dims[3], const int ext[3], 
     g->pitch = ((g->M + 1 + 15) / 16) * 16;
     if (!make_plan(g->M, &g->plan_x) || !make_plan(g->P[1], &g->plan_y) || !make_plan(g->P[2], &g->plan_z))
         return bs_set_error(ctx, BS_ERR_UNSUPPORTED, "pcm: cannot plan FFT for padded size %dx%dx%d", g->P[0], g->P[1], g->P[2]);
-    // lines per CTA for the x kernels: largest power of two <= 16 that fits shared memory
-    int ls = env_int("BS_FFT_XLINES_LOG2", 4);
+    // lines per CTA for the x kernels: largest power of two <= 16 for which both kernels fit shared memory
+    auto smem_r2c = [&](int ls) { return ((size_t)g->P[0] + 2 * (size_t)g->M * ((1 << ls) + 1)) * sizeof(float2); };
+    int ls = 4;
     for (;; --ls) {
-        const int LB = 1 << ls;
-        g->smem_x_r2c = ((size_t)g->P[0] + 2 * (size_t)g->M * (LB + 1)) * sizeof(float2);
-        g->smem_x_c2r = ((size_t)g->P[0] + (size_t)(2 * g->M + 1) * (LB + 1)) * sizeof(float2);
-        if (g->smem_x_c2r <= PCM_SMEM_MAX && g->smem_x_r2c <= PCM_SMEM_MAX) break;
+        g->smem_x_c2r = ((size_t)g->P[0] + (size_t)(2 * g->M + 1) * ((1 << ls) + 1)) * sizeof(float2);
+        if (g->smem_x_c2r <= PCM_SMEM_MAX && smem_r2c(ls) <= PCM_SMEM_MAX) break;
         if (ls == 0) return bs_set_error(ctx, BS_ERR_UNSUPPORTED, "pcm: x size %d too large for shared memory", g->P[0]);
     }
     g->lshift_x = ls;
-    g->lshift_r2c = std::min(ls, env_int("BS_FFT_R2C_LINES_LOG2", 3));
-    g->smem_x_r2c = ((size_t)g->P[0] + 2 * (size_t)g->M * ((1 << g->lshift_r2c) + 1)) * sizeof(float2);
+    g->lshift_r2c = std::min(ls, 3);
+    g->smem_x_r2c = smem_r2c(g->lshift_r2c);
     auto strided = [&](int N, int nbuf, int pref, int* tshift, size_t* smem) -> bool {
         for (int ts = pref; ts >= 1; --ts) {
             const size_t b = ((size_t)((N + 1) & ~1) + (size_t)nbuf * N * (1 << ts)) * sizeof(float2);
@@ -2187,8 +2176,6 @@ static int pcm_geometry(bs_ctx* ctx, const long long dims[3], const int ext[3], 
         !strided(g->P[2], 3, env_int("BS_FFT_ZTILE_LOG2", 3), &g->tshift_z, &g->smem_z))
         return bs_set_error(ctx, BS_ERR_UNSUPPORTED, "pcm: y/z size %dx%d too large for shared memory", g->P[1], g->P[2]);
     const bool allow_static = env_int("BS_FFT_STATIC", 1) != 0;
-    g->static_x = allow_static && g->M == FftX270::N && (g->lshift_x == FftX270::LSHIFT || g->lshift_x == FftX270L8::LSHIFT) &&
-                  (g->lshift_r2c == 3 || g->lshift_r2c == 4);
     // k_fft_col540 / k_fft_xpower_col540: the pitch (a multiple of 16) always divides into 16-column tiles
     g->static_y = allow_static && g->P[1] == Col540::N;
     g->static_z = allow_static && g->P[2] == Col540::N;
@@ -2279,9 +2266,8 @@ static int pcm_sync_handoff(bs_ctx* ctx) {
     return pcm_handoff_error(ctx, code);
 }
 
-static int set_smem(bs_ctx* ctx, const void* fn, size_t bytes) {
+static int set_smem(bs_ctx* ctx, const void* fn) {
     BS_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PCM_SMEM_MAX));
-    (void)bytes;
     return BS_OK;
 }
 
@@ -2322,34 +2308,28 @@ static int launch_col540(bs_ctx* ctx, const StridedArgs& a, int tiles_x, int n_o
 static int pcm_kernel_attrs(bs_ctx* ctx) {
     if (ctx->pcm_attr_done) return BS_OK;
     int rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c<FftGeneric>, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_strided<FftGeneric>, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r<FftGeneric>, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c<FftX270>, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c<FftX270L8>, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_tma<FftX270L8>, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_w<FftW270S>, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_w<FftWGeneric>, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r_w<FftW270>, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r_w<FftWGeneric>, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_tma<FftX270>, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_tma<FftGeneric>, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r<FftX270L8>, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_strided_pipe<FftGeneric>, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_xpower_pipe<FftGeneric>, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_col540, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_xpower_col540, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r<FftX270>, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_col540, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r_col540, 0))) return rc;
-    if ((rc = set_smem(ctx, (const void*)k_fft_xy_col540, 0))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_strided))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_w<FftW270S>))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_w<FftWGeneric>))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r_w<FftW270>))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r_w<FftWGeneric>))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_tma))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_strided_pipe))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_xpower_pipe))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_col540))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_xpower_col540))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_r2c_col540))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_x_c2r_col540))) return rc;
+    if ((rc = set_smem(ctx, (const void*)k_fft_xy_col540))) return rc;
     ctx->pcm_attr_done = true;
     return BS_OK;
 }
 
 // The five FFT passes.  Each launches one kernel on ctx->stream and, when `info` is not NULL, writes the
 // instantiation it chose (plus the plan's radices for runtime-planned kernels), e.g.
-// "k_fft_strided_pipe<FftGeneric> 15x12x3", into info[PCM_INFO_LEN].  bs_pcm_debug_pass runs them one at a time.
+// "k_fft_strided_pipe 15x12x3", into info[PCM_INFO_LEN].  bs_pcm_debug_pass runs them one at a time.
 #define PCM_INFO_LEN 128
 static void pass_info(char* info, const char* kernel, const FftPlan* plan) {
     if (!info) return;
@@ -2449,25 +2429,11 @@ static int pcm_pass_x_r2c(bs_ctx* ctx, const void* d1, const void* d2, int dtype
             m.esize = esize;
             const int per_sm = std::max(1, (int)(PCM_SMEM_MAX / (smem_tma + 1024)));
             const int nctas = std::min(m.n_items, ctx->sm_count * std::min(per_sm, 4));
-            if (g.static_x && g.lshift_r2c == 3) {
-                k_fft_x_r2c_tma<FftX270L8><<<nctas, PCM_THREADS, smem_tma, ctx->stream>>>(m);
-                pass_info(info, "k_fft_x_r2c_tma<FftX270L8>", nullptr);
-            } else if (g.static_x && g.lshift_r2c == 4) {
-                k_fft_x_r2c_tma<FftX270><<<nctas, PCM_THREADS, smem_tma, ctx->stream>>>(m);
-                pass_info(info, "k_fft_x_r2c_tma<FftX270>", nullptr);
-            } else {
-                k_fft_x_r2c_tma<FftGeneric><<<nctas, PCM_THREADS, smem_tma, ctx->stream>>>(m);
-                pass_info(info, "k_fft_x_r2c_tma<FftGeneric>", &g.plan_x);
-            }
-        } else if (g.static_x && g.lshift_r2c == 3) {
-            k_fft_x_r2c<FftX270L8><<<grid, PCM_THREADS, g.smem_x_r2c, ctx->stream>>>(a);
-            pass_info(info, "k_fft_x_r2c<FftX270L8>", nullptr);
-        } else if (g.static_x && g.lshift_r2c == 4) {
-            k_fft_x_r2c<FftX270><<<grid, PCM_THREADS, g.smem_x_r2c, ctx->stream>>>(a);
-            pass_info(info, "k_fft_x_r2c<FftX270>", nullptr);
+            k_fft_x_r2c_tma<<<nctas, PCM_THREADS, smem_tma, ctx->stream>>>(m);
+            pass_info(info, "k_fft_x_r2c_tma", &g.plan_x);
         } else {
-            k_fft_x_r2c<FftGeneric><<<grid, PCM_THREADS, g.smem_x_r2c, ctx->stream>>>(a);
-            pass_info(info, "k_fft_x_r2c<FftGeneric>", &g.plan_x);
+            k_fft_x_r2c<<<grid, PCM_THREADS, g.smem_x_r2c, ctx->stream>>>(a);
+            pass_info(info, "k_fft_x_r2c", &g.plan_x);
         }
     }
     BS_CUDA(ctx, cudaGetLastError());
@@ -2500,11 +2466,11 @@ static int pcm_launch_y(bs_ctx* ctx, const PcmGeometry& g, PcmDeviceTables* t, i
             pp.n_tiles = pp.tiles_x * pp.n_other * n_img;
             const int per_sm = std::max(1, std::min(2, (int)(PCM_SMEM_MAX / (smem_pipe + 1024))));
             const int nctas = std::min(pp.n_tiles, ctx->sm_count * per_sm);
-            k_fft_strided_pipe<FftGeneric><<<nctas, PCM_THREADS, smem_pipe, ctx->stream>>>(pp);
-            pass_info(info, "k_fft_strided_pipe<FftGeneric>", &g.plan_y);
+            k_fft_strided_pipe<<<nctas, PCM_THREADS, smem_pipe, ctx->stream>>>(pp);
+            pass_info(info, "k_fft_strided_pipe", &g.plan_y);
         } else {
-            k_fft_strided<FftGeneric><<<grid, PCM_THREADS, g.smem_y, ctx->stream>>>(a);
-            pass_info(info, "k_fft_strided<FftGeneric>", &g.plan_y);
+            k_fft_strided<<<grid, PCM_THREADS, g.smem_y, ctx->stream>>>(a);
+            pass_info(info, "k_fft_strided", &g.plan_y);
         }
     }
     BS_CUDA(ctx, cudaGetLastError());
@@ -2541,8 +2507,8 @@ static int pcm_pass_z_xpower(bs_ctx* ctx, const PcmGeometry& g, PcmDeviceTables*
             pp.n_tiles = pp.tiles_x * pp.n_other;
             const int per_sm = std::max(1, std::min(2, (int)(PCM_SMEM_MAX / (g.smem_z + 1024))));
             const int nctas = std::min(pp.n_tiles, ctx->sm_count * per_sm);
-            k_fft_xpower_pipe<FftGeneric><<<nctas, PCM_THREADS, g.smem_z, ctx->stream>>>(pp);
-            pass_info(info, "k_fft_xpower_pipe<FftGeneric>", &g.plan_z);
+            k_fft_xpower_pipe<<<nctas, PCM_THREADS, g.smem_z, ctx->stream>>>(pp);
+            pass_info(info, "k_fft_xpower_pipe", &g.plan_z);
         }
     }
     BS_CUDA(ctx, cudaGetLastError());
@@ -2588,15 +2554,9 @@ static int pcm_pass_x_c2r(bs_ctx* ctx, const PcmGeometry& g, PcmDeviceTables* t,
                 k_fft_x_c2r_w<FftWGeneric><<<nctas, PCM_THREADS, smem_w, ctx->stream>>>(a);
                 pass_info(info, "k_fft_x_c2r_w<FftWGeneric>", &g.plan_x);
             }
-        } else if (g.static_x && g.lshift_x == 3) {
-            k_fft_x_c2r<FftX270L8><<<grid, PCM_THREADS, g.smem_x_c2r, ctx->stream>>>(a);
-            pass_info(info, "k_fft_x_c2r<FftX270L8>", nullptr);
-        } else if (g.static_x) {
-            k_fft_x_c2r<FftX270><<<grid, PCM_THREADS, g.smem_x_c2r, ctx->stream>>>(a);
-            pass_info(info, "k_fft_x_c2r<FftX270>", nullptr);
         } else {
-            k_fft_x_c2r<FftGeneric><<<grid, PCM_THREADS, g.smem_x_c2r, ctx->stream>>>(a);
-            pass_info(info, "k_fft_x_c2r<FftGeneric>", &g.plan_x);
+            k_fft_x_c2r<<<grid, PCM_THREADS, g.smem_x_c2r, ctx->stream>>>(a);
+            pass_info(info, "k_fft_x_c2r", &g.plan_x);
         }
     }
     BS_CUDA(ctx, cudaGetLastError());

@@ -254,71 +254,6 @@ __device__ __forceinline__ float2* fft_tile(float2* a, float2* b, const float2* 
 
 
 // ------------------------------------------------------------------------------------------
-// Compile-time plans.  For the transform lengths that dominate real workloads (the padded
-// sizes of 512^3 / 256^3 overlaps) every stride, trip count and twiddle step is a constant:
-// shared-memory accesses use immediate offsets, `j % Ls` becomes a multiply-shift and the
-// item loops are fully unrolled.  Other lengths run the generic runtime-planned path above.
-template <int N, int R, int LS, int LSHIFT, int LSTRIDE, int TWMUL, int NT>
-__device__ __forceinline__ void fft_stage_s(const float2* __restrict__ in, float2* __restrict__ out,
-                                            const float2* __restrict__ tw) {
-    constexpr int m = N / R;
-    constexpr int nitems = m << LSHIFT;
-    constexpr int lmask = (1 << LSHIFT) - 1;
-    constexpr int twstep = (N / (LS * R)) * TWMUL;
-    constexpr int iters = (nitems + NT - 1) / NT;
-#pragma unroll
-    for (int it = 0; it < iters; ++it) {
-        const int item = threadIdx.x + it * NT;
-        if ((nitems % NT) != 0 && it == iters - 1 && item >= nitems) break;
-        const int j = item >> LSHIFT;
-        const int l = item & lmask;
-        const int k = (LS == 1) ? 0 : (j % LS);
-        float2 x[R];
-        const float2* p = in + j * LSTRIDE + l;
-#pragma unroll
-        for (int q = 0; q < R; ++q) x[q] = p[q * m * LSTRIDE];
-        if (LS > 1) {
-            const float2* t = tw + k * twstep;
-#pragma unroll
-            for (int q = 1; q < R; ++q) x[q] = cmulf(x[q], t[(q - 1) * k * twstep]);
-        }
-        dft<R>(x);
-        float2* o = out + ((j - k) * R + k) * LSTRIDE + l;
-#pragma unroll
-        for (int q = 0; q < R; ++q) o[q * LS * LSTRIDE] = x[q];
-    }
-}
-
-template <int N, int LS, int LSHIFT, int LSTRIDE, int TWMUL, int NT, int R, int... Rest>
-__device__ __forceinline__ float2* fft_tile_s(float2* a, float2* b, const float2* tw) {
-    fft_stage_s<N, R, LS, LSHIFT, LSTRIDE, TWMUL, NT>(a, b, tw);
-    __syncthreads();
-    if constexpr (sizeof...(Rest) == 0) return b;
-    else return fft_tile_s<N, LS * R, LSHIFT, LSTRIDE, TWMUL, NT, Rest...>(b, a, tw);
-}
-
-// Policy types the kernels are templated on.
-struct FftGeneric {
-    static constexpr bool kStatic = false;
-    static constexpr int N = 0, LSHIFT = 0;
-    static __device__ __forceinline__ float2* run(float2* a, float2* b, const float2* tw, const FftPlan& plan,
-                                                  int lshift, int lstride, int twmul) {
-        return fft_tile(a, b, tw, plan, lshift, lstride, twmul);
-    }
-};
-
-template <int N_, int LSHIFT_, int LSTRIDE_, int TWMUL_, int NT_, int... Rs>
-struct FftStatic {
-    static constexpr bool kStatic = true;
-    static constexpr int N = N_, LSHIFT = LSHIFT_;
-    static __device__ __forceinline__ float2* run(float2* a, float2* b, const float2* tw, const FftPlan&, int, int,
-                                                  int) {
-        return fft_tile_s<N_, 1, LSHIFT_, LSTRIDE_, TWMUL_, NT_, Rs...>(a, b, tw);
-    }
-};
-
-
-// ------------------------------------------------------------------------------------------
 // Register-resident two-stage transform of a column tile: TC columns of N = RA * RB points, element n of column
 // c at g[n * estride + c].  Cooley-Tukey with n = RB n1 + n2 and k = k1 + RA k2:
 //   stage 1  item (n2, c) holds x[RB n1 + n2], n1 < RA, in registers: dft<RA>, times W_N^(n2 k1), and ONE write

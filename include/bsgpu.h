@@ -155,7 +155,7 @@ int bs_pcm_debug_pcm(bs_ctx* ctx, const void* img1, const void* img2, const long
  * in_b / out_b are ignored (may be NULL) for passes 3 and 4, out_b also for pass 2.  poison != 0 fills the device
  * spectra with NaN bytes first, so anything a pass fails to write shows up as NaN.  info (may be NULL) receives the
  * kernel instantiation launched, and for runtime-planned kernels the radices of the plan, e.g.
- * "k_fft_strided_pipe<FftGeneric> 15x12x3" (NUL-terminated, at most 128 bytes). */
+ * "k_fft_strided_pipe 15x12x3" (NUL-terminated, at most 128 bytes). */
 int bs_pcm_debug_pass(bs_ctx* ctx, int pass, const long long dims[3], int dtype, const int extension[3],
                       const void* in_a, const void* in_b, void* out_a, void* out_b, int poison, int pad_out[3],
                       char info[128]);

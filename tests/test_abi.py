@@ -79,3 +79,9 @@ def test_product_never_imports_oracle():
             if fn.endswith((".py", ".cu", ".cuh", ".cpp", ".h")):
                 txt = open(os.path.join(dirpath, fn)).read()
                 assert not re.search(r"^\s*(from|import)\s+oracle", txt, flags=re.M), fn
+
+
+def test_pcm_switch_list_matches_the_source():
+    from tests.pcm_switches import SWITCHES
+    src = open(os.path.join(ROOT, "bigstitcher-spark_b200", "csrc", "pcm.cu")).read()
+    assert sorted(SWITCHES) == sorted(set(re.findall(r'env_int\("(BS_FFT_\w+)"', src)))

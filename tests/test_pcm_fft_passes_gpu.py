@@ -18,11 +18,10 @@ import pytest
 from oracle import pcm_oracle as po
 from oracle import pcm_passes as pp
 from tests import synth
+from tests.pcm_switches import set_switches
 
 pytestmark = pytest.mark.gpu
 
-ENV = ("BS_FFT_X_WARP", "BS_FFT_R2C_TMA", "BS_FFT_R2C_LINES_LOG2", "BS_FFT_XLINES_LOG2", "BS_FFT_STATIC",
-       "BS_FFT_YTILE_LOG2", "BS_FFT_ZTILE_LOG2")
 #: allowed worst-line error, in multiples of scipy's single-precision worst-line error (floored at one float32 ulp,
 #: so that a length scipy happens to transform exactly does not make the bar 0)
 BAR = 8.0
@@ -31,9 +30,9 @@ RADICES = {16, 15, 12, 10, 9, 8, 6, 5, 4, 3, 2}
 #: generic (runtime-planned) kernel families whose plans must, together, use every radix of the planner
 FAMILIES = {
     "warp-x": ("k_fft_x_r2c_w<FftWGeneric>", "k_fft_x_c2r_w<FftWGeneric>"),
-    "cta-x": ("k_fft_x_r2c<FftGeneric>", "k_fft_x_r2c_tma<FftGeneric>", "k_fft_x_c2r<FftGeneric>"),
-    "strided-pipe": ("k_fft_strided_pipe<FftGeneric>",),
-    "strided": ("k_fft_strided<FftGeneric>",),
+    "cta-x": ("k_fft_x_r2c", "k_fft_x_r2c_tma", "k_fft_x_c2r"),
+    "strided-pipe": ("k_fft_strided_pipe",),
+    "strided": ("k_fft_strided",),
 }
 #: k_fft_strided only runs y lengths whose pipelined tiles do not fit shared memory (1161..1709 and 2236..3228 with
 #: the default tiles, 594..880 with 16-column tiles, 4151..5811); no 5-smooth length there has a radix-8 plan
@@ -75,64 +74,51 @@ CASES = [
     case(0, (520, 6, 3), "k_fft_x_r2c_w<FftW270S>", dtype="u8"),
     case(0, (520, 6, 3), "k_fft_x_r2c_w<FftWGeneric> tma", env=STATIC0),
     *[case(0, (crop_for(2 * m, True), 5, 2), "k_fft_x_r2c_w<FftWGeneric>") for m in GEN],
-    case(0, (520, 6, 3), "k_fft_x_r2c_tma<FftX270L8>", env={**CTA, "BS_FFT_R2C_LINES_LOG2": 3}),
-    case(0, (520, 6, 3), "k_fft_x_r2c_tma<FftX270>", env={**CTA, "BS_FFT_R2C_LINES_LOG2": 4}),
-    case(0, (520, 6, 3), "k_fft_x_r2c<FftX270L8>", env={**CTA_NOTMA, "BS_FFT_R2C_LINES_LOG2": 3}),
-    case(0, (520, 6, 3), "k_fft_x_r2c<FftX270>", env={**CTA_NOTMA, "BS_FFT_R2C_LINES_LOG2": 4}),
-    case(0, (520, 6, 3), "k_fft_x_r2c<FftX270L8>", env=CTA, misalign=1, tag="-misaligned"),
-    *[case(0, (crop_for(2 * m, True), 5, 2), "k_fft_x_r2c<FftGeneric>", env=CTA_NOTMA) for m in GEN],
-    case(0, (340, 5, 2), "k_fft_x_r2c_tma<FftGeneric>", dtype="f32", env=CTA),
-    case(0, (784, 7, 2), "k_fft_x_r2c_tma<FftGeneric>"),                 # M = 405 > 319: CTA kernels by default
-    case(0, (790, 7, 2), "k_fft_x_r2c<FftGeneric>"),                     # ... without TMA (row of 1580 B)
-    case(0, (790, 7, 2), "k_fft_x_r2c<FftGeneric>", dtype="f32"),
-    case(0, (4000, 3, 1), "k_fft_x_r2c<FftGeneric>"),                    # M = 2025: 4 lines per CTA
-    case(0, (4000, 3, 1), "k_fft_x_r2c_tma<FftGeneric>", dtype="u8"),    # ... and its staged rows still fit
+    case(0, (crop_for(2 * 180, True), 5, 2), "k_fft_x_r2c", env=CTA, misalign=1, tag="-misaligned"),
+    *[case(0, (crop_for(2 * m, True), 5, 2), "k_fft_x_r2c", env=CTA_NOTMA) for m in GEN],
+    case(0, (340, 5, 2), "k_fft_x_r2c_tma", dtype="f32", env=CTA),
+    case(0, (784, 7, 2), "k_fft_x_r2c_tma"),                 # M = 405 > 319: CTA kernels by default
+    case(0, (790, 7, 2), "k_fft_x_r2c"),                     # ... without TMA (row of 1580 B)
+    case(0, (790, 7, 2), "k_fft_x_r2c", dtype="f32"),
+    case(0, (4000, 3, 1), "k_fft_x_r2c"),                    # M = 2025: 4 lines per CTA
+    case(0, (4000, 3, 1), "k_fft_x_r2c_tma", dtype="u8"),    # ... and its staged rows still fit
     *[case(0, d, "k_fft_x_r2c_w<FftWGeneric>") for d in EDGES],
-    *[case(0, d, "k_fft_x_r2c<FftGeneric>", env=CTA_NOTMA) for d in EDGES],
+    *[case(0, d, "k_fft_x_r2c", env=CTA_NOTMA) for d in EDGES],
     # ---- pass 1: y forward of both spectra
     case(1, (12, 520, 3), "k_fft_col540"),
     case(1, (520, 520, 2), "k_fft_col540"),
-    case(1, (12, 520, 3), "k_fft_strided_pipe<FftGeneric>", env=STATIC0),
-    *[case(1, (10, crop_for(p), 2), "k_fft_strided_pipe<FftGeneric>") for p in GEN],
+    case(1, (12, 520, 3), "k_fft_strided_pipe", env=STATIC0),
+    *[case(1, (10, crop_for(p), 2), "k_fft_strided_pipe") for p in GEN],
     # k_fft_strided: Py = 1200 (15x5x16), 1458 (9x9x9x2), 1620 (15x9x12), 1440 (15x16x6), 2400 (15x16x10, 4-column
     # tiles); with 16-column tiles Py = 600 (15x10x4) and 675 (15x15x3)
-    case(1, (12, 1180, 1), "k_fft_strided<FftGeneric>"),
-    *[case(1, (10, crop_for(p), 1), "k_fft_strided<FftGeneric>") for p in (1458, 1620, 1440, 2400)],
-    *[case(1, (10, crop_for(p), 1), "k_fft_strided<FftGeneric>", env={"BS_FFT_YTILE_LOG2": 4}) for p in (600, 675)],
-    *[case(1, d, "k_fft_strided_pipe<FftGeneric>") for d in EDGES],
+    case(1, (12, 1180, 1), "k_fft_strided"),
+    *[case(1, (10, crop_for(p), 1), "k_fft_strided") for p in (1458, 1620, 1440, 2400)],
+    *[case(1, (10, crop_for(p), 1), "k_fft_strided", env={"BS_FFT_YTILE_LOG2": 4}) for p in (600, 675)],
+    *[case(1, d, "k_fft_strided_pipe") for d in EDGES],
     # ---- pass 2: z cross-power
     case(2, (12, 6, 520), "k_fft_xpower_col540"),
     case(2, (10, 13, 520), "k_fft_xpower_col540"),
-    case(2, (12, 6, 520), "k_fft_xpower_pipe<FftGeneric>", env=STATIC0),
-    case(2, (12, 5, 44), "k_fft_xpower_pipe<FftGeneric>"),
-    case(2, (12, 5, 25), "k_fft_xpower_pipe<FftGeneric>", env={"BS_FFT_ZTILE_LOG2": 2}),
-    *[case(2, d, "k_fft_xpower_pipe<FftGeneric>") for d in EDGES],
+    case(2, (12, 6, 520), "k_fft_xpower_pipe", env=STATIC0),
+    case(2, (12, 5, 44), "k_fft_xpower_pipe"),
+    case(2, (12, 5, 25), "k_fft_xpower_pipe", env={"BS_FFT_ZTILE_LOG2": 2}),
+    *[case(2, d, "k_fft_xpower_pipe") for d in EDGES],
     # ---- pass 3: y forward of the product
     case(3, (12, 520, 3), "k_fft_col540"),
-    case(3, (12, 520, 3), "k_fft_strided_pipe<FftGeneric>", env=STATIC0),
-    case(3, (10, 25, 3), "k_fft_strided_pipe<FftGeneric>"),
-    case(3, (12, 1180, 1), "k_fft_strided<FftGeneric>"),
-    case(3, (10, crop_for(600), 1), "k_fft_strided<FftGeneric>", env={"BS_FFT_YTILE_LOG2": 4}),
-    *[case(3, d, "k_fft_strided_pipe<FftGeneric>") for d in EDGES],
+    case(3, (12, 520, 3), "k_fft_strided_pipe", env=STATIC0),
+    case(3, (10, 25, 3), "k_fft_strided_pipe"),
+    case(3, (12, 1180, 1), "k_fft_strided"),
+    case(3, (10, crop_for(600), 1), "k_fft_strided", env={"BS_FFT_YTILE_LOG2": 4}),
+    *[case(3, d, "k_fft_strided_pipe") for d in EDGES],
     # ---- pass 4: x c2r
     case(4, (520, 6, 3), "k_fft_x_c2r_w<FftW270>"),
     case(4, (520, 6, 3), "k_fft_x_c2r_w<FftWGeneric>", env=STATIC0),
     *[case(4, (crop_for(2 * m, True), 5, 2), "k_fft_x_c2r_w<FftWGeneric>") for m in GEN],
-    case(4, (520, 6, 3), "k_fft_x_c2r<FftX270L8>", env={**CTA, "BS_FFT_XLINES_LOG2": 3}),
-    case(4, (520, 6, 3), "k_fft_x_c2r<FftX270>", env={**CTA, "BS_FFT_XLINES_LOG2": 4}),
-    *[case(4, (crop_for(2 * m, True), 5, 2), "k_fft_x_c2r<FftGeneric>", env=CTA) for m in GEN],
-    case(4, (790, 7, 2), "k_fft_x_c2r<FftGeneric>"),
-    case(4, (4000, 3, 1), "k_fft_x_c2r<FftGeneric>"),
+    *[case(4, (crop_for(2 * m, True), 5, 2), "k_fft_x_c2r", env=CTA) for m in GEN],
+    case(4, (790, 7, 2), "k_fft_x_c2r"),
+    case(4, (4000, 3, 1), "k_fft_x_c2r"),
     *[case(4, d, "k_fft_x_c2r_w<FftWGeneric>") for d in EDGES],
-    *[case(4, d, "k_fft_x_c2r<FftGeneric>", env=CTA) for d in EDGES],
+    *[case(4, d, "k_fft_x_c2r", env=CTA) for d in EDGES],
 ]
-
-
-def _set_env(monkeypatch, env):
-    for k in ENV:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, str(v))
 
 
 def _kernel(info):
@@ -248,7 +234,7 @@ def _check_linear(got, ref, f32, axis, what):
 
 @pytest.mark.parametrize("pass_no,dims,kernel,dtype,env,misalign", CASES)
 def test_fft_pass(ctx, monkeypatch, pass_no, dims, kernel, dtype, env, misalign):
-    _set_env(monkeypatch, env)
+    set_switches(monkeypatch, env)
     P, M = _geometry(dims)
     seed = sum(dims) * 7 + pass_no
     rng = np.random.default_rng(seed)
@@ -310,7 +296,7 @@ def test_generic_plans_cover_every_radix(ctx, monkeypatch):
         fam = [f for f, ks in FAMILIES.items() if kernel in ks]
         if not fam:
             continue
-        _set_env(monkeypatch, env)
+        set_switches(monkeypatch, env)
         P, M = _geometry(dims)
         if pass_no == 0:
             a, b = _crops(dims, dtype, 1)

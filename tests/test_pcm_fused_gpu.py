@@ -13,20 +13,13 @@ import numpy as np
 import pytest
 
 from tests import synth
+from tests.pcm_switches import set_switches
 
 pytestmark = pytest.mark.gpu
 
-ENV = ("BS_FFT_XY_FUSE", "BS_FFT_XY_KX", "BS_FFT_XY_WINDOW", "BS_FFT_X_COL540", "BS_FFT_STATIC")
 XY = "k_fft_xy_col540"
 # dz -> Pz with the extension 10: 3 -> 9 (odd, below the window), 4 -> 12, 61 -> 81 (odd, several windows deep)
 DZ = [3, 4, 61]
-
-
-def _set_env(monkeypatch, **env):
-    for k in ENV:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, str(v))
 
 
 def _geometry(dims):
@@ -55,10 +48,10 @@ def _same_bits(x, y):
 def test_forward_matches_two_passes(ctx, monkeypatch, dz, env):
     dims = (512, 512, dz)
     ta, tb = _device_crops(dims, 11 * dz)
-    _set_env(monkeypatch, **env)
+    set_switches(monkeypatch, env)
     fa, fb, info = ctx.pcm_debug_pass(5, dims, ta, tb)
     assert info == XY, info
-    _set_env(monkeypatch, BS_FFT_XY_FUSE=0)
+    set_switches(monkeypatch, {"BS_FFT_XY_FUSE": 0})
     xa, xb, _ = ctx.pcm_debug_pass(0, dims, ta, tb)
     ya, yb, _ = ctx.pcm_debug_pass(1, dims, xa, xb)
     for got, ref in ((fa, ya), (fb, yb)):
@@ -69,7 +62,7 @@ def test_forward_matches_two_passes(ctx, monkeypatch, dz, env):
 def test_fused_pass_repeats_bit_identically(ctx, monkeypatch):
     dims = (512, 512, 61)
     ta, tb = _device_crops(dims, 3)
-    _set_env(monkeypatch)
+    set_switches(monkeypatch)
     first = ctx.pcm_debug_pass(5, dims, ta, tb)[:2]
     again = ctx.pcm_debug_pass(5, dims, ta, tb)[:2]
     for x, y in zip(first, again):
@@ -79,13 +72,13 @@ def test_fused_pass_repeats_bit_identically(ctx, monkeypatch):
 def test_dispatch_rule(ctx, monkeypatch):
     dims = (512, 512, 4)
     ta, tb = _device_crops(dims, 1)
-    _set_env(monkeypatch)
+    set_switches(monkeypatch)
     assert ctx.pcm_debug_pass(5, dims, ta, tb)[2] == XY
     # the switch keeps the five-pass chain
-    _set_env(monkeypatch, BS_FFT_XY_FUSE=0)
+    set_switches(monkeypatch, {"BS_FFT_XY_FUSE": 0})
     assert ctx.pcm_debug_pass(5, dims, ta, tb)[2] == "k_fft_x_r2c_col540 + k_fft_col540"
     # Py != 540: the y pass is not Col540's
-    _set_env(monkeypatch)
+    set_switches(monkeypatch)
     dims_y = (512, 480, 4)
     ua, ub = _device_crops(dims_y, 2)
     assert _geometry(dims_y)[0][1] != 540
@@ -105,7 +98,7 @@ def test_pair_results_identical(ctx, monkeypatch):
     p = ctx.pcm_params(peaks_to_check=5, do_subpixel=True, min_overlap_frac=0.25, extension=(10, 10, 10))
     res = {}
     for fuse in (0, 1):
-        _set_env(monkeypatch, BS_FFT_XY_FUSE=fuse)
+        set_switches(monkeypatch, {"BS_FFT_XY_FUSE": fuse})
         res[fuse] = dataclasses.asdict(ctx.pcm_pair(imgs1[0], imgs2[0], p, dtype=None))
     assert res[1]["found"]
     assert res[0] == res[1]

@@ -168,7 +168,7 @@ def test_oversized_dims_rejected_before_any_copy(ctx):
 
 
 # ---- the code paths bench.py runs: compile-time plans for padded length 540 (x: FftWStatic<270>, y/z:
-# FftStatic<540> two-stage 27x20, cp.async pipelined y pass, z cross-power pass).  The static plans are
+# k_fft_col540 y pass and k_fft_xpower_col540 z cross-power pass on RegFft2<20, 27>).  The static plans are
 # selected per axis, so three thin crops reach each of them cheaply; the full 512^3 pair is the bench unit.
 @pytest.mark.parametrize("shape,shift", [
     ((24, 24, 500), (7, -3, 2)),     # x pads to 540  -> k_fft_x_r2c_w / k_fft_x_c2r_w <FftWStatic<270>>

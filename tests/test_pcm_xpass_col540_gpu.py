@@ -11,23 +11,15 @@ import pytest
 from oracle import pcm_oracle as po
 from oracle import pcm_passes as pp
 from tests import synth
+from tests.pcm_switches import set_switches
 
 pytestmark = pytest.mark.gpu
 
-ENV = ("BS_FFT_X_COL540", "BS_FFT_X_WARP", "BS_FFT_R2C_TMA", "BS_FFT_R2C_LINES_LOG2", "BS_FFT_XLINES_LOG2",
-       "BS_FFT_STATIC")
 BAR = 8.0
 ULP32 = 2.0 ** -24
 _DT = {"u16": (np.uint16, 0), "f32": (np.float32, 1), "u8": (np.uint8, 2)}
 R2C, C2R = "k_fft_x_r2c_col540", "k_fft_x_c2r_col540"
 FORCE = {"BS_FFT_X_COL540": 2}
-
-
-def _set_env(monkeypatch, env):
-    for k in ENV:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in env.items():
-        monkeypatch.setenv(k, str(v))
 
 
 def _crops(dims, dtype, seed):
@@ -96,7 +88,7 @@ GEOMS = ((512, 100, 60), (520, 13, 7), (520, 25, 5))
 
 @pytest.mark.parametrize("dims", GEOMS)
 def test_r2c_col540(ctx, monkeypatch, dims):
-    _set_env(monkeypatch, FORCE)
+    set_switches(monkeypatch, FORCE)
     a, b, out_a, out_b, info = _pass0(ctx, dims)
     assert info == R2C, info
     assert np.isfinite(out_a).all() and np.isfinite(out_b).all()
@@ -106,7 +98,7 @@ def test_r2c_col540(ctx, monkeypatch, dims):
 
 def test_r2c_col540_blank_rows_stay_zero(ctx, monkeypatch):
     """A row that is zero in one crop only: its spectrum is exactly 0, not the partner row's rounding noise."""
-    _set_env(monkeypatch, FORCE)
+    set_switches(monkeypatch, FORCE)
     dims = (520, 13, 7)
     a, b, out_a, out_b, info = _pass0(ctx, dims, blank=((0, 3, 5), (1, 4, 9), (0, 0, 0)))
     assert info == R2C, info
@@ -116,7 +108,7 @@ def test_r2c_col540_blank_rows_stay_zero(ctx, monkeypatch):
 
 @pytest.mark.parametrize("dims", GEOMS)
 def test_c2r_col540(ctx, monkeypatch, dims):
-    _set_env(monkeypatch, FORCE)
+    set_switches(monkeypatch, FORCE)
     s, P = _spectrum(dims, sum(dims) + 4)
     out, _, info = ctx.pcm_debug_pass(4, dims, s)
     assert info == C2R, info
@@ -132,7 +124,7 @@ def test_c2r_col540(ctx, monkeypatch, dims):
 ], ids=["misaligned", "u8", "f32", "odd-row"])
 def test_r2c_falls_back(ctx, monkeypatch, dims, dtype, misalign, kernel):
     """Crops the staged-row kernel does not take keep today's kernel even when the Col540 kernels are forced."""
-    _set_env(monkeypatch, FORCE)
+    set_switches(monkeypatch, FORCE)
     a, b, out_a, out_b, info = _pass0(ctx, dims, dtype, misalign)
     assert info == kernel, info
     _check_linear(out_a, pp.pass0(a), pp.pass0_f32(a), 2, info + " (A)")
@@ -145,14 +137,14 @@ def test_default_rule_by_tile_count(ctx, monkeypatch):
     for env, dims, r2c, c2r in (({}, small, warp_r2c, "k_fft_x_c2r_w<FftW270>"),
                                 ({}, large, R2C, C2R),
                                 ({"BS_FFT_X_COL540": 0}, large, warp_r2c, "k_fft_x_c2r_w<FftW270>")):
-        _set_env(monkeypatch, env)
+        set_switches(monkeypatch, env)
         assert _pass0(ctx, dims)[4] == r2c, (env, dims)
         s, _ = _spectrum(dims, 1)
         assert ctx.pcm_debug_pass(4, dims, s)[2] == c2r, (env, dims)
 
 
 def test_col540_runs_are_bit_identical(ctx, monkeypatch):
-    _set_env(monkeypatch, FORCE)
+    set_switches(monkeypatch, FORCE)
     dims = (512, 100, 60)
     first = _pass0(ctx, dims, seed=3)
     again = _pass0(ctx, dims, seed=3)
@@ -167,7 +159,7 @@ def test_col540_runs_are_bit_identical(ctx, monkeypatch):
 @pytest.mark.parametrize("env", [{}, FORCE], ids=["default", "forced"])
 def test_pipeline_pair_on_col540(ctx, monkeypatch, env):
     """A whole pair at a geometry where the default switch picks both Col540 kernels, against the oracle."""
-    _set_env(monkeypatch, env)
+    set_switches(monkeypatch, env)
     shape = (60, 60, 504)   # (z, y, x): padded 80 x 80 x 540, rows of 1008 bytes
     a, b = synth.shifted_pair(shape, (6, -4, 3), seed=91, margin=16)
     dims = shape[::-1]

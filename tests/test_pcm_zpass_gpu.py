@@ -19,6 +19,7 @@ import pytest
 
 from oracle import pcm_oracle as po
 from oracle import pcm_passes as pp
+from tests.pcm_switches import set_switches
 from tests.test_pcm_fft_passes_gpu import BAR, MEASURED, ULP32, UNIT, ZERO, _z_lines
 
 pytestmark = pytest.mark.gpu
@@ -55,8 +56,7 @@ def _dims(kind, sm):
 @pytest.mark.parametrize("kind", ["many", "above", "below"])
 def test_zpass_rotating_buffers(ctx, monkeypatch, kind):
     import torch
-    for k in ("BS_FFT_STATIC", "BS_FFT_ZTILE_LOG2"):
-        monkeypatch.delenv(k, raising=False)
+    set_switches(monkeypatch)
     sm = torch.cuda.get_device_properties(0).multi_processor_count
     dims = _dims(kind, sm)
     n_tiles = _n_tiles(dims)
