@@ -44,6 +44,8 @@ struct bs_pending_event {
     std::string tag;
 };
 
+struct PcmPending;   // pcm.cu: one result slot of the pair pipeline
+
 // Workspace of the phase-correlation pipeline (grown on demand, reused between pairs).
 struct bs_pcm_workspace {
     void* spec_a = nullptr;      // complex64 [Pz][Py][pitch]; also the real PCM (in place)
@@ -55,6 +57,7 @@ struct bs_pcm_workspace {
     void* small = nullptr;       // device scratch for peaks / pearson sums
     size_t small_bytes = 0;
     void* small_host = nullptr;  // pinned mirror
+    PcmPending* slots = nullptr; // the result slots in small / small_host, each with its completion event
     void* sync = nullptr;        // int: hand-off error word, then the per-plane counters of the fused FFT kernels
     size_t sync_bytes = 0;
     cudaEvent_t crop_ready[2] = {nullptr, nullptr};
@@ -102,7 +105,11 @@ struct bs_ctx {
     bool pearson_attr_done = false;   // the same for k_pearson_u16 (set from its first launch)
     size_t pearson_smem = 0;          // dynamic smem of k_pearson_u16's last launch on this context ...
     int pearson_occ = 0;              // ... and its resident CTAs per SM
+    int peak_occ = 0;                 // k_peaks' resident CTAs per SM, at most 8 (set from its first launch)
 };
+
+// bytes per voxel of a BS_DTYPE_*
+static inline size_t bs_out_elem_size(int dt) { return dt == BS_DTYPE_F32 ? 4 : dt == BS_DTYPE_U16 ? 2 : 1; }
 
 int bs_set_error(bs_ctx* ctx, int code, const char* fmt, ...);
 

@@ -134,5 +134,3 @@ static inline bool bs_invert34(const double* m, double* inv) {
     return true;
 }
 
-static inline size_t bs_out_elem_size(int dt) { return dt == BS_DTYPE_F32 ? 4 : dt == BS_DTYPE_U16 ? 2 : 1; }
-

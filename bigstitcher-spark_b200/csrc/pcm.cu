@@ -2108,10 +2108,28 @@ static PcmDeviceTables* tables_of(bs_ctx* ctx) {
     return (PcmDeviceTables*)ctx->ws.tables;
 }
 
-void bs_pcm_slots_free(bs_ctx* ctx);
+// Result slots: a pair's device-side result block (peaks, neighbourhoods, candidates, Pearson sums) is read back by
+// ONE async copy into slot i & 1 of ws.small_host.  pcm_run_pairs, the one pair loop of every batch entry point, runs
+// the host math of pair i (r from integer sums, candidate sort, sub-pixel solve) after pair i+1 has been enqueued, so
+// the stream never drains between pairs.
+#define PCM_SLOTS 2
+struct PcmPending {
+    bool active = false;
+    PcmGeometry g;
+    bs_pcm_params p;
+    int dtype = 0;
+    long long min_px = 0;
+    size_t off_sel = 0, off_cands = 0, off_sums = 0, off_err = 0, slot_base = 0;
+    cudaEvent_t done = nullptr;   // recorded after the slot's read-back
+};
+
 void bs_pcm_workspace_free(bs_ctx* ctx) {
-    bs_pcm_slots_free(ctx);
     bs_pcm_workspace& ws = ctx->ws;
+    if (ws.slots) {
+        for (int i = 0; i < PCM_SLOTS; ++i)
+            if (ws.slots[i].done) cudaEventDestroy(ws.slots[i].done);
+        delete[] ws.slots;
+    }
     if (ws.spec_a) cudaFree(ws.spec_a);
     if (ws.spec_b) cudaFree(ws.spec_b);
     for (int i = 0; i < 2; ++i)
@@ -2327,6 +2345,16 @@ static int pcm_kernel_attrs(bs_ctx* ctx) {
     return BS_OK;
 }
 
+// what every pair needs before its first pass: geometry, tables and workspace for its dims, the kernels' shared-memory
+// opt-in and a cleared hand-off error word
+static int pcm_prepare(bs_ctx* ctx, const long long dims[3], const int ext[3], PcmGeometry* g, PcmDeviceTables** t) {
+    int rc;
+    if ((rc = pcm_geometry(ctx, dims, ext, g)) || (rc = pcm_tables(ctx, *g, t)) || (rc = pcm_workspace(ctx, *g)) ||
+        (rc = pcm_kernel_attrs(ctx)))
+        return rc;
+    return pcm_reset_handoff(ctx);
+}
+
 // The five FFT passes.  Each launches one kernel on ctx->stream and, when `info` is not NULL, writes the
 // instantiation it chose (plus the plan's radices for runtime-planned kernels), e.g.
 // "k_fft_strided_pipe 15x12x3", into info[PCM_INFO_LEN].  bs_pcm_debug_pass runs them one at a time.
@@ -2370,7 +2398,7 @@ static XR2CArgs r2c_args(bs_ctx* ctx, const void* d1, const void* d2, int dtype,
 // k_fft_x_r2c_col540's arguments and dynamic shared memory; false when pass 0 does not take that kernel
 static bool r2c_col540(bs_ctx* ctx, const XR2CArgs& a, int dtype, const PcmGeometry& g, XR2CCol540Args* c,
                        size_t* smem) {
-    const int row_bytes = g.d[0] * (dtype == BS_DTYPE_U16 ? 2 : dtype == BS_DTYPE_F32 ? 4 : 1);
+    const int row_bytes = g.d[0] * (int)bs_out_elem_size(dtype);
     const int col_tiles = (g.P[1] * g.P[2] + COL540_TC - 1) / COL540_TC;
     int raw_stride = (row_bytes + 15) & ~15;   // 16 staged rows on 8 different banks: 4 words times an odd number
     while ((raw_stride / 4) % 8 != 4) raw_stride += 16;
@@ -2392,7 +2420,7 @@ static int pcm_pass_x_r2c(bs_ctx* ctx, const void* d1, const void* d2, int dtype
     dim3 grid((g.P[1] + LB - 1) / LB, g.P[2], 2);
     {
         bs_launch_scope sc(ctx, "fft_x_r2c");
-        const int esize = dtype == BS_DTYPE_U16 ? 2 : dtype == BS_DTYPE_F32 ? 4 : 1;
+        const int esize = (int)bs_out_elem_size(dtype);
         const int row_bytes = g.d[0] * esize;
         const size_t smem_tma = g.smem_x_r2c + 2 * (size_t)LB * row_bytes + 16;
         const bool tma_ok = env_int("BS_FFT_R2C_TMA", 1) != 0 && (row_bytes % 16) == 0 && ((size_t)d1 % 16) == 0 &&
@@ -2647,12 +2675,11 @@ static int pcm_pass_xy(bs_ctx* ctx, const void* d1, const void* d2, int dtype, c
 }
 
 
-// forward pipeline up to the real PCM in ws.spec_a (row pitch 2*pitch floats).  The caller resets the hand-off
-// error word (pcm_reset_handoff) before and checks it once the stream has passed the pair.
+// forward pipeline up to the real PCM in ws.spec_a (row pitch 2*pitch floats).  The caller runs pcm_prepare before
+// and checks the hand-off error word once the stream has passed the pair.
 static int pcm_compute_pcm(bs_ctx* ctx, const void* d1, const void* d2, int dtype, const PcmGeometry& g,
                            PcmDeviceTables* t) {
     int rc;
-    if ((rc = pcm_kernel_attrs(ctx))) return rc;
     if ((rc = pcm_pass_xy(ctx, d1, d2, dtype, g, t, nullptr))) return rc;
     if ((rc = pcm_pass_z_xpower(ctx, g, t, nullptr))) return rc;
     if ((rc = pcm_pass_y_inv(ctx, g, t, nullptr))) return rc;
@@ -2718,51 +2745,21 @@ static double pearson_from_dbl_sums(const double s[5], long long n) {
     return cov / std::sqrt(va * vb);
 }
 
-// full pipeline on device-resident crops
-// Result slots: a pair's device-side result block (peaks, neighbourhoods, candidates, Pearson sums) is read
-// back by ONE async copy; the host math of pair i (r from integer sums, candidate sort, sub-pixel solve) runs
-// after pair i+1 has been enqueued, so the stream never drains between pairs.
-#define PCM_SLOTS 2
-struct PcmPending {
-    bool active = false;
-    PcmGeometry g;
-    bs_pcm_params p;
-    int dtype = 0;
-    long long min_px = 0;
-    size_t off_sel = 0, off_cands = 0, off_sums = 0, off_err = 0, slot_base = 0;
-};
-
-struct PcmSlotState {
-    PcmPending pend[PCM_SLOTS];
-    cudaEvent_t done[PCM_SLOTS] = {};
-};
-static std::mutex g_slot_mu;
-static std::unordered_map<bs_ctx*, PcmSlotState*> g_slot_states;
-static PcmSlotState* slots_of(bs_ctx* ctx) {
-    std::lock_guard<std::mutex> lk(g_slot_mu);
-    auto it = g_slot_states.find(ctx);
-    if (it != g_slot_states.end()) return it->second;
-    PcmSlotState* s = new PcmSlotState();
-    g_slot_states[ctx] = s;
-    return s;
-}
-void bs_pcm_slots_free(bs_ctx* ctx) {
-    std::lock_guard<std::mutex> lk(g_slot_mu);
-    auto it = g_slot_states.find(ctx);
-    if (it == g_slot_states.end()) return;
-    for (int i = 0; i < PCM_SLOTS; ++i)
-        if (it->second->done[i]) cudaEventDestroy(it->second->done[i]);
-    delete it->second;
-    g_slot_states.erase(it);
-}
-
-static int pcm_check_params(bs_ctx* ctx, const bs_pcm_params* p, int dtype) {
-    if (p->peaks_to_check < 1 || p->peaks_to_check > PCM_KMAX)
+// Everything a PCM entry point checks before it allocates, copies or launches anything: the parameters (p is NULL
+// for bs_pcm_debug_pcm, which takes only the extension), the dtype and the geometry of every pair's dims_of(i).
+template <class DimsOf>
+static int pcm_check_params(bs_ctx* ctx, const bs_pcm_params* p, const int ext[3], int dtype, int n, DimsOf dims_of) {
+    if (p && (p->peaks_to_check < 1 || p->peaks_to_check > PCM_KMAX))
         return bs_set_error(ctx, BS_ERR_ARG, "pcm: peaks_to_check must be in [1,%d]", PCM_KMAX);
-    if (p->interpolate_xcorr)
+    if (p && p->interpolate_xcorr)
         return bs_set_error(ctx, BS_ERR_UNSUPPORTED, "pcm: interpolate_xcorr is not supported (reference default false)");
     if (dtype != BS_DTYPE_U16 && dtype != BS_DTYPE_F32 && dtype != BS_DTYPE_U8)
         return bs_set_error(ctx, BS_ERR_ARG, "pcm: bad dtype %d", dtype);
+    for (int i = 0; i < n; ++i) {
+        PcmGeometry g;
+        const int rc = pcm_geometry(ctx, dims_of(i), ext, &g);
+        if (rc) return rc;
+    }
     return BS_OK;
 }
 
@@ -2818,31 +2815,29 @@ static int pearson_launch(bs_ctx* ctx, const void* d1, const void* d2, int dtype
     return BS_OK;
 }
 
-// everything of one pair that runs on the device, asynchronously, into result slot `slot`
+// everything of one pair that runs on the device, asynchronously, into result slot `slot` (p, dtype and dims as
+// pcm_check_params accepted them)
 static int pcm_enqueue(bs_ctx* ctx, const void* d1, const void* d2, const long long dims[3], int dtype,
                        const bs_pcm_params* p, int slot) {
-    int rc = pcm_check_params(ctx, p, dtype);
-    if (rc) return rc;
-    PcmSlotState* S = slots_of(ctx);
-    PcmPending& pd = S->pend[slot];
-    if ((rc = pcm_geometry(ctx, dims, p->extension, &pd.g))) return rc;
-    const PcmGeometry& g = pd.g;
+    bs_pcm_workspace& ws = ctx->ws;
+    if (!ws.slots) ws.slots = new PcmPending[PCM_SLOTS];
+    PcmPending& pd = ws.slots[slot];
     PcmDeviceTables* t;
-    if ((rc = pcm_tables(ctx, g, &t))) return rc;
-    if ((rc = pcm_workspace(ctx, g))) return rc;
-    if ((rc = pcm_reset_handoff(ctx))) return rc;
+    int rc;
+    if ((rc = pcm_prepare(ctx, dims, p->extension, &pd.g, &t))) return rc;
+    const PcmGeometry& g = pd.g;
     if ((rc = pcm_compute_pcm(ctx, d1, d2, dtype, g, t))) return rc;
 
-    bs_pcm_workspace& ws = ctx->ws;
     const int K = p->peaks_to_check;
     // one resident wave of persistent CTAs (the kernel is latency bound: a second, partial wave halves the bytes in flight
     // for the tail of the launch)
-    static int peak_occ = 0;
-    if (!peak_occ) {
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&peak_occ, k_peaks, PCM_THREADS, 0) != cudaSuccess || peak_occ < 1) peak_occ = 4;
-        peak_occ = std::min(peak_occ, env_int("BS_PEAKS_CTAS_PER_SM", 8));
+    if (!ctx->peak_occ) {
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->peak_occ, k_peaks, PCM_THREADS, 0) != cudaSuccess ||
+            ctx->peak_occ < 1)
+            ctx->peak_occ = 4;
+        ctx->peak_occ = std::min(ctx->peak_occ, 8);
     }
-    const int peak_ctas = std::max(1, std::min(ctx->sm_count * peak_occ, (g.P[1] * g.P[2] + 7) / 8));
+    const int peak_ctas = std::max(1, std::min(ctx->sm_count * ctx->peak_occ, (g.P[1] * g.P[2] + 7) / 8));
     // small-buffer layout of one slot (device and pinned mirror share offsets)
     const size_t slot_bytes = ws.small_bytes / PCM_SLOTS;
     pd.slot_base = (size_t)slot * slot_bytes;
@@ -2895,21 +2890,20 @@ static int pcm_enqueue(bs_ctx* ctx, const void* d1, const void* d2, const long l
         return rc;
     BS_CUDA(ctx, cudaMemcpyAsync(hsmall, dsmall, readback, cudaMemcpyDeviceToHost, ctx->stream));
     BS_CUDA(ctx, cudaMemcpyAsync(hsmall + pd.off_err, ws.sync, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    if (!S->done[slot]) BS_CUDA(ctx, cudaEventCreateWithFlags(&S->done[slot], cudaEventDisableTiming));
-    BS_CUDA(ctx, cudaEventRecord(S->done[slot], ctx->stream));
+    if (!pd.done) BS_CUDA(ctx, cudaEventCreateWithFlags(&pd.done, cudaEventDisableTiming));
+    BS_CUDA(ctx, cudaEventRecord(pd.done, ctx->stream));
     pd.active = true;
     return BS_OK;
 }
 
 // host half of a pair: wait for its result block, derive r, sort the candidates, solve the sub-pixel fit
 static int pcm_finish(bs_ctx* ctx, int slot, bs_pcm_result* out) {
-    PcmSlotState* S = slots_of(ctx);
-    PcmPending& pd = S->pend[slot];
+    PcmPending& pd = ctx->ws.slots[slot];
     memset(out, 0, sizeof(*out));
     out->r = -INFINITY;
     if (!pd.active) return bs_set_error(ctx, BS_ERR_ARG, "pcm: no pending pair in slot %d", slot);
     pd.active = false;
-    BS_CUDA(ctx, cudaEventSynchronize(S->done[slot]));
+    BS_CUDA(ctx, cudaEventSynchronize(pd.done));
     const PcmGeometry& g = pd.g;
     for (int d = 0; d < 3; ++d) out->pad[d] = g.P[d];
     const unsigned char* hsmall = (const unsigned char*)ctx->ws.small_host + pd.slot_base;
@@ -2976,8 +2970,7 @@ static int pcm_finish(bs_ctx* ctx, int slot, bs_pcm_result* out) {
 }
 
 static size_t crop_bytes_of(const long long dims[3], int dtype) {
-    const size_t es = dtype == BS_DTYPE_U16 ? 2 : dtype == BS_DTYPE_F32 ? 4 : 1;
-    return (size_t)dims[0] * dims[1] * dims[2] * es;
+    return (size_t)dims[0] * dims[1] * dims[2] * bs_out_elem_size(dtype);
 }
 
 static int ensure_crop_buffers(bs_ctx* ctx, size_t bytes, int nbuf) {
@@ -3000,6 +2993,29 @@ static int ensure_crop_buffers(bs_ctx* ctx, size_t bytes, int nbuf) {
     }
     ws.crop_bytes = nb;
     return BS_OK;
+}
+
+// The pair pipeline of every batch entry point.  Pair i's kernels run into result slot i & 1; the host half of the
+// pending pair i-1 (pcm_finish) runs once pair i is enqueued, unless the dims change: tables and workspace are then
+// rebuilt, so the pending pair is finished first.  ready(i, &d1, &d2) makes pair i's crops ready on ctx->stream; when
+// crop_free is not NULL, crop_free[i & 1] is recorded after pair i's kernels, the last readers of its crops.
+template <class DimsOf, class Ready>
+static int pcm_run_pairs(bs_ctx* ctx, int n, int dtype, const bs_pcm_params* p, bs_pcm_result* out, DimsOf dims_of,
+                         const cudaEvent_t* crop_free, Ready ready) {
+    int pending = -1, rc;
+    for (int i = 0; i < n; ++i) {
+        const void *d1 = nullptr, *d2 = nullptr;
+        if ((rc = ready(i, &d1, &d2))) return rc;
+        if (pending >= 0 && memcmp(dims_of(i), dims_of(pending), 3 * sizeof(long long))) {
+            if ((rc = pcm_finish(ctx, pending & 1, out + pending))) return rc;
+            pending = -1;
+        }
+        if ((rc = pcm_enqueue(ctx, d1, d2, dims_of(i), dtype, p, i & 1))) return rc;
+        if (crop_free) BS_CUDA(ctx, cudaEventRecord(crop_free[i & 1], ctx->stream));
+        if (pending >= 0 && (rc = pcm_finish(ctx, pending & 1, out + pending))) return rc;
+        pending = i;
+    }
+    return pending >= 0 ? pcm_finish(ctx, pending & 1, out + pending) : BS_OK;
 }
 
 extern "C" {
@@ -3029,71 +3045,45 @@ int bs_pcm_batch(bs_ctx* ctx, int n, const void* const* img1, const void* const*
         return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_batch: NULL argument");
     if (n == 0) return BS_OK;
     BS_CUDA(ctx, cudaSetDevice(ctx->device));
-    if (n > 0 && (params->peaks_to_check < 1 || params->peaks_to_check > PCM_KMAX))
-        return bs_set_error(ctx, BS_ERR_ARG, "pcm: peaks_to_check must be in [1,%d]", PCM_KMAX);
-    for (int i = 0; i < n; ++i) {
+    for (int i = 0; i < n; ++i)
         if (!img1[i] || !img2[i]) return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_batch: pair %d has a NULL image", i);
-        for (int d = 0; d < 3; ++d)
-            if (dims[3 * i + d] <= 0) return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_batch: pair %d has dims[%d] <= 0", i, d);
-        // validate every pair's geometry BEFORE any byte is copied or any kernel is launched
-        PcmGeometry g;
-        const int rc = pcm_geometry(ctx, dims + 3 * i, params->extension, &g);
-        if (rc) return rc;
-    }
-    // pair i's host half (result read-back, candidate sort, sub-pixel solve) runs after pair i+1 was enqueued.
-    // A change of geometry rebuilds tables / workspace, so the previous pair is finished first.
-    auto same_dims = [&](int i, int j) {
-        return dims[3 * i] == dims[3 * j] && dims[3 * i + 1] == dims[3 * j + 1] && dims[3 * i + 2] == dims[3 * j + 2];
-    };
+    auto dims_of = [&](int i) { return dims + 3 * i; };
+    int rc = pcm_check_params(ctx, params, params->extension, dtype, n, dims_of);
+    if (rc) return rc;
     if (on_device) {
-        int pending = -1;
-        for (int i = 0; i < n; ++i) {
-            if (pending >= 0 && !same_dims(i, pending)) {
-                int rc = pcm_finish(ctx, pending & 1, out + pending);
-                if (rc) return rc;
-                pending = -1;
-            }
-            int rc = pcm_enqueue(ctx, img1[i], img2[i], dims + 3 * i, dtype, params, i & 1);
-            if (rc) return rc;
-            if (pending >= 0 && (rc = pcm_finish(ctx, pending & 1, out + pending))) return rc;
-            pending = i;
-        }
-        if (pending >= 0) return pcm_finish(ctx, pending & 1, out + pending);
-        return BS_OK;
+        auto ready = [&](int i, const void** d1, const void** d2) {
+            *d1 = img1[i];
+            *d2 = img2[i];
+            return BS_OK;
+        };
+        return pcm_run_pairs(ctx, n, dtype, params, out, dims_of, nullptr, ready);
     }
     // host inputs: double-buffered H2D on the copy stream, overlapped with the previous pair
     size_t maxb = 0;
-    for (int i = 0; i < n; ++i) maxb = std::max(maxb, crop_bytes_of(dims + 3 * i, dtype));
-    int rc = ensure_crop_buffers(ctx, maxb, n > 1 ? 2 : 1);
-    if (rc) return rc;
+    for (int i = 0; i < n; ++i) maxb = std::max(maxb, crop_bytes_of(dims_of(i), dtype));
+    if ((rc = ensure_crop_buffers(ctx, maxb, n > 1 ? 2 : 1))) return rc;
     bs_pcm_workspace& ws = ctx->ws;
     auto enqueue_copy = [&](int i) -> int {
         const int b = i & 1;
-        const size_t bytes = crop_bytes_of(dims + 3 * i, dtype);
+        const size_t bytes = crop_bytes_of(dims_of(i), dtype);
         if (i >= 2) BS_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ws.crop_free[b], 0));
         BS_CUDA(ctx, cudaMemcpyAsync(ws.crop[b][0], img1[i], bytes, cudaMemcpyHostToDevice, ctx->copy_stream));
         BS_CUDA(ctx, cudaMemcpyAsync(ws.crop[b][1], img2[i], bytes, cudaMemcpyHostToDevice, ctx->copy_stream));
         BS_CUDA(ctx, cudaEventRecord(ws.crop_ready[b], ctx->copy_stream));
         return BS_OK;
     };
-    if (n > 0 && (rc = enqueue_copy(0))) return rc;
-    int pending = -1;
-    for (int i = 0; i < n; ++i) {
+    if ((rc = enqueue_copy(0))) return rc;
+    // pair i+1's copy is queued before the host can block on a pending pair
+    auto ready = [&](int i, const void** d1, const void** d2) -> int {
         const int b = i & 1;
+        int rc;
         if (i + 1 < n && (rc = enqueue_copy(i + 1))) return rc;
-        if (pending >= 0 && !same_dims(i, pending)) {
-            if ((rc = pcm_finish(ctx, pending & 1, out + pending))) return rc;
-            pending = -1;
-        }
         BS_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ws.crop_ready[b], 0));
-        rc = pcm_enqueue(ctx, ws.crop[b][0], ws.crop[b][1], dims + 3 * i, dtype, params, b);
-        if (rc) return rc;
-        BS_CUDA(ctx, cudaEventRecord(ws.crop_free[b], ctx->stream));
-        if (pending >= 0 && (rc = pcm_finish(ctx, pending & 1, out + pending))) return rc;
-        pending = i;
-    }
-    if (pending >= 0) return pcm_finish(ctx, pending & 1, out + pending);
-    return BS_OK;
+        *d1 = ws.crop[b][0];
+        *d2 = ws.crop[b][1];
+        return BS_OK;
+    };
+    return pcm_run_pairs(ctx, n, dtype, params, out, dims_of, ws.crop_free, ready);
 }
 
 int bs_pcm_volumes_batch(bs_ctx* ctx, int n, const bs_pcm_job* jobs, const bs_pcm_params* params, bs_pcm_result* out) {
@@ -3119,9 +3109,6 @@ int bs_pcm_volumes_batch(bs_ctx* ctx, int n, const bs_pcm_job* jobs, const bs_pc
                 j.min2[d] + j.dims[d] > i2->second.dims[d])
                 return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_volumes_batch: job %d: overlap interval outside the volume (axis %d)", i, d);
         }
-        PcmGeometry g;
-        int rc = pcm_geometry(ctx, j.dims, params->extension, &g);
-        if (rc) return rc;
         const bool whole1 = j.dims[0] == i1->second.dims[0] && j.dims[1] == i1->second.dims[1] && j.dims[2] == i1->second.dims[2];
         const bool whole2 = j.dims[0] == i2->second.dims[0] && j.dims[1] == i2->second.dims[1] && j.dims[2] == i2->second.dims[2];
         if (!whole1 || !whole2) {
@@ -3129,11 +3116,12 @@ int bs_pcm_volumes_batch(bs_ctx* ctx, int n, const bs_pcm_job* jobs, const bs_pc
             maxb = std::max(maxb, crop_bytes_of(j.dims, dtype));
         }
     }
-    int rc = pcm_check_params(ctx, params, dtype);
+    auto dims_of = [&](int i) { return jobs[i].dims; };
+    int rc = pcm_check_params(ctx, params, params->extension, dtype, n, dims_of);
     if (rc) return rc;
     if (need_crop && (rc = ensure_crop_buffers(ctx, maxb, 2))) return rc;
     bs_pcm_workspace& ws = ctx->ws;
-    const size_t es = dtype == BS_DTYPE_U16 ? 2 : dtype == BS_DTYPE_F32 ? 4 : 1;
+    const size_t es = bs_out_elem_size(dtype);
     // the overlap crop of a volume: the volume itself when the interval covers it, else a strided device copy
     auto crop = [&](bs_volume& v, const long long mn[3], const long long dims[3], void* dst, const void** out_ptr) -> int {
         if (dims[0] == v.dims[0] && dims[1] == v.dims[1] && dims[2] == v.dims[2]) { *out_ptr = v.dev; return BS_OK; }
@@ -3149,30 +3137,18 @@ int bs_pcm_volumes_batch(bs_ctx* ctx, int n, const bs_pcm_job* jobs, const bs_pc
         *out_ptr = dst;
         return BS_OK;
     };
-    auto same_dims = [&](int i, int j) {
-        return jobs[i].dims[0] == jobs[j].dims[0] && jobs[i].dims[1] == jobs[j].dims[1] && jobs[i].dims[2] == jobs[j].dims[2];
-    };
-    int pending = -1;
-    for (int i = 0; i < n; ++i) {
+    auto ready = [&](int i, const void** p1, const void** p2) -> int {
         const bs_pcm_job& j = jobs[i];
         bs_volume& v1 = ctx->vols.find(j.vol1)->second;
         bs_volume& v2 = ctx->vols.find(j.vol2)->second;
-        if ((rc = bs_volume_acquire(ctx, v1)) || (rc = bs_volume_acquire(ctx, v2))) return rc;
-        if (pending >= 0 && !same_dims(i, pending)) {
-            if ((rc = pcm_finish(ctx, pending & 1, out + pending))) return rc;
-            pending = -1;
-        }
         const int b = i & 1;
-        const void *p1 = nullptr, *p2 = nullptr;
+        int rc;
+        if ((rc = bs_volume_acquire(ctx, v1)) || (rc = bs_volume_acquire(ctx, v2))) return rc;
         // crop buffers of slot b were last read by pair i-2's Pearson kernel: same stream, already ordered
-        if ((rc = crop(v1, j.min1, j.dims, need_crop ? ws.crop[b][0] : nullptr, &p1))) return rc;
-        if ((rc = crop(v2, j.min2, j.dims, need_crop ? ws.crop[b][1] : nullptr, &p2))) return rc;
-        if ((rc = pcm_enqueue(ctx, p1, p2, j.dims, dtype, params, b))) return rc;
-        if (pending >= 0 && (rc = pcm_finish(ctx, pending & 1, out + pending))) return rc;
-        pending = i;
-    }
-    if (pending >= 0) return pcm_finish(ctx, pending & 1, out + pending);
-    return BS_OK;
+        if ((rc = crop(v1, j.min1, j.dims, need_crop ? ws.crop[b][0] : nullptr, p1))) return rc;
+        return crop(v2, j.min2, j.dims, need_crop ? ws.crop[b][1] : nullptr, p2);
+    };
+    return pcm_run_pairs(ctx, n, dtype, params, out, dims_of, nullptr, ready);
 }
 
 int bs_pcm_debug_pcm(bs_ctx* ctx, const void* img1, const void* img2, const long long dims[3], int dtype,
@@ -3182,18 +3158,16 @@ int bs_pcm_debug_pcm(bs_ctx* ctx, const void* img1, const void* img2, const long
     if (!img1 || !img2 || !dims || !extension || !out_pcm)
         return bs_set_error(ctx, BS_ERR_ARG, "bs_pcm_debug_pcm: NULL argument");
     BS_CUDA(ctx, cudaSetDevice(ctx->device));
-    PcmGeometry g;
-    int rc = pcm_geometry(ctx, dims, extension, &g);
+    int rc = pcm_check_params(ctx, nullptr, extension, dtype, 1, [&](int) { return dims; });
     if (rc) return rc;
+    PcmGeometry g;
     PcmDeviceTables* t;
-    if ((rc = pcm_tables(ctx, g, &t))) return rc;
-    if ((rc = pcm_workspace(ctx, g))) return rc;
+    if ((rc = pcm_prepare(ctx, dims, extension, &g, &t))) return rc;
     const size_t bytes = crop_bytes_of(dims, dtype);
     if ((rc = ensure_crop_buffers(ctx, bytes, 1))) return rc;
     bs_pcm_workspace& ws = ctx->ws;
     BS_CUDA(ctx, cudaMemcpyAsync(ws.crop[0][0], img1, bytes, cudaMemcpyHostToDevice, ctx->stream));
     BS_CUDA(ctx, cudaMemcpyAsync(ws.crop[0][1], img2, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    if ((rc = pcm_reset_handoff(ctx))) return rc;
     if ((rc = pcm_compute_pcm(ctx, ws.crop[0][0], ws.crop[0][1], dtype, g, t))) return rc;
     BS_CUDA(ctx, cudaMemcpy2DAsync(out_pcm, sizeof(float) * g.P[0], ws.spec_a, sizeof(float2) * g.pitch,
                                    sizeof(float) * g.P[0], (size_t)g.P[1] * g.P[2], cudaMemcpyDeviceToHost, ctx->stream));
@@ -3224,12 +3198,9 @@ int bs_pcm_debug_pass(bs_ctx* ctx, int pass, const long long dims[3], int dtype,
                                 i ? 'b' : 'a');
     }
     PcmGeometry g;
-    int rc = pcm_geometry(ctx, dims, extension, &g);
-    if (rc) return rc;
     PcmDeviceTables* t;
-    if ((rc = pcm_tables(ctx, g, &t))) return rc;
-    if ((rc = pcm_workspace(ctx, g))) return rc;
-    if ((rc = pcm_kernel_attrs(ctx))) return rc;
+    int rc = pcm_prepare(ctx, dims, extension, &g, &t);
+    if (rc) return rc;
     bs_pcm_workspace& ws = ctx->ws;
     const size_t spec_bytes = (size_t)g.P[2] * g.P[1] * g.pitch * sizeof(float2);
     const size_t row = (size_t)(g.M + 1) * sizeof(float2), rows = (size_t)g.P[1] * g.P[2];
@@ -3237,7 +3208,6 @@ int bs_pcm_debug_pass(bs_ctx* ctx, int pass, const long long dims[3], int dtype,
     const void* in[2] = {in_a, in_b};
     void* out[2] = {out_a, out_b};
     for (int i = 0; i < 2; ++i) BS_CUDA(ctx, cudaMemsetAsync(spec[i], poison ? 0xff : 0, spec_bytes, ctx->stream));
-    if ((rc = pcm_reset_handoff(ctx))) return rc;
     if (!crops)
         for (int i = 0; i < (two ? 2 : 1); ++i)
             BS_CUDA(ctx, cudaMemcpy2DAsync(spec[i], sizeof(float2) * g.pitch, in[i], row, row, rows, cudaMemcpyHostToDevice,

@@ -131,15 +131,102 @@ def test_bad_arguments(ctx):
         ctx.pcm_pair(a, a, ctx.pcm_params(peaks_to_check=1000))
 
 
+#: shapes and planted shifts of the mixed-size batches: the dims change from one pair to the next
+MIXED_SPECS = [((40, 48, 56), (2, -1, 3)), ((64, 64, 64), (-3, 4, 1)), ((33, 45, 71), (1, 1, -2)), ((40, 48, 56), (0, 5, -4))]
+
+
+def _mixed_pairs():
+    return [synth.shifted_pair(sh, s, seed=60 + i) for i, (sh, s) in enumerate(MIXED_SPECS)]
+
+
 def test_mixed_size_batch_regrows_workspace(ctx):
     """Pairs of different sizes in one call: workspace, twiddle tables and profiles are rebuilt per size."""
-    specs = [((40, 48, 56), (2, -1, 3)), ((64, 64, 64), (-3, 4, 1)), ((33, 45, 71), (1, 1, -2)), ((40, 48, 56), (0, 5, -4))]
-    pairs = [synth.shifted_pair(sh, s, seed=60 + i) for i, (sh, s) in enumerate(specs)]
+    pairs = _mixed_pairs()
     batch = ctx.pcm_batch([p[0] for p in pairs], [p[1] for p in pairs])
-    for (sh, s), r, (a, b) in zip(specs, batch, pairs):
+    for (sh, s), r, (a, b) in zip(MIXED_SPECS, batch, pairs):
         o = po.pcm_shift(a, b)
         assert r.found and r.shift_int == o.shift_int == s and r.pad == o.pad
         assert np.allclose(r.shift_sub, o.shift_sub, atol=1e-3) and abs(r.r - o.r) < 1e-9
+
+
+def test_mixed_size_batch_device_inputs(ctx):
+    """The same mixed sizes as device-resident crops: each result equals the pair run alone."""
+    import torch
+    pairs = _mixed_pairs()
+    dev = [[torch.from_numpy(x.view(np.int16)).cuda() for x in p] for p in pairs]
+    torch.cuda.synchronize()
+    assert ctx.pcm_batch([d[0] for d in dev], [d[1] for d in dev]) == [ctx.pcm_pair(a, b) for a, b in pairs]
+
+
+def test_mixed_size_volumes_batch(ctx):
+    """pcm_volumes_batch over resident volumes whose overlap dims change twice (A B A); pair B's first crop is cut
+    from a larger volume on the device.  Each result equals the pair run alone."""
+    pairs = _mixed_pairs()
+    pairs = [pairs[0], pairs[1], pairs[3]]
+    a1, b1 = pairs[1]
+    big = np.zeros((a1.shape[0] + 3, a1.shape[1] + 5, a1.shape[2] + 7), a1.dtype)
+    big[1:1 + a1.shape[0], 2:2 + a1.shape[1], 3:3 + a1.shape[2]] = a1
+    vols = [pairs[0], (big, b1), pairs[2]]
+    mins = [((0, 0, 0), (0, 0, 0)), ((3, 2, 1), (0, 0, 0)), ((0, 0, 0), (0, 0, 0))]
+    handles = [(ctx.volume_upload(v1), ctx.volume_upload(v2)) for v1, v2 in vols]
+    jobs = [(h1, h2, m1, m2, a.shape[::-1]) for (h1, h2), (m1, m2), (a, _) in zip(handles, mins, pairs)]
+    try:
+        got = ctx.pcm_volumes_batch(jobs)
+    finally:
+        for h in handles:
+            ctx.volume_free(h[0])
+            ctx.volume_free(h[1])
+    assert got == [ctx.pcm_pair(a, b) for a, b in pairs]
+
+
+def _pcm_via(ctx, entry, a, b, params=None, dtype=None):
+    """Phase correlation of one host pair through one entry point (debug_pcm: the PCM volume); `dtype`, when given,
+    is the code handed to the library as is."""
+    if entry == "host":
+        return ctx.pcm_batch([a], [b], params, dtype=dtype)[0]
+    if entry == "device":
+        import torch
+        ta, tb = (torch.from_numpy(x.view(np.int16)).cuda() for x in (a, b))
+        torch.cuda.synchronize()
+        return ctx.pcm_batch([ta], [tb], params, dtype=dtype)[0]
+    if entry == "volumes":
+        h1, h2 = ctx.volume_upload(a), ctx.volume_upload(b)
+        try:
+            return ctx.pcm_volumes_batch([(h1, h2, (0, 0, 0), (0, 0, 0), a.shape[::-1])], params)[0]
+        finally:
+            ctx.volume_free(h1)
+            ctx.volume_free(h2)
+    return ctx.pcm_debug_pcm(a, b)
+
+
+@pytest.mark.parametrize("entry", ["host", "device", "volumes", "debug_pcm"])
+def test_bad_parameters_rejected_on_every_entry_point(ctx, entry):
+    """interpolate_xcorr, peaks_to_check outside [1, 32] and an unknown dtype code (where the caller passes one) are
+    refused by every PCM entry point, and the context then still returns the right result for a valid pair."""
+    import ctypes as C
+    import bsgpu
+    a, b = synth.shifted_pair((24, 32, 40), (2, -3, 1), seed=110)
+    want = _pcm_via(ctx, entry, a, b)
+    bad = []   # (message, call)
+    if entry == "debug_pcm":   # takes only the extension of the parameters; the wrapper derives the dtype from a
+        _check_pcm_volume(want, a, b)
+        out, pad = np.empty_like(want), (C.c_int * 3)()
+        dims, ext = (C.c_longlong * 3)(*a.shape[::-1]), (C.c_int * 3)(10, 10, 10)
+        bad.append(("dtype", lambda: ctx._check(ctx.lib.bs_pcm_debug_pcm(ctx.h, a.ctypes.data, b.ctypes.data, dims, 99,
+                                                                          ext, out.ctypes.data, pad))))
+    else:
+        assert want.found and want.shift_int == (2, -3, 1)
+        for field, value in (("interpolate_xcorr", 1), ("peaks_to_check", 0), ("peaks_to_check", 33)):
+            p = ctx.pcm_params()
+            setattr(p, field, value)
+            bad.append((field, lambda p=p: _pcm_via(ctx, entry, a, b, params=p)))
+    if entry in ("host", "device"):
+        bad.append(("dtype", lambda: _pcm_via(ctx, entry, a, b, dtype=99)))
+    for msg, call in bad:
+        with pytest.raises(bsgpu.BsError, match=msg):
+            call()
+        got = _pcm_via(ctx, entry, a, b)
+        assert np.array_equal(got, want) if entry == "debug_pcm" else got == want
 
 
 def test_large_single_axis_generic_path(ctx):
