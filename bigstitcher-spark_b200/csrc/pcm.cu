@@ -1074,6 +1074,10 @@ struct XR2CCol540Args {
     int n_tiles;      // ceil(Py * Pz / 16)
 };
 
+// (float)v of a 16-bit sample, exactly: 2^23 + v as a float's bits, minus 2^23.  An integer-to-float conversion runs
+// at a quarter of the FP32 add rate on sm_90, and the x tiles convert 40 samples per thread.
+__device__ __forceinline__ float u16_to_float(unsigned int v) { return __int_as_float(0x4B000000u | v) - 8388608.f; }
+
 // Tiles t, t + stride, ... of the pass.  As the producer of k_fft_xy_col540, a tile's stores wait for the window of
 // the last plane they reach, and the tile's lines are published per plane at the next tile's B1 (the last tile's
 // after a barrier of its own).
@@ -1114,6 +1118,10 @@ __device__ __forceinline__ void x_r2c_col540_tiles(const XR2CCol540Args& P, int 
     cp_async_wait<0>();
     __syncthreads();
     const int c = threadIdx.x % TC;   // this thread's column in both of its stage-1 items and its stage-2 item
+    // Points n1 = 1..18 of every stage-1 item are the padded positions 27..512.  When the crop covers all of them
+    // (ex <= 27 and ex + dx > 512), a line of weight wy = wz = 1 reads them straight from its staged row, without the
+    // table, the product and the zero test; points 0 and 19 and every other line keep the table.
+    const bool mid = a.ex <= 27 && a.ex + a.dx > 18 * 27 + 26;
     auto publish = [&](int tp) {      // thread 0, after a barrier that follows tile tp's stores
         for_planes(tp * TC, min(tp * TC + TC, n_lines), a.Py, [&](int z, int n) { handoff_publish(h, z, n); });
     };
@@ -1124,6 +1132,7 @@ __device__ __forceinline__ void x_r2c_col540_tiles(const XR2CCol540Args& P, int 
         const int zp = L / a.Py, yp = L - zp * a.Py;
         const bool live = L < n_lines && zp < a.Ez && yp < a.Ey;
         const float wy = live ? __ldg(a.w_y + yp) : 0.f, wz = live ? __ldg(a.w_z + zp) : 0.f;
+        const bool unit = wy == 1.f && wz == 1.f;   // implies live
         if (t + stride < P.n_tiles) stage(t + stride, b ^ 1);   // buffer b^1 was read before the last B1
         const unsigned short* ra = reinterpret_cast<const unsigned short*>(raw + ((size_t)b * 2 * TC + c) * P.raw_stride);
         const unsigned short* rb = reinterpret_cast<const unsigned short*>(raw + ((size_t)(b * 2 + 1) * TC + c) * P.raw_stride);
@@ -1133,17 +1142,37 @@ __device__ __forceinline__ void x_r2c_col540_tiles(const XR2CCol540Args& P, int 
         for (int u = 0; u < Col540X::IT1; ++u) {
             if (!Col540X::live1(u)) continue;
             const int n2 = (threadIdx.x + u * COL540X_NT) / TC;
-#pragma unroll
-            for (int n1 = 0; n1 < 20; ++n1) {
+            auto table_point = [&](int n1) {   // the blended mirrored extension through the xw table
                 float2 z = make_float2(0.f, 0.f);
                 if (live) {
                     const int2 e = xw[27 * n1 + n2];
                     const float g = (__int_as_float(e.y) * wy) * wz;
-                    if (g != 0.f) z = make_float2((float)ra[e.x] * g, (float)rb[e.x] * g);
+                    if (g != 0.f) z = make_float2(u16_to_float(ra[e.x]) * g, u16_to_float(rb[e.x]) * g);
                 }
                 nza |= z.x != 0.f;
                 nzb |= z.y != 0.f;
                 v[u][n1] = z;
+            };
+            table_point(0);
+            table_point(19);
+            if (unit && mid) {
+                // the row's samples themselves: there the table holds idx = p - ex and w = 1, and wy = wz = 1, so
+                // the product the table path forms is exactly the sample
+                const unsigned short* pa = ra + n2 - a.ex;
+                const unsigned short* pb = rb + n2 - a.ex;
+                unsigned int sa = 0u, sb = 0u;   // OR of the samples
+#pragma unroll
+                for (int n1 = 1; n1 < 19; ++n1) {
+                    const unsigned int ia = pa[27 * n1], ib = pb[27 * n1];
+                    sa |= ia;
+                    sb |= ib;
+                    v[u][n1] = make_float2(u16_to_float(ia), u16_to_float(ib));
+                }
+                nza |= sa != 0u;
+                nzb |= sb != 0u;
+            } else {
+#pragma unroll
+                for (int n1 = 1; n1 < 19; ++n1) table_point(n1);
             }
         }
         if (nza) nz[(b * 2) * TC + c] = 1;
@@ -2602,10 +2631,10 @@ static int xy_fuse(bs_ctx* ctx, const PcmGeometry& g, const void* fn, size_t sme
     return BS_OK;
 }
 
-// CTAs of k_fft_xy_col540's x role: 80 of 132 measured best (DESIGN.md), scaled to the SM count;
+// CTAs of k_fft_xy_col540's x role: 74 of 132 measured best (DESIGN.md), scaled to the SM count;
 // BS_FFT_XY_KX overrides it
 static int xy_split(bs_ctx* ctx) {
-    return std::max(1, std::min(ctx->sm_count - 1, env_int("BS_FFT_XY_KX", (80 * ctx->sm_count + 66) / 132)));
+    return std::max(1, std::min(ctx->sm_count - 1, env_int("BS_FFT_XY_KX", (74 * ctx->sm_count + 66) / 132)));
 }
 
 // counters in ws.sync; window: as many planes of plane_bytes as fill half of L2 (BS_FFT_XY_WINDOW overrides)
