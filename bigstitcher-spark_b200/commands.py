@@ -10,6 +10,8 @@
   match_interestpoints    J/SparkGeometricDescriptorMatching.java:161-545 (PRECISE_TRANSLATION, correspondences)
   solver                  J/Solver.java:161-432                   (ONE_ROUND_SIMPLE / ONE_ROUND_ITERATIVE, registrations)
   resave                  J/SparkResaveN5.java:80-455             (OME-ZARR or BDV-N5 with the pyramid built on the device)
+  match_intensities       J/SparkIntensityMatching.java:84-190    (pairwise intensity matches, RANSAC on the device)
+  solve_intensities       J/IntensitySolver.java:50-123           (per-view intensity coefficients)
 
 Every command reads its images through viewsource.py, so `bdv.n5` and `bdv.multimg.zarr` datasets both work.
 
@@ -28,6 +30,7 @@ from . import fusion as bf
 from . import n5 as bn5
 from . import zarr as bzarr
 from . import matching as bm
+from . import intensity as bint
 from . import native, solver as bsolver, stitching as bst, viewsource as bvs
 from .native import Context
 from .spimdata import SpimData2
@@ -205,7 +208,8 @@ def _source_window(src_to_world, level_dims, wmin, wmax, margin=3):
 
 def affine_fusion(out_path, ctx: Context, fusion_type="AVG_BLEND", block_scale=(2, 2, 1), channel=None, timepoint=None,
                   retries=5, blocks_per_call=16, interpolation=1, shard=(0, 1), barrier=None, masks=False,
-                  mask_offset=(0.0, 0.0, 0.0), view_selection=None):
+                  mask_offset=(0.0, 0.0, 0.0), view_selection=None, intensity_n5_path=None, intensity_n5_storage=None,
+                  intensity_n5_group="", intensity_n5_dataset="intensity"):
     """`./affine-fusion -o fused.zarr [-f AVG_BLEND] [--blockScale 2,2,1] [-c channelIndex] [-t timepointIndex]
     [--masks [--maskOffset x,y,z]]`:
     read the container metadata and, for every (channel, timepoint) volume (J/SparkAffineFusion.java:425-440), fuse
@@ -225,7 +229,17 @@ def affine_fusion(out_path, ctx: Context, fusion_type="AVG_BLEND", block_scale=(
     covers it; the pyramid is then built from that s0 as usual.
 
     Multi-GPU (SURVEY 8e, "one N5 block-grid slab per device"): rank r of w (``shard``) fuses a contiguous run of
-    z-slabs, no data-path collective; ``barrier()`` separates s0 from the pyramid levels that re-read it."""
+    z-slabs, no data-path collective; ``barrier()`` separates s0 from the pyramid levels that re-read it.
+
+    ``intensity_n5_path`` (`--intensityN5Path`, with `--intensityN5Storage` / `--intensityN5Group` /
+    `--intensityN5Dataset`, J/SparkAffineFusion.java:158-168, 542-559): the coefficients solve-intensities wrote.  Each
+    view's level volume is then staged whole, corrected on the device to float32 (bs_intensity_apply, before the
+    n-linear resampling) and fused from that; content weights come from the corrected volume.  ``masks`` ignores them.
+    A selected view without a coefficient dataset raises ValueError.  None: nothing changes."""
+    coeffs = None
+    if intensity_n5_path is not None and not masks:
+        coeffs = (intensity_n5_path, bint.guess_storage(intensity_n5_path, intensity_n5_storage), intensity_n5_group,
+                  intensity_n5_dataset)
     is_zarr = os.path.exists(os.path.join(out_path, ".zgroup"))
     store, meta = (bzarr.read_fusion_container_zarr if is_zarr else bn5.read_fusion_container)(out_path)
     data = SpimData2.load(meta["input_xml"])
@@ -250,13 +264,14 @@ def affine_fusion(out_path, ctx: Context, fusion_type="AVG_BLEND", block_scale=(
                 continue                                             # nothing selected for this volume
             _fuse_volume_blockwise(ctx, data, src, _Sink(store, is_zarr, ci, ti), meta, levels, vol_views,
                                    fusion_type, interpolation, block_scale, retries, blocks_per_call, shard, barrier,
-                                   masks, mask_offset)
+                                   masks, mask_offset, coeffs)
             written.append(levels[0]["dataset"])
     return written
 
 
 def _fuse_volume_blockwise(ctx, data, src, sink, meta, levels, view_ids, fusion_type, interpolation, block_scale,
-                           retries, blocks_per_call, shard=(0, 1), barrier=None, masks=False, mask_offset=(0.0, 0.0, 0.0)):
+                           retries, blocks_per_call, shard=(0, 1), barrier=None, masks=False, mask_offset=(0.0, 0.0, 0.0),
+                           coeffs=None):
     af = meta["anisotropy_factor"] if meta["preserve_anisotropy"] else float("nan")
     regs = bf.adjust_all_transforms({v: data.model(*v) for v in view_ids}, af)
     bb_min = np.asarray(meta["bb_min"], dtype=np.int64)
@@ -288,6 +303,18 @@ def _fuse_volume_blockwise(ctx, data, src, sink, meta, levels, view_ids, fusion_
     vregs = {v: info[v]["model"] for v in view_ids}
     windowed_ok = (ft in (native.FUSE_AVG, native.FUSE_AVG_BLEND) and interpolation == 1 and
                    all(info[v]["dtype"] == "uint16" and info[v]["dims"][0] % 8 == 0 for v in view_ids))
+    correction = {}
+    if coeffs is not None:
+        # corrected sources are float32 whole-view volumes (the windowed fusion kernel reads uint16 windows only)
+        windowed_ok = False
+        path, storage, group, dataset = coeffs
+        for v in view_ids:
+            c = bint.read_coefficients(path, storage, group, dataset, v)
+            if c is None:
+                raise ValueError(f"no intensity coefficients for view (timepoint {v[0]}, setup {v[1]}) in {path} "
+                                 f"({bint.coefficient_dataset(group, v, dataset)})")
+            factors, mts = src.mipmap_info(v)
+            correction[v] = (c, mts[info[v]["level"]], tuple(int(d) for d in data.setups[v[1]].size))
     content = ft in (native.FUSE_AVG_CONTENT, native.FUSE_AVG_BLEND_CONTENT)
 
     # pyramid straight from the resident fused block when every super-block maps onto whole voxels of every level
@@ -349,6 +376,13 @@ def _fuse_volume_blockwise(ctx, data, src, sink, meta, levels, view_ids, fusion_
                     else:
                         if v not in whole:
                             h = ctx.volume_upload(src.read_volume(v, info[v]["level"]))
+                            if v in correction:
+                                (ca, cb), mt, full = correction[v]
+                                try:
+                                    hc = ctx.intensity_apply(h, full, mt, ca, cb)
+                                finally:
+                                    ctx.volume_free(h)
+                                h = hc
                             whole[v] = (h, ctx.content_weights(h) if content else 0)
                         views[v] = dict(src_to_world=info[v]["model"], vol_handle=whole[v][0], content_handle=whole[v][1],
                                         blend_border=border, blend_range=rng)
@@ -1105,6 +1139,90 @@ def solver(xml_path, ctx: Context, source, labels=None, label_weights=None, meth
 
 # --------------------------------------------------------------------------------------------- resave
 RESAVE_COMPRESSION = {"zstd": "zstd", "zstandard": "zstd", "gzip": "gzip", "raw": "raw"}
+
+
+# --------------------------------------------------------------------------------------------- intensity correction
+def match_intensities(xml_path, ctx: Context, out_path, num_coefficients=(8, 8, 8), render_scale=0.25, min_threshold=1.0,
+                      max_threshold=float("nan"), min_num_candidates=1000, method="RANSAC", num_iterations=1000,
+                      max_epsilon=5.1, min_inlier_ratio=0.1, min_num_inliers=10, max_trust=3.0, view_selection=None,
+                      dry_run=False, chunk_points=0):
+    """`./match-intensities -x dataset.xml -o matches.n5 [--numCoefficients 8,8,8] [--renderScale 0.25] ...`
+    (J/SparkIntensityMatching.java:84-190): for every selected pair i < j whose transformed bounds intersect (across
+    timepoints), render the intersection at ``render_scale`` on the device, bucket the overlapping intensities by
+    (cell of A, cell of B), run RANSAC on the device and the filter on the host, and write coefficientsSize plus the
+    accepted inliers per (pair, cellA, cellB) under ``out_path`` (intensity.MatchesIO).  Returns
+    {(viewA, viewB): [(cellA, cellB, inliers)]}.  ``dry_run`` computes the matches and writes nothing."""
+    if str(method).upper() == "HISTOGRAM":
+        raise NotImplementedError("match-intensities --method HISTOGRAM")
+    if str(method).upper() != "RANSAC":
+        raise ValueError(f"unknown method {method!r}")
+    data = SpimData2.load(xml_path)
+    src = bvs.open_views(data)
+    views = data.select_views(**view_selection) if view_selection else data.view_ids()
+    n_cells = tuple(int(v) for v in num_coefficients)
+    regs = {v: data.model(*v) for v in views}
+    dims = {v: tuple(int(d) for d in data.setups[v[1]].size) for v in views}
+    bounds = {v: bint.view_bounds(dims[v], regs[v]) for v in views}
+    todo = bint.pairs(views, bounds)
+    io = None
+    if not dry_run:
+        io = bint.MatchesIO(out_path, create=True)
+        io.write_coefficients_size(n_cells)
+    levels = {}
+    for v in views:
+        factors, mts = src.mipmap_info(v)
+        lvl = bint.render_level(regs[v], render_scale, factors, mts)
+        levels[v] = (lvl, mts[lvl])
+    resident = {}
+    out = {}
+    try:
+        for a, b in todo:
+            for v in (a, b):
+                if v not in resident:
+                    resident[v] = ctx.volume_upload(src.read_volume(v, levels[v][0]))
+            lo = np.maximum(bounds[a][0], bounds[b][0])
+            hi = np.minimum(bounds[a][1], bounds[b][1])
+            rmin, rmax = bint.render_range(lo, hi, render_scale)
+            va = bint.device_view(resident[a], regs[a], levels[a][1], dims[a], n_cells)
+            vb = bint.device_view(resident[b], regs[b], levels[b][1], dims[b], n_cells)
+            cells, _ = bint.match_pair(ctx, va, vb, render_scale, rmin, rmax, min_threshold, max_threshold,
+                                       min_num_candidates, num_iterations, max_epsilon, min_inlier_ratio,
+                                       min_num_inliers, max_trust, chunk_points)
+            out[(a, b)] = cells
+            if io is not None:
+                io.write(a, b, cells)
+            # a view's volume stays resident until its last pair
+            for v in (a, b):
+                if not any(v in p for p in todo[todo.index((a, b)) + 1:]):
+                    ctx.volume_free(resident.pop(v))
+    finally:
+        for h in resident.values():
+            ctx.volume_free(h)
+    return out
+
+
+def solve_intensities(xml_path, out_path, matches_path, num_coefficients=(8, 8, 8), max_iterations=1000, storage=None,
+                      group="", dataset="intensity", view_selection=None):
+    """`./solve-intensities -x dataset.xml --matchesPath matches.n5 -o coefficients.n5 [-s N5|ZARR]
+    [--intensityN5Group ""] [--intensityN5Dataset intensity]` (J/IntensitySolver.java:50-123): read the pairwise
+    matches of every selected pair, solve one 1-D model per (view, cell) on the host (intensity.solve) and write each
+    view's coefficients to `{group}/setup{s}/timepoint{t}/{dataset}`.  A ``num_coefficients`` that differs from the one
+    stored with the matches warns and the stored one is used.  Returns {view: (a, b)}."""
+    storage = bint.guess_storage(out_path, storage)
+    data = SpimData2.load(xml_path)
+    views = data.select_views(**view_selection) if view_selection else data.view_ids()
+    io = bint.MatchesIO(matches_path)
+    stored = io.read_coefficients_size()
+    bint.check_coefficients_size(stored, num_coefficients)
+    matches = {}
+    for i, a in enumerate(views):
+        for b in views[i + 1:]:
+            m = io.read(a, b)
+            if m is not None:
+                matches[(a, b)] = m
+    coeffs = bint.solve(views, stored, matches, max_iterations)
+    bint.write_coefficients(out_path, storage, group, dataset, coeffs)
+    return coeffs
 
 
 def propose_mipmaps(size_xyz, voxel_size_xyz=(1.0, 1.0, 1.0)):

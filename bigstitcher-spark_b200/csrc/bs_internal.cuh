@@ -96,6 +96,7 @@ struct bs_ctx {
     void* dog = nullptr;              // dog.cu workspace (region buffers, detection list)
     void* nonrigid = nullptr;         // nonrigid.cu workspace (view table, points, control-point grids)
     void* match = nullptr;            // match.cu workspace (resident descriptor sets, per-split match results)
+    void* intensity = nullptr;        // intensity.cu workspace (resident pair candidates)
     void* nccl_comm = nullptr;        // comm.cu: ncclComm_t of the view-sharded exchange (bs_comm_init)
     int nccl_ranks = 0;
     // recycled device buffers of async-uploaded volumes, keyed by byte size
@@ -162,6 +163,8 @@ void bs_dog_free(bs_ctx* ctx);
 void bs_nonrigid_free(bs_ctx* ctx);
 // match.cu
 void bs_match_free(bs_ctx* ctx);
+// intensity.cu
+void bs_intensity_free(bs_ctx* ctx);
 // comm.cu
 void bs_comm_free(bs_ctx* ctx);
 // fuse.cu: generic tile kernel for one block into a device buffer (ctx->mu held by the caller)

@@ -84,6 +84,16 @@ class SolveStatsC(C.Structure):
 SOLVE_MODELS = {"NONE": -1, "IDENTITY": 0, "TRANSLATION": 1, "RIGID": 2, "AFFINE": 3}
 
 
+class IntensityViewC(C.Structure):
+    _fields_ = [("vol_handle", C.c_ulonglong), ("world_to_px", C.c_double * 12), ("px_to_level", C.c_double * 12),
+                ("full_dims", C.c_longlong * 3), ("n_cells", C.c_int * 3), ("pad", C.c_int)]
+
+
+class IntensityParamsC(C.Structure):
+    _fields_ = [("render_scale", C.c_double), ("min_threshold", C.c_double), ("max_threshold", C.c_double),
+                ("render_min", C.c_longlong * 3), ("render_max", C.c_longlong * 3), ("chunk_points", C.c_longlong)]
+
+
 class PcmJobC(C.Structure):
     _fields_ = [("vol1", C.c_ulonglong), ("vol2", C.c_ulonglong), ("min1", C.c_longlong * 3),
                 ("min2", C.c_longlong * 3), ("dims", C.c_longlong * 3)]
@@ -130,6 +140,8 @@ SYMBOLS = [
     "bs_downsample_float", "bs_median_divide", "bs_sample_nlinear", "bs_nonrigid_fuse_blocks", "bs_nonrigid_debug_grid",
     "bs_descriptors_build", "bs_descriptors_free", "bs_descriptors_neighbors", "bs_descriptors_match",
     "bs_solve_tiles",
+    "bs_intensity_pair_candidates", "bs_intensity_candidates_get", "bs_intensity_candidates_free", "bs_intensity_ransac",
+    "bs_intensity_apply",
 ]
 
 #: fixed parameters of the reference's non-rigid fusion (J/SparkNonRigidFusion.java:373-383): control-point distance
@@ -213,6 +225,12 @@ def load_library():
     lib.bs_descriptors_match.argtypes = [vp, ull, ull, dbl, P(ip), P(dbl), P(dbl)]
     lib.bs_solve_tiles.argtypes = [vp, ip, ip, P(ip), P(ip), P(ip), ip, P(ip), P(ll), P(dbl), P(dbl), P(dbl),
                                    P(SolveParamsC), P(dbl), P(SolveStatsC), P(dbl), P(dbl), P(dbl)]
+    lib.bs_intensity_pair_candidates.argtypes = [vp, P(IntensityViewC), P(IntensityViewC), P(IntensityParamsC), P(ull),
+                                                 P(ll), P(ll)]
+    lib.bs_intensity_candidates_get.argtypes = [vp, ull, P(ll), P(ll), P(ll), vp]
+    lib.bs_intensity_candidates_free.argtypes = [vp, ull]
+    lib.bs_intensity_ransac.argtypes = [vp, ull, ll, ip, dbl, P(dbl), P(dbl), P(ip)]
+    lib.bs_intensity_apply.argtypes = [vp, ull, P(ll), P(ll), P(dbl), P(ip), P(dbl), P(dbl), P(ull)]
     _lib = lib
     return lib
 
@@ -793,6 +811,68 @@ class Context:
         stats = dict(iterations=st.iterations, error=st.error, skipped_fits=st.skipped_fits, stopped=bool(st.stopped),
                      blocks=st.blocks, models_in_shared=bool(st.models_in_shared))
         return M, stats, te, lm[:L], lx[:L]
+
+    # -- intensity correction
+    @staticmethod
+    def _intensity_view(v):
+        c = IntensityViewC()
+        c.vol_handle = int(v["vol_handle"])
+        c.world_to_px[:] = [float(x) for x in np.asarray(v["world_to_px"], dtype=np.float64).ravel()]
+        c.px_to_level[:] = [float(x) for x in np.asarray(v["px_to_level"], dtype=np.float64).ravel()]
+        c.full_dims[:] = [int(x) for x in v["full_dims"]]
+        c.n_cells[:] = [int(x) for x in v["n_cells"]]
+        return c
+
+    def intensity_candidates(self, view_a, view_b, render_scale, render_min, render_max, min_threshold=1.0,
+                             max_threshold=float("nan"), chunk_points=0):
+        """Candidates of one view pair (include/bsgpu.h bs_intensity_pair_candidates), kept resident.  ``view_a`` /
+        ``view_b``: dicts(vol_handle, world_to_px (3, 4), px_to_level (3, 4), full_dims, n_cells).  Returns
+        (handle, keys int64, offsets int64, counts int64, values float32 (n, 2)); free the handle with
+        intensity_candidates_free."""
+        a, b = self._intensity_view(view_a), self._intensity_view(view_b)
+        p = IntensityParamsC(float(render_scale), float(min_threshold), float(max_threshold),
+                             (C.c_longlong * 3)(*[int(v) for v in render_min]),
+                             (C.c_longlong * 3)(*[int(v) for v in render_max]), int(chunk_points))
+        h, nb, nv = C.c_ulonglong(), C.c_longlong(), C.c_longlong()
+        self._check(self.lib.bs_intensity_pair_candidates(self.h, C.byref(a), C.byref(b), C.byref(p), C.byref(h),
+                                                          C.byref(nb), C.byref(nv)))
+        keys, off, cnt = (np.empty(max(nb.value, 1), dtype=np.int64) for _ in range(3))
+        vals = np.empty((max(nv.value, 1), 2), dtype=np.float32)
+        LL = C.POINTER(C.c_longlong)
+        self._check(self.lib.bs_intensity_candidates_get(self.h, h.value, keys.ctypes.data_as(LL), off.ctypes.data_as(LL),
+                                                         cnt.ctypes.data_as(LL), vals.ctypes.data))
+        return h.value, keys[:nb.value], off[:nb.value], cnt[:nb.value], vals[:nv.value]
+
+    def intensity_candidates_free(self, handle: int):
+        self._check(self.lib.bs_intensity_candidates_free(self.h, handle))
+
+    def intensity_ransac(self, handle: int, n_buckets: int, min_num_candidates=1000, num_iterations=1000, max_epsilon=5.1):
+        """Best RANSAC hypothesis per bucket of a resident candidate set: (a, b, count) arrays; count -1 for buckets
+        below ``min_num_candidates``."""
+        n = max(int(n_buckets), 1)
+        a, b, cnt = np.empty(n), np.empty(n), np.empty(n, dtype=np.int32)
+        D = C.POINTER(C.c_double)
+        self._check(self.lib.bs_intensity_ransac(self.h, handle, int(min_num_candidates), int(num_iterations),
+                                                 float(max_epsilon), a.ctypes.data_as(D), b.ctypes.data_as(D),
+                                                 cnt.ctypes.data_as(C.POINTER(C.c_int))))
+        return a[:n_buckets], b[:n_buckets], cnt[:n_buckets]
+
+    def intensity_apply(self, handle: int, full_dims_xyz, level_to_full, coeff_a, coeff_b, window_min_xyz=(0, 0, 0)) -> int:
+        """New float32 volume a(q) v + b(q) of a resident (window of a) level volume; ``coeff_a`` / ``coeff_b``:
+        cell values [nz, ny, nx]."""
+        ca = np.ascontiguousarray(coeff_a, dtype=np.float64)
+        cb = np.ascontiguousarray(coeff_b, dtype=np.float64)
+        if ca.ndim != 3 or ca.shape != cb.shape:
+            raise ValueError("coefficients must be two [nz, ny, nx] arrays of one shape")
+        fd = (C.c_longlong * 3)(*[int(v) for v in full_dims_xyz])
+        wm = (C.c_longlong * 3)(*[int(v) for v in window_min_xyz])
+        m = (C.c_double * 12)(*[float(x) for x in np.asarray(level_to_full, dtype=np.float64).ravel()])
+        n = (C.c_int * 3)(*ca.shape[::-1])
+        h = C.c_ulonglong()
+        D = C.POINTER(C.c_double)
+        self._check(self.lib.bs_intensity_apply(self.h, handle, fd, wm, m, n, ca.ctypes.data_as(D), cb.ctypes.data_as(D),
+                                                C.byref(h)))
+        return h.value
 
     @staticmethod
     def comm_unique_id() -> bytes:

@@ -442,6 +442,66 @@ int bs_solve_tiles(bs_ctx* ctx, int n_tiles, int n_colours, const int* colour_of
                    const double* q, const double* w, const bs_solve_params* params, double* models,
                    bs_solve_stats* stats, double* tile_error, double* link_mean, double* link_max);
 
+/* ---------------------------------------------------------------- intensity correction
+ * match-intensities (IntensityCorrection.matchRansac, J/SparkIntensityMatching.java:166-183) and the coefficient
+ * application of affine-fusion --intensityN5Path (J/SparkAffineFusion.java:602-615).  Additive: the ABI version stays
+ * 107 (the existing structs and functions are unchanged).  Profile tags "intensity_render", "intensity_ransac",
+ * "intensity_apply". */
+typedef struct {
+    unsigned long long vol_handle;   /* resident WHOLE level volume of the view (U16 / F32 / U8) */
+    double    world_to_px[12];       /* row-packed 3x4: world -> full-resolution pixel (inverse registration) */
+    double    px_to_level[12];       /* full-resolution pixel -> pixel of the level volume (inverse mipmap transform) */
+    long long full_dims[3];          /* full-resolution view size */
+    int       n_cells[3];            /* --numCoefficients */
+    int       pad;
+} bs_intensity_view;
+
+typedef struct {
+    double    render_scale;          /* --renderScale s */
+    double    min_threshold;         /* --minThreshold */
+    double    max_threshold;         /* --maxThreshold, NaN: none */
+    long long render_min[3];         /* render grid: integers r with render_min <= r <= render_max, world r / s */
+    long long render_max[3];
+    long long chunk_points;          /* render points per z-chunk, 0: the library default (the output does not depend on it) */
+} bs_intensity_params;
+
+/* Candidates of one view pair, kept resident under *handle (free with bs_intensity_candidates_free).  Per render point,
+ * in FP64 with __dmul_rn / __dadd_rn / __ddiv_rn: w = r / s per axis; p = world_to_px . (w, 1) per row as
+ * ((m0 wx + m1 wy) + m2 wz) + m3; the point is kept when every p_d of both views is in [0, full_dims_d - 1]; level
+ * coordinates q = px_to_level . (p, 1) (same order), rounded to float32; value = n-linear float32 sample at q with
+ * border extension on both sides (the arithmetic of sample() in csrc/fuse_common.cuh, taps clamped to the volume);
+ * kept when both values are >= min_threshold and, unless NaN, <= max_threshold; cell_d = clamp(floor(p_d n_d /
+ * full_dims_d), 0, n_d - 1), flattened x-fastest; key = cellA * cells(B) + cellB.  Buckets are in ascending key order,
+ * values (v_A, v_B) float32 pairs grouped by bucket and in ascending render index (x-fastest) within one.  No order
+ * depends on atomics; the output is the same for every chunk_points. */
+int bs_intensity_pair_candidates(bs_ctx* ctx, const bs_intensity_view* view_a, const bs_intensity_view* view_b,
+                                 const bs_intensity_params* params, unsigned long long* handle, long long* n_buckets,
+                                 long long* n_values);
+/* host copies: keys / offsets / counts [n_buckets] (offsets into values, in pairs), values [2 n_values]; any may be NULL */
+int bs_intensity_candidates_get(bs_ctx* ctx, unsigned long long handle, long long* keys, long long* offsets,
+                                long long* counts, float* values);
+int bs_intensity_candidates_free(bs_ctx* ctx, unsigned long long handle);
+
+/* RANSAC hypotheses (the sampling loop of mpicbg Model.ransac behind IntensityCorrection.matchRansac) of every bucket
+ * with at least max(2, min_num_candidates) candidates: hypothesis h = 0 .. num_iterations - 1 draws candidates
+ * i = splitmix64(SEED ^ (key << 32) ^ 2h) mod n, j = splitmix64(SEED ^ (key << 32) ^ (2h + 1)) mod (n - 1), j += (j >= i),
+ * SEED = 0x2545F4914F6CDD1D, and is skipped when x_i == x_j; its model a = (y_j - y_i) / (x_j - x_i),
+ * b = y_i - a x_i counts the inliers |(a x + b) - y| < max_epsilon (FP64, those operations in that order).  Per bucket:
+ * the hypothesis with the most inliers, the lower h on a tie, as (a, b, count); count 0 and a = b = NaN when every
+ * hypothesis was skipped; count -1 for buckets below the threshold.  Outputs have n_buckets entries. */
+int bs_intensity_ransac(bs_ctx* ctx, unsigned long long handle, long long min_num_candidates, int num_iterations,
+                        double max_epsilon, double* a, double* b, int* count);
+
+/* v' = a(q) v + b(q) on a resident volume (U16 / F32 / U8) -> new F32 volume handle.  The volume is the window
+ * [window_min, window_min + dims) (window_min NULL: zeros) of the level of a view of full-resolution size full_dims;
+ * level_to_full is the mipmap transform.  In float32 (inputs rounded to float): l = window_min + voxel;
+ * q_d = ((m0 l_x + m1 l_y) + m2 l_z) + m3; u_d = clamp((q_d + 0.5) (n_d / full_dims_d) - 0.5, 0, n_d - 1) (cell
+ * centres at (c + 0.5) full_dims / n - 0.5); a and b are the n-linear interpolation of the cell values coeff_a /
+ * coeff_b (x-fastest, n cells) at u, in the lerp order of sample(); v' = (a v) + b. */
+int bs_intensity_apply(bs_ctx* ctx, unsigned long long vol_handle, const long long full_dims[3], const long long window_min[3],
+                       const double level_to_full[12], const int n_cells[3], const double* coeff_a, const double* coeff_b,
+                       unsigned long long* out_handle);
+
 #ifdef __cplusplus
 }
 #endif

@@ -713,3 +713,103 @@ JF(jdoubleArray, solveTiles)(JNIEnv* env, jclass, jlong ctx, jintArray colourOff
     env->SetDoubleArrayRegion(r, 0, 4, out);
     return r;
 }
+
+// ------------------------------------------------------------------------------------------------- intensity correction
+// match-intensities (IntensityCorrection.matchRansac, J/SparkIntensityMatching.java:166-183).  A view is
+// {volHandle, worldToPx double[12], pxToLevel double[12], fullDims long[3], nCells int[3]}; params =
+// {renderScale, minThreshold, maxThreshold}, render long[6] = {min xyz, max xyz}.  Returns the resident candidate
+// handle; sizes (long[2]) receives {nBuckets, nValues}.
+static bs_intensity_view intensity_view(JNIEnv* env, jlong handle, jdoubleArray worldToPx, jdoubleArray pxToLevel,
+                                        jlongArray fullDims, jintArray nCells) {
+    bs_intensity_view v;
+    memset(&v, 0, sizeof(v));
+    v.vol_handle = (unsigned long long)handle;
+    env->GetDoubleArrayRegion(worldToPx, 0, 12, v.world_to_px);
+    env->GetDoubleArrayRegion(pxToLevel, 0, 12, v.px_to_level);
+    get3(env, fullDims, v.full_dims);
+    jint n[3];
+    env->GetIntArrayRegion(nCells, 0, 3, n);
+    for (int k = 0; k < 3; ++k) v.n_cells[k] = n[k];
+    return v;
+}
+
+JF(jlong, intensityPairCandidates)(JNIEnv* env, jclass, jlong ctx, jlong volA, jdoubleArray worldToPxA, jdoubleArray pxToLevelA,
+                                   jlongArray fullDimsA, jintArray nCellsA, jlong volB, jdoubleArray worldToPxB,
+                                   jdoubleArray pxToLevelB, jlongArray fullDimsB, jintArray nCellsB, jdoubleArray params,
+                                   jlongArray render, jlongArray sizes) {
+    const bs_intensity_view a = intensity_view(env, volA, worldToPxA, pxToLevelA, fullDimsA, nCellsA);
+    const bs_intensity_view b = intensity_view(env, volB, worldToPxB, pxToLevelB, fullDimsB, nCellsB);
+    jdouble d[3];
+    env->GetDoubleArrayRegion(params, 0, 3, d);
+    jlong r[6];
+    env->GetLongArrayRegion(render, 0, 6, r);
+    bs_intensity_params p;
+    memset(&p, 0, sizeof(p));
+    p.render_scale = d[0]; p.min_threshold = d[1]; p.max_threshold = d[2];
+    for (int k = 0; k < 3; ++k) {
+        p.render_min[k] = r[k];
+        p.render_max[k] = r[3 + k];
+    }
+    unsigned long long h = 0;
+    long long nb = 0, nv = 0;
+    if (failed(env, ctx, bs_intensity_pair_candidates(C(ctx), &a, &b, &p, &h, &nb, &nv))) return 0;
+    const jlong s[2] = {nb, nv};
+    env->SetLongArrayRegion(sizes, 0, 2, s);
+    return (jlong)h;
+}
+
+// keys / offsets / counts long[nBuckets], values double[2 * nValues] ({vA, vB} per candidate, exact float32 values)
+JF(void, intensityCandidatesGet)(JNIEnv* env, jclass, jlong ctx, jlong handle, jlongArray keys, jlongArray offsets,
+                                 jlongArray counts, jdoubleArray values) {
+    const jsize nb = env->GetArrayLength(keys), nv = env->GetArrayLength(values);
+    std::vector<long long> k((size_t)nb), o((size_t)nb), c((size_t)nb);
+    std::vector<float> v((size_t)nv);
+    if (failed(env, ctx, bs_intensity_candidates_get(C(ctx), (unsigned long long)handle, k.data(), o.data(), c.data(), v.data())))
+        return;
+    const std::vector<jlong> kl(k.begin(), k.end()), ol(o.begin(), o.end()), cl(c.begin(), c.end());
+    env->SetLongArrayRegion(keys, 0, nb, kl.data());
+    env->SetLongArrayRegion(offsets, 0, nb, ol.data());
+    env->SetLongArrayRegion(counts, 0, nb, cl.data());
+    const std::vector<jdouble> vd(v.begin(), v.end());
+    env->SetDoubleArrayRegion(values, 0, nv, vd.data());
+}
+
+JF(void, intensityCandidatesFree)(JNIEnv* env, jclass, jlong ctx, jlong handle) {
+    failed(env, ctx, bs_intensity_candidates_free(C(ctx), (unsigned long long)handle));
+}
+
+// per bucket: a / b double[nBuckets], count long[nBuckets] (-1: below minNumCandidates)
+JF(void, intensityRansac)(JNIEnv* env, jclass, jlong ctx, jlong handle, jlong minNumCandidates, jint numIterations,
+                          jdouble maxEpsilon, jdoubleArray a, jdoubleArray b, jlongArray count) {
+    const jsize n = env->GetArrayLength(count);
+    std::vector<jdouble> av((size_t)n), bv((size_t)n);
+    std::vector<int> cv((size_t)n);
+    if (failed(env, ctx, bs_intensity_ransac(C(ctx), (unsigned long long)handle, minNumCandidates, numIterations, maxEpsilon,
+                                             av.data(), bv.data(), cv.data())))
+        return;
+    const std::vector<jlong> cl(cv.begin(), cv.end());
+    env->SetDoubleArrayRegion(a, 0, n, av.data());
+    env->SetDoubleArrayRegion(b, 0, n, bv.data());
+    env->SetLongArrayRegion(count, 0, n, cl.data());
+}
+
+// affine-fusion --intensityN5Path (J/SparkAffineFusion.java:602-615): a new float32 volume a(q) v + b(q); coefficients
+// a / b double[nx * ny * nz] x-fastest
+JF(jlong, intensityApply)(JNIEnv* env, jclass, jlong ctx, jlong handle, jlongArray fullDims, jlongArray windowMin,
+                          jdoubleArray levelToFull, jintArray nCells, jdoubleArray coeffA, jdoubleArray coeffB) {
+    long long fd[3], wm[3];
+    get3(env, fullDims, fd);
+    get3(env, windowMin, wm);
+    jdouble m[12];
+    env->GetDoubleArrayRegion(levelToFull, 0, 12, m);
+    jint nj[3];
+    env->GetIntArrayRegion(nCells, 0, 3, nj);
+    const int n[3] = {nj[0], nj[1], nj[2]};
+    const jsize nc = env->GetArrayLength(coeffA);
+    std::vector<jdouble> ca((size_t)nc), cb((size_t)nc);
+    env->GetDoubleArrayRegion(coeffA, 0, nc, ca.data());
+    env->GetDoubleArrayRegion(coeffB, 0, nc, cb.data());
+    unsigned long long h = 0;
+    return failed(env, ctx, bs_intensity_apply(C(ctx), (unsigned long long)handle, fd, wm, m, n, ca.data(), cb.data(), &h))
+               ? 0 : (jlong)h;
+}

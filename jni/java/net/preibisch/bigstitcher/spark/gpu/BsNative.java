@@ -121,4 +121,21 @@ public final class BsNative
 	public static native double[] solveTiles( long ctx, int[] colourOffsets, int[] colourTiles, int[] fixed, int[] links,
 			long[] matchOffsets, double[] p, double[] q, double[] w, int[] iparams, double[] dparams, double[] models,
 			double[] tileError, double[] linkMean, double[] linkMax );
+
+	/** match-intensities (replaces the rendering and RANSAC sampling of IntensityCorrection.matchRansac): the candidates of
+	 *  one view pair, kept resident.  A view: level volume handle, world -> full pixel and full pixel -> level transforms
+	 *  (double[12]), full dims, cells per axis; params = {renderScale, minThreshold, maxThreshold}, render = {min xyz, max xyz};
+	 *  sizes receives {nBuckets, nValues}; returns the candidate handle */
+	public static native long intensityPairCandidates( long ctx, long volA, double[] worldToPxA, double[] pxToLevelA, long[] fullDimsA,
+			int[] nCellsA, long volB, double[] worldToPxB, double[] pxToLevelB, long[] fullDimsB, int[] nCellsB, double[] params,
+			long[] render, long[] sizes );
+	/** bucket keys / offsets / counts (long[nBuckets]) and the {vA, vB} values (double[2 * nValues], exact float32 values) */
+	public static native void intensityCandidatesGet( long ctx, long handle, long[] keys, long[] offsets, long[] counts, double[] values );
+	public static native void intensityCandidatesFree( long ctx, long handle );
+	/** best RANSAC hypothesis per bucket (a, b, inlier count; count -1 below minNumCandidates) */
+	public static native void intensityRansac( long ctx, long handle, long minNumCandidates, int numIterations, double maxEpsilon,
+			double[] a, double[] b, long[] count );
+	/** affine-fusion --intensityN5Path: a new float32 volume a(q) v + b(q) of a (windowed) level volume */
+	public static native long intensityApply( long ctx, long handle, long[] fullDims, long[] windowMin, double[] levelToFull,
+			int[] nCells, double[] coeffA, double[] coeffB );
 }
