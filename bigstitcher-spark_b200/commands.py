@@ -3,7 +3,7 @@
 `native.Context` (BASELINE north_star), SpimData2 XML in, N5 / OME-Zarr blocks out.
 
   stitching               J/SparkPairwiseStitching.java:110-392
-  create_fusion_container J/CreateFusionContainer.java:122-519   (N5 or OME-ZARR, all channels / timepoints, pyramid)
+  create_fusion_container J/CreateFusionContainer.java:122-519   (N5 or OME-ZARR, named boxes, BDV projects, pyramid)
   affine_fusion           J/SparkAffineFusion.java:179-800       (s0 + multi-resolution pyramid)
   nonrigid_fusion         J/SparkNonRigidFusion.java:124-446     (MLS grids from interest-point correspondences)
   detect_interestpoints   J/SparkInterestPointDetection.java:173-964 (block-wise DoG, interestpoints.n5 + the XML)
@@ -33,7 +33,7 @@ from . import matching as bm
 from . import intensity as bint
 from . import native, solver as bsolver, stitching as bst, viewsource as bvs
 from .native import Context
-from .spimdata import SpimData2
+from .spimdata import SpimData2, fusion_project
 
 
 def stitching(xml_path, ctx: Context, downsampling=(2, 2, 1), peaks_to_check=5, disable_subpixel=False,
@@ -102,22 +102,51 @@ def estimate_multires_pyramid(dims_xyz, anisotropy_factor=float("nan"), min_size
 
 def create_fusion_container(xml_path, out_path, block_size=(128, 128, 128), dtype="float32", min_intensity=None,
                             max_intensity=None, preserve_anisotropy=False, anisotropy_factor=float("nan"),
-                            storage=None, downsamplings=(), multi_res=False, compression="zstd"):
+                            storage=None, downsamplings=(), multi_res=False, compression="zstd", bounding_box=None,
+                            bdv=False, xml_out=None, num_channels=None, num_timepoints=None):
     """`./create-fusion-container -x dataset.xml -o fused.zarr [-s ZARR|N5] -d FLOAT32 --blockSize ... [--multiRes |
-    -ds ...] [-c Zstandard]`: bounding box of all views (Import.getBoundingBox, J/CreateFusionContainer.java:184-211),
-    NumChannels / NumTimepoints from the XML (:213-216), datasets + metadata.  Defaults follow the reference: OME-ZARR
-    storage unless the path ends in .n5 (:67-69), Zstandard compression (:71-76).  ``downsamplings``: relative steps."""
+    -ds ...] [-c Zstandard] [-b name] [-ch n] [-tp n] [--bdv -xo fused.xml]`: the fusion target
+    (Import.getBoundingBox, J/CreateFusionContainer.java:184-211, J/util/Import.java:39-66), datasets + metadata.
+    Defaults follow the reference: OME-ZARR storage unless the path ends in .n5 (:67-69), Zstandard compression
+    (:71-76).  ``downsamplings``: relative steps.
+
+    ``bounding_box`` (`-b`): the named <BoundingBoxDefinition> of the XML instead of the box of all views; an unknown
+    name raises ValueError.  With ``preserve_anisotropy`` its z range becomes floor(min_z / af) .. ceil(max_z / af)
+    (:204-206), which needs ``anisotropy_factor``.
+
+    ``num_channels`` / ``num_timepoints`` (`-ch` / `-tp`): the number of fused volumes per axis, default the XML's
+    (:157-176).  affine_fusion then needs its ``channel`` and ``timepoint`` to fill them.
+
+    ``bdv`` (`--bdv`, :391-487) also writes ``xml_out`` (`-xo`, required: ValueError without it), a BigStitcher
+    project of the fused volumes (spimdata.fusion_project): one setup per channel, timepoints 0 .. n-1, read through a
+    `bdv.n5` loader (N5: the volumes become `setup{c}/timepoint{t}/s{l}`) or a `bdv.multimg.zarr` loader whose
+    `<zgroup>`s point at the container's root multiscale group with indices [c, t] (ZARR: the 5-D arrays are
+    unchanged).  affine_fusion fills either layout.  Everything else, and the default containers, are unchanged."""
+    if bdv and xml_out is None:
+        raise ValueError("Please specify the output XML for the BDV dataset: -xo")
     data = SpimData2.load(xml_path)
-    lo = np.full(3, np.inf)
-    hi = np.full(3, -np.inf)
     af = anisotropy_factor if preserve_anisotropy else float("nan")
-    regs = bf.adjust_all_transforms({v: data.model(*v) for v in data.view_ids()}, af)
-    for v, M in regs.items():
-        bmin, bmax = bf.transformed_bounding_box(data.setups[v[1]].size, M)
-        lo = np.minimum(lo, bmin)
-        hi = np.maximum(hi, bmax)
+    if bounding_box is None:
+        lo = np.full(3, np.inf)
+        hi = np.full(3, -np.inf)
+        regs = bf.adjust_all_transforms({v: data.model(*v) for v in data.view_ids()}, af)
+        for v, M in regs.items():
+            bmin, bmax = bf.transformed_bounding_box(data.setups[v[1]].size, M)
+            lo = np.minimum(lo, bmin)
+            hi = np.maximum(hi, bmax)
+    else:
+        boxes = data.bounding_boxes()
+        if bounding_box not in boxes:
+            raise ValueError(f"Bounding box '{bounding_box}' not present in XML.")
+        lo, hi = (b.copy() for b in boxes[bounding_box])
+        if preserve_anisotropy:
+            if math.isnan(af):
+                raise ValueError("a named bounding box with preserve_anisotropy needs anisotropy_factor")
+            lo[2] = math.floor(lo[2] / af)
+            hi[2] = math.ceil(hi[2] / af)
     if storage is None:   # guessed from the extension like the reference (J/SparkAffineFusion.java:206-225)
         storage = "N5" if out_path.rstrip("/").lower().endswith(".n5") else "ZARR"
+    is_zarr = storage.upper() == "ZARR"
     dims = [int(hi[d] - lo[d] + 1) for d in range(3)]
     if multi_res and not downsamplings:
         downsamplings = estimate_multires_pyramid(dims, af)
@@ -125,13 +154,26 @@ def create_fusion_container(xml_path, out_path, block_size=(128, 128, 128), dtyp
         top = 255.0 if dtype == "uint8" else 65535.0
         min_intensity = 0.0 if min_intensity is None else min_intensity
         max_intensity = top if max_intensity is None else max_intensity
-    kw = dict(anisotropy_factor=af if preserve_anisotropy else None, num_channels=len(data.channels_ordered()),
-              num_timepoints=len(data.timepoints), compression=compression, downsamplings=downsamplings)
-    if storage.upper() == "ZARR":
-        return bzarr.create_fusion_container_zarr(out_path, os.path.abspath(xml_path), lo.astype(np.int64),
-                                                  hi.astype(np.int64), block_size, dtype, min_intensity, max_intensity, **kw)
-    return bn5.create_fusion_container(out_path, os.path.abspath(xml_path), lo.astype(np.int64), hi.astype(np.int64),
-                                       block_size, dtype, min_intensity, max_intensity, **kw)
+    nc = len(data.channels_ordered()) if num_channels is None else int(num_channels)
+    nt = len(data.timepoints) if num_timepoints is None else int(num_timepoints)
+    kw = dict(anisotropy_factor=af if preserve_anisotropy else None, num_channels=nc, num_timepoints=nt,
+              compression=compression, downsamplings=downsamplings)
+    if bdv:
+        kw["output_xml"] = os.path.abspath(xml_out)
+    create = bzarr.create_fusion_container_zarr if is_zarr else bn5.create_fusion_container
+    store = create(out_path, os.path.abspath(xml_path), lo.astype(np.int64), hi.astype(np.int64), block_size, dtype,
+                   min_intensity, max_intensity, **kw)
+    if bdv:
+        project = fusion_project(xml_out, dims, nc, nt, af if preserve_anisotropy else None)
+        if is_zarr:
+            # the level datasets are "0", "1", ... of the root group (J/CreateFusionContainer.java:443-449)
+            project.set_image_loader("bdv.multimg.zarr", out_path, xml_out,
+                                     {(t, c): ("", c, t) for c in range(nc) for t in range(nt)})
+        else:
+            project.set_image_loader("bdv.n5", out_path, xml_out)
+        os.makedirs(os.path.dirname(os.path.abspath(xml_out)), exist_ok=True)
+        project.save(xml_out)
+    return store
 
 
 # --------------------------------------------------------------------------------------------- affine-fusion
@@ -216,6 +258,12 @@ def affine_fusion(out_path, ctx: Context, fusion_type="AVG_BLEND", block_scale=(
     its views super-block by super-block on the device, write the blocks with N5Utils.saveBlock semantics and build
     the multi-resolution pyramid (:703-782).  Returns the list of s0 datasets written.
 
+    Every container create_fusion_container writes is filled: plain N5 / OME-ZARR and the BDV projects (FusionFormat
+    "BDV/N5": volume (c, t) is MultiResolutionInfos[c + t * NumChannels], the BDV-N5 view (t, setup c); "BDV/OME-ZARR":
+    the 5-D arrays at [t, c]).  The views come from InputXML.  When the container's NumChannels / NumTimepoints differ
+    from the XML's (`-ch` / `-tp`), ``channel`` and ``timepoint`` are required and name the one container volume to
+    fuse; every view of ``view_selection`` (default all) goes into it (J/SparkAffineFusion.java:255-264,327-340,439).
+
     Source staging is block-wise (OverlappingBlocks / ViewUtil.findOverlappingBlocks, J/fusion/OverlappingBlocks.java:
     133-161): the super-block grid is walked in z-slabs; for every slab only the source WINDOW of each overlapping
     view is read from its container -- at the mipmap level ViewUtil's best-resolution rule picks
@@ -245,9 +293,15 @@ def affine_fusion(out_path, ctx: Context, fusion_type="AVG_BLEND", block_scale=(
     data = SpimData2.load(meta["input_xml"])
     src = bvs.open_views(data)
     nc, nt = int(meta["num_channels"]), int(meta["num_timepoints"])
-    if nc != len(data.channels_ordered()) or nt != len(data.timepoints):
+    # a container sized by -ch / -tp: the caller names the volume and the views that go into it
+    # (J/SparkAffineFusion.java:255-264,327-340,439)
+    manual = nc != len(data.channels_ordered()) or nt != len(data.timepoints)
+    if manual and (channel is None or timepoint is None):
         raise ValueError(f"container says {nc} channel(s) / {nt} timepoint(s), the XML has "
-                         f"{len(data.channels_ordered())} / {len(data.timepoints)}")
+                         f"{len(data.channels_ordered())} / {len(data.timepoints)}: give channel and timepoint (the "
+                         f"container volume to fuse) and, optionally, view_selection (the views fused into it)")
+    if manual and not (0 <= int(channel) < nc and 0 <= int(timepoint) < nt):
+        raise ValueError(f"channel {channel} / timepoint {timepoint} outside the container's {nc} x {nt} volumes")
     written = []
     done = set()
     selected = data.select_views(**view_selection) if view_selection else None
@@ -259,7 +313,7 @@ def affine_fusion(out_path, ctx: Context, fusion_type="AVG_BLEND", block_scale=(
                 continue
             done.add((ci, ti))
             levels = meta["mr_infos"][0 if is_zarr else ci + ti * nc]
-            vol_views = data.views_of(ci, ti, selected)
+            vol_views = (selected or data.view_ids()) if manual else data.views_of(ci, ti, selected)
             if not vol_views:
                 continue                                             # nothing selected for this volume
             _fuse_volume_blockwise(ctx, data, src, _Sink(store, is_zarr, ci, ti), meta, levels, vol_views,
@@ -1337,8 +1391,7 @@ def resave(xml_path, ctx: Context, xml_out=None, n5=False, out_path=None, block_
         for v in views:
             dims0, dt = meta[v]
             if n5:
-                store.set_attributes(f"setup{v[1]}", {"downsamplingFactors": [list(s) for s in steps], "dataType": dt})
-                store.set_attributes(f"setup{v[1]}/timepoint{v[0]}", {"resolution": [1.0, 1.0, 1.0], "multiScale": True})
+                bn5.set_bdv_attributes(store, v[1], v[0], steps, dt)
                 for li, f in enumerate(steps):
                     store.create_dataset(bn5.bdv_dataset(v[1], v[0], li), [int(dims0[d]) // f[d] for d in range(3)], bs,
                                          np.dtype(dt), comp, compression_level)

@@ -289,26 +289,38 @@ def bdv_dataset(setup: int, timepoint: int, level: int = 0) -> str:
     return f"setup{setup}/timepoint{timepoint}/s{level}"
 
 
+def set_bdv_attributes(store: N5Store, setup: int, timepoint: int, factors, dtype):
+    """The BDV-N5 metadata of one view (PARITY_GAPS R6): `setup{S}` gets the absolute `downsamplingFactors` of every
+    level and `dataType`, `setup{S}/timepoint{T}` gets `resolution` [1, 1, 1] and `multiScale` true."""
+    store.set_attributes(f"setup{setup}", {"downsamplingFactors": [list(f) for f in factors],
+                                           "dataType": _dtype_name(dtype)})
+    store.set_attributes(f"setup{setup}/timepoint{timepoint}", {"resolution": [1.0, 1.0, 1.0], "multiScale": True})
+
+
 def write_bdv_setup(store: N5Store, setup: int, timepoint: int, volume: np.ndarray, block_size=(128, 128, 128),
                     downsampling_factors=((1, 1, 1),), compression="raw"):
-    store.set_attributes(f"setup{setup}", {"downsamplingFactors": [list(f) for f in downsampling_factors],
-                                           "dataType": _dtype_name(volume.dtype)})
-    store.set_attributes(f"setup{setup}/timepoint{timepoint}", {"resolution": [1.0, 1.0, 1.0], "multiScale": True})
+    set_bdv_attributes(store, setup, timepoint, downsampling_factors, volume.dtype)
     store.write_volume(bdv_dataset(setup, timepoint, 0), volume, block_size, compression)
 
 
 def create_fusion_container(root, input_xml, bb_min, bb_max, block_size=(128, 128, 128), dtype="float32",
                             min_intensity=None, max_intensity=None, num_timepoints=1, num_channels=1,
-                            anisotropy_factor=None, compression="raw", downsamplings=()):
+                            anisotropy_factor=None, compression="raw", downsamplings=(), output_xml=None):
     """`create-fusion-container -s N5` (J/CreateFusionContainer.java:302-320,490-519): per
     (channel, timepoint) dataset `ch{c}tp{t}/s0` plus the `Bigstitcher-Spark/*` root attributes
-    that `affine-fusion` reads back (J/SparkAffineFusion.java:241-307)."""
+    that `affine-fusion` reads back (J/SparkAffineFusion.java:241-307).
+
+    With ``output_xml`` (`--bdv -xo`, :391-487) the volumes are BDV-N5 views instead: view (t, setup c) at
+    `setup{c}/timepoint{t}/s{l}` with the BDV-N5 attributes (set_bdv_attributes), FusionFormat "BDV/N5" and
+    OutputXML = ``output_xml``.  Either way MultiResolutionInfos[c + t * num_channels] holds volume (c, t), the
+    index affine-fusion reads (J/SparkAffineFusion.java:454)."""
     store = N5Store(root, create=True)
     dims = [int(bb_max[d] - bb_min[d] + 1) for d in range(3)]
+    name = bdv_dataset if output_xml else (lambda c, t, lvl: f"ch{c}tp{t}/s{lvl}")
     mr = []
     for t in range(num_timepoints):
         for c in range(num_channels):
-            ds = f"ch{c}tp{t}/s0"
+            ds = name(c, t, 0)
             store.create_dataset(ds, dims, block_size, _DTYPES[dtype], compression)
             levels = [{"dataset": ds, "dimensions": dims, "blockSize": list(block_size),
                        "relativeDownsampling": [1, 1, 1], "absoluteDownsampling": [1, 1, 1], "dataType": dtype}]
@@ -318,13 +330,16 @@ def create_fusion_container(root, input_xml, bb_min, bb_max, block_size=(128, 12
             for lvl, rel in enumerate(downsamplings, start=1):
                 cur = [cur[d] // int(rel[d]) for d in range(3)]
                 absd = [absd[d] * int(rel[d]) for d in range(3)]
-                dsl = f"ch{c}tp{t}/s{lvl}"
+                dsl = name(c, t, lvl)
                 store.create_dataset(dsl, cur, block_size, _DTYPES[dtype], compression)
                 levels.append({"dataset": dsl, "dimensions": list(cur), "blockSize": list(block_size),
                                "relativeDownsampling": [int(v) for v in rel], "absoluteDownsampling": list(absd),
                                "dataType": dtype})
+            if output_xml:
+                set_bdv_attributes(store, c, t, [lv["absoluteDownsampling"] for lv in levels], _DTYPES[dtype])
             mr.append(levels)
-    flat = {"FusionFormat": "N5", "InputXML": input_xml, "NumTimepoints": num_timepoints, "NumChannels": num_channels,
+    flat = {"FusionFormat": "BDV/N5" if output_xml else "N5", "InputXML": input_xml,
+            "NumTimepoints": num_timepoints, "NumChannels": num_channels,
             "Boundingbox_min": [int(v) for v in bb_min], "Boundingbox_max": [int(v) for v in bb_max],
             "PreserveAnisotropy": anisotropy_factor is not None,
             "DataType": dtype.lower(),      # N5's DataType adapter (de)serialises lowercase names
@@ -334,6 +349,8 @@ def create_fusion_container(root, input_xml, bb_min, bb_max, block_size=(128, 12
     if dtype != "float32":
         flat["MinIntensity"] = float(min_intensity)
         flat["MaxIntensity"] = float(max_intensity)
+    if output_xml:
+        flat["OutputXML"] = output_xml
     attrs = bs_attrs(flat)
     store.set_attributes("", attrs)
     return store

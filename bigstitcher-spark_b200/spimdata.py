@@ -11,6 +11,8 @@ extensions) -- the fields the two hot paths consume and produce:
     overlap_boundingbox (6 doubles)                                   (J/SparkPairwiseStitching.java:284-301,328-390)
   * <ViewInterestPoints><ViewInterestPointsFile timepoint setup label params>path of the label's group in
     interestpoints.n5 (InterestPointTools.addInterestPoints, J/SparkInterestPointDetection.java:898-903)
+  * <BoundingBoxes><BoundingBoxDefinition name>: <min> and <max> (inclusive) integer corners in world coordinates
+    (XmlIoBoundingBoxes, recalled; read by Import.getBoundingBox, J/util/Import.java:39-66)
 
 Host-side plumbing only.  Everything else in the file is preserved verbatim on save.
 """
@@ -357,6 +359,71 @@ class SpimData2:
             entries[(int(tp), int(setup), label)] = f
         for k in sorted(entries):
             vip.append(entries[k])
+
+    # ------------------------------------------------------------------ bounding boxes
+    def bounding_boxes(self):
+        """{name: (min int64[3], max int64[3])} of <BoundingBoxes>, max inclusive.  When two definitions share a name
+        the later one wins, as in Import.getBoundingBox (J/util/Import.java:53-57)."""
+        out = {}
+        bbs = self.root.find("BoundingBoxes")
+        for b in (bbs.findall("BoundingBoxDefinition") if bbs is not None else []):
+            out[b.get("name")] = tuple(np.array([int(v) for v in b.findtext(k).split()], dtype=np.int64)
+                                       for k in ("min", "max"))
+        return out
+
+    def set_bounding_box(self, name, bb_min, bb_max):
+        """Append a <BoundingBoxDefinition> (earlier ones of the same name stay, and lose to this one on reading)."""
+        bbs = self.root.find("BoundingBoxes")
+        if bbs is None:
+            bbs = ET.SubElement(self.root, "BoundingBoxes")
+        b = ET.SubElement(bbs, "BoundingBoxDefinition", name=str(name))
+        ET.SubElement(b, "min").text = " ".join(str(int(v)) for v in bb_min)
+        ET.SubElement(b, "max").text = " ".join(str(int(v)) for v in bb_max)
+
+
+# ---------------------------------------------------------------------------------------------
+def fusion_project(xml_path, dims_xyz, num_channels, num_timepoints, anisotropy_factor=None) -> SpimData2:
+    """The BigStitcher project of a fused container (SpimData2Tools.createNewSpimDataForFusion, recalled; the setups
+    and timepoints are J/CreateFusionContainer.java:404-434, in-repo): one ViewSetup per channel c (id c, name
+    "setup c", size ``dims_xyz``, Tile 0, Channel c, Angle 0, Illumination 0), timepoints 0 .. n-1, and one
+    `calibration` ViewTransform per view, diag(1, 1, af) with ``anisotropy_factor`` (identity without), matching the
+    voxel size (1, 1, af) or (1, 1, 1) micrometer.  The box minimum is not carried: world = fused pixel grid.  No
+    ImageLoader yet (set_image_loader adds it); not saved."""
+    af = 1.0 if anisotropy_factor is None else float(anisotropy_factor)
+    root = ET.Element("SpimData", version="0.2")
+    ET.SubElement(root, "BasePath", type="relative").text = "."
+    seq = ET.SubElement(root, "SequenceDescription")
+    vss = ET.SubElement(seq, "ViewSetups")
+    for c in range(num_channels):
+        vs = ET.SubElement(vss, "ViewSetup")
+        ET.SubElement(vs, "id").text = str(c)
+        ET.SubElement(vs, "name").text = f"setup {c}"
+        ET.SubElement(vs, "size").text = " ".join(str(int(v)) for v in dims_xyz)
+        vx = ET.SubElement(vs, "voxelSize")
+        ET.SubElement(vx, "unit").text = "micrometer"
+        ET.SubElement(vx, "size").text = _fmt([1.0, 1.0, af])
+        at = ET.SubElement(vs, "attributes")
+        for tag, v in (("illumination", 0), ("channel", c), ("tile", 0), ("angle", 0)):
+            ET.SubElement(at, tag).text = str(v)
+    for tag, ids in (("illumination", [0]), ("channel", range(num_channels)), ("tile", [0]), ("angle", [0])):
+        a = ET.SubElement(vss, "Attributes", name=tag)
+        for i in ids:
+            e = ET.SubElement(a, tag.capitalize())
+            ET.SubElement(e, "id").text = str(i)
+            ET.SubElement(e, "name").text = f"Channel {i}" if tag == "channel" else str(i)
+    tp = ET.SubElement(seq, "Timepoints", type="pattern")
+    ET.SubElement(tp, "integerpattern").text = "0" if num_timepoints == 1 else f"0-{num_timepoints - 1}"
+    ET.SubElement(seq, "MissingViews")
+    vrs = ET.SubElement(root, "ViewRegistrations")
+    for t in range(num_timepoints):
+        for c in range(num_channels):
+            vr = ET.SubElement(vrs, "ViewRegistration", timepoint=str(t), setup=str(c))
+            vt = ET.SubElement(vr, "ViewTransform", type="affine")
+            ET.SubElement(vt, "Name").text = "calibration"
+            ET.SubElement(vt, "affine").text = _fmt([1, 0, 0, 0, 0, 1, 0, 0, 0, 0, af, 0])
+    for tag in ("ViewInterestPoints", "BoundingBoxes", "PointSpreadFunctions", "StitchingResults", "IntensityAdjustments"):
+        ET.SubElement(root, tag)
+    return SpimData2(ET.ElementTree(root), xml_path)
 
 
 # ---------------------------------------------------------------------------------------------

@@ -261,11 +261,13 @@ def create_multiscale_group(store: ZarrStore, group, dims_xyz, dtype, block_size
 def create_fusion_container_zarr(root, input_xml, bb_min, bb_max, block_size=(128, 128, 128), dtype="float32",
                                  min_intensity=None, max_intensity=None, num_timepoints=1, num_channels=1,
                                  anisotropy_factor=None, compression="raw", voxel_size=(1.0, 1.0, 1.0),
-                                 downsamplings=()):
+                                 downsamplings=(), output_xml=None):
     """`create-fusion-container -s ZARR` (J/CreateFusionContainer.java:331-389): one 5-D array per resolution level
     ("0", "1", ...: levelToName :346), the OME-NGFF v0.4 `multiscales` attribute with one scale + translation per
     level (:374-388) and the `Bigstitcher-Spark/*` root attributes.  ``downsamplings``: RELATIVE steps after s0
-    (e.g. [(2,2,1), (2,2,2)]); the 5-D pyramid of N5ApiTools.setupMultiResolutionPyramid never downsamples c / t."""
+    (e.g. [(2,2,1), (2,2,2)]); the 5-D pyramid of N5ApiTools.setupMultiResolutionPyramid never downsamples c / t.
+    With ``output_xml`` (`--bdv -xo`, :391-402) the arrays are the same; FusionFormat is "BDV/OME-ZARR" and
+    OutputXML = ``output_xml``."""
     st = ZarrStore(root, create=True)
     dims = [int(bb_max[d] - bb_min[d] + 1) for d in range(3)]
     levels, datasets = [], []
@@ -290,7 +292,8 @@ def create_fusion_container_zarr(root, input_xml, bb_min, bb_max, block_size=(12
                              {"name": "y", "type": "space", "unit": "micrometer"},
                              {"name": "x", "type": "space", "unit": "micrometer"}],
                     "datasets": datasets}]
-    flat = {"FusionFormat": "OME-ZARR", "InputXML": input_xml, "NumTimepoints": num_timepoints, "NumChannels": num_channels,
+    flat = {"FusionFormat": "BDV/OME-ZARR" if output_xml else "OME-ZARR", "InputXML": input_xml,
+            "NumTimepoints": num_timepoints, "NumChannels": num_channels,
             "Boundingbox_min": [int(v) for v in bb_min], "Boundingbox_max": [int(v) for v in bb_max],
             "PreserveAnisotropy": anisotropy_factor is not None, "DataType": dtype.lower(),
             "BlockSize": list(block_size), "MultiResolutionInfos": [levels]}
@@ -299,6 +302,8 @@ def create_fusion_container_zarr(root, input_xml, bb_min, bb_max, block_size=(12
     if dtype != "float32":
         flat["MinIntensity"] = float(min_intensity)
         flat["MaxIntensity"] = float(max_intensity)
+    if output_xml:
+        flat["OutputXML"] = output_xml
     attrs = {"multiscales": multiscales}
     attrs.update(bs_attrs(flat))
     st.set_attributes("", attrs)
@@ -308,6 +313,6 @@ def create_fusion_container_zarr(root, input_xml, bb_min, bb_max, block_size=(12
 def read_fusion_container_zarr(root):
     st = ZarrStore(root)
     meta = parse_fusion_metadata(st.get_attributes(""))
-    if meta["format"] != "OME-ZARR":
+    if meta["format"] not in ("OME-ZARR", "BDV/OME-ZARR"):
         raise KeyError("not a BigStitcher-Spark OME-ZARR fusion container")
     return st, meta
