@@ -5,7 +5,9 @@ import pytest
 
 from bsgpu import commands, intensity as bint, n5 as bn5, spimdata
 from oracle import intensity_oracle as io
-from tests.intensity_scene import IntensityFakeContext, overlap_disagreement, planted_dataset
+from tests.intensity_scene import (DEFAULT_GRID, WIDE_SLOTS, IntensityFakeContext, apply_bound, apply_case,
+                                   candidate_value_bound, integer_scene, later_round_bucket, overlap_disagreement,
+                                   planted_dataset, shifted_grid_scene)
 
 
 def test_cell_index_at_the_edges():
@@ -144,3 +146,72 @@ def test_num_coefficients_mismatch_warns_and_uses_the_stored_size(tmp_path):
     with pytest.warns(UserWarning, match="numCoefficients"):
         co = commands.solve_intensities(xml, str(tmp_path / "c.zarr"), m, num_coefficients=(8, 8, 8), max_iterations=20)
     assert all(a.shape == (1, 2, 2) for a, _ in co.values())
+
+
+# ------------------------------------------------------------------------------------------------ float64 references
+@pytest.mark.parametrize("scene", ["default_grid", "wide_slots", "integer_200", "integer_nan"])
+def test_candidates_reference_agrees_with_the_oracle(scene):
+    """On the exact-geometry scenes of the kernel tests the float64 reference keeps the same points under the same
+    keys as the bit-level oracle, and its values are within 16 u max|corner| (PARITY_GAPS row 37)."""
+    if scene.startswith("integer"):
+        A, B, va, vb, rmin, rmax = integer_scene()
+        th = (1.0, 200.0 if scene == "integer_200" else float("nan"))
+    else:
+        A, B, va, vb, rmin, rmax = shifted_grid_scene(**(DEFAULT_GRID if scene == "default_grid" else WIDE_SLOTS))
+        th = (1.0, float("nan"))
+    want = io.candidates(A, va, B, vb, 1.0, rmin, rmax, *th)
+    keys, offs, cnts, vals, cmax = io.candidates_reference(A, va, B, vb, 1.0, rmin, rmax, *th, corners=True)
+    for g, w in zip((keys, offs, cnts), want[:3]):
+        assert np.array_equal(g, w)
+    assert np.all(np.abs(want[3] - vals) <= candidate_value_bound(cmax))
+    assert len(keys) >= 32 and len(vals) > 10000
+
+
+def test_integer_scene_sits_on_every_boundary():
+    """The integer scene reaches what its GPU test relies on: values exactly at min_threshold 1 and max_threshold
+    200 among the kept points (so > instead of >= changes the output), and render points exactly on p = d - 1 and on
+    cell borders p n / d in Z of both views."""
+    A, B, va, vb, rmin, rmax = integer_scene()
+    _, _, _, vals = io.candidates_reference(A, va, B, vb, 1.0, rmin, rmax, 1.0, 200.0)
+    assert (vals == 1.0).any() and (vals == 200.0).any()
+    strict = io.candidates_reference(A, va, B, vb, 1.0, rmin, rmax, np.nextafter(1.0, 2.0), np.nextafter(200.0, 0.0))
+    assert len(strict[3]) < len(vals)
+    g = np.stack(np.meshgrid(*[np.arange(rmin[k], rmax[k] + 1) for k in range(3)], indexing="ij")).reshape(3, -1)
+    for v in (va, vb):
+        m = np.asarray(v["world_to_px"]).reshape(3, 4)
+        p = m[:, :3] @ g + m[:, 3:]
+        d, n = np.asarray(v["full_dims"])[:, None], np.asarray(v["n_cells"])[:, None]
+        assert (p == d - 1).any()
+        border = (p * n % d == 0) & (p > 0)
+        assert border.any(axis=1).all()
+
+
+@pytest.mark.parametrize("x", [1, 257, 600])
+@pytest.mark.parametrize("level", [0, 1, 2])
+@pytest.mark.parametrize("dtype", [np.uint8, np.uint16, np.float32])
+def test_apply_reference_agrees_with_the_oracle(x, level, dtype):
+    vol, wmin, mt, full, ca, cb = apply_case(x, level, dtype)
+    want = io.apply(vol, wmin, mt, full, ca, cb)
+    ref = io.apply_reference(vol, wmin, mt, full, ca, cb)
+    assert np.all(np.abs(want - ref) <= apply_bound(vol, wmin, mt, full, ca, cb))
+
+
+def test_apply_reference_is_the_cell_value_at_centres_and_clamps():
+    # 2 cells over 34 px: centres at 8 and 25, constant beyond them; halfway between them the mean
+    ca, cb = np.array([[[2.0, 5.0]]]), np.array([[[-1.0, 3.0]]])
+    out = io.apply_reference(np.full((1, 1, 34), 2.0), (0, 0, 0), np.eye(3, 4), (34, 1, 1), ca, cb)[0, 0]
+    assert out[0] == out[8] == 3.0 and out[25] == out[33] == 13.0
+    assert np.isclose(out[16], 2 * (2 + 3 * 8 / 17) - 1 + 4 * 8 / 17, rtol=1e-15)
+    # a 2x level: level voxel l sits at full-resolution q = 2 l + 0.5, so l = 4 is at fractional cell 9 * 2 / 34 - 0.5
+    mt = np.array([[2, 0, 0, 0.5], [0, 1, 0, 0], [0, 0, 1, 0]], np.float64)
+    u = 9 * 2 / 34 - 0.5
+    got = io.apply_reference(np.ones((1, 1, 17)), (0, 0, 0), mt, (34, 1, 1), ca, cb)[0, 0, 4]
+    assert np.isclose(got, (2 + 3 * u) + (-1 + 4 * u), rtol=1e-15)
+
+
+def test_later_round_bucket_has_one_triple_found_first_at_h_1024():
+    x, y = later_round_bucket()
+    for iters, want in ((1024, 2), (1025, 3)):
+        a, b, c = io.ransac_bucket(np.stack([x, y], 1), 0, iters, 1e-3)
+        assert c == want
+    assert (a, b) == (2.0, 3.0)
