@@ -12,6 +12,10 @@
   resave                  J/SparkResaveN5.java:80-455             (OME-ZARR or BDV-N5 with the pyramid built on the device)
   match_intensities       J/SparkIntensityMatching.java:84-190    (pairwise intensity matches, RANSAC on the device)
   solve_intensities       J/IntensitySolver.java:50-123           (per-view intensity coefficients)
+  downsample              J/SparkDownsample.java:60-190           (pyramid levels of an existing dataset, on the device)
+  clear_interestpoints    J/ClearInterestPoints.java              (points + correspondences, or correspondences only)
+  clear_registrations     J/ClearRegistrations.java               (drop the latest <ViewTransform>s)
+  transform_points        J/TransformPoints.java                  (view pixel coordinates -> world, host only)
 
 Every command reads its images through viewsource.py, so `bdv.n5` and `bdv.multimg.zarr` datasets both work.
 
@@ -21,6 +25,7 @@ from __future__ import annotations
 
 import math
 import os
+import re
 import shutil
 from decimal import Decimal
 
@@ -536,13 +541,18 @@ def _write_resident_levels(ctx, cur_h, gb, sink, levels, bs, np_dt):
         ctx.volume_free(cur_h)
 
 
-def _pyramid_from_stored(ctx, volumes, first, compute, bs, shard=(0, 1), retries=5, barrier=None):
+def _pyramid_from_stored(ctx, volumes, first, compute, bs, shard=(0, 1), retries=5, barrier=None, resident=1):
     """Levels ``first`` .. N of every volume in ``volumes`` ([(sink, levels, numpy dtype)]): every compute block of level
     l is the 2x average of its region of level l-1, read back from the container and averaged on the device.  Rank r of
     w takes blocks [r::w] of each level; ``barrier()`` runs before each level so that level l-1 is complete on every
-    rank.  Failed blocks are retried up to ``retries`` times (RetryTrackerSpark)."""
+    rank.  Failed blocks are retried up to ``retries`` times (RetryTrackerSpark).
+
+    ``resident`` > 1: levels first + 1 .. first + resident - 1 are derived from each compute block of level ``first``
+    while it is on the device (_write_resident_levels); those compute blocks must cover whole storage blocks of them."""
     rank, world = shard
-    for li in range(first, max(len(lv) for _, lv, _ in volumes)):
+    li = first
+    while li < max(len(lv) for _, lv, _ in volumes):
+        n = resident if li == first else 1
         if barrier is not None:
             barrier()                                # level l-1 is complete on every rank
         work = []
@@ -560,19 +570,20 @@ def _pyramid_from_stored(ctx, volumes, first, compute, bs, shard=(0, 1), retries
                 sink, levels, np_dt, (off, size, gpos) = item
                 prev, cur = levels[li - 1], levels[li]
                 rel = [int(v) for v in cur["relativeDownsampling"][:3]]
-                h = h2 = None
+                h = None
                 try:
                     srcblk = sink.read_region(prev["dataset"], [off[d] * rel[d] for d in range(3)], [size[d] * rel[d] for d in range(3)])
                     h = ctx.volume_upload(np.ascontiguousarray(srcblk))
-                    h2 = ctx.downsample(h, rel)
-                    sink.save(cur["dataset"], ctx.volume_download(h2, size, np_dt), gpos)
+                    # the downsampled block is freed by _write_resident_levels
+                    _write_resident_levels(ctx, ctx.downsample(h, rel), (off, size, gpos), sink, levels[li:li + n], bs,
+                                           np_dt)
                 except native.BsError:
                     failed.append(item)
                 finally:
-                    for hh in (h, h2):
-                        if hh is not None:
-                            ctx.volume_free(hh)
+                    if h is not None:
+                        ctx.volume_free(h)
             todo = failed
+        li += n
 
 
 def _storage_cells(gb, bs):
@@ -1448,3 +1459,238 @@ def resave(xml_path, ctx: Context, xml_out=None, n5=False, out_path=None, block_
 def _resave_group(view):
     """The OME-ZARR group of a resaved view (PARITY_GAPS R3)."""
     return f"s{view[1]}-t{view[0]}.zarr"
+
+
+# --------------------------------------------------------------------------------------------- downsample
+DOWNSAMPLE_DTYPES = ("uint8", "uint16", "float32")          # what bs_downsample takes
+
+
+def parse_downsample_steps(downsampling):
+    """`-ds "2,2,1; 2,2,1; 2,2,2"` (or a list of triples): the consecutive steps of `downsample`, each RELATIVE to the
+    level before.  A step must be 1 or 2 per axis (PARITY_GAPS U1); anything else raises ValueError."""
+    if isinstance(downsampling, str):
+        steps = [tuple(int(v) for v in s.split(",")) for s in downsampling.split(";") if s.strip()]
+    else:
+        steps = [tuple(int(v) for v in s) for s in downsampling]
+    if not steps or any(len(s) != 3 for s in steps):
+        raise ValueError(f"-ds {downsampling}: need x,y,z triples")
+    for s in steps:
+        if any(v not in (1, 2) for v in s):
+            raise ValueError(f"-ds {downsampling}: step {s} is not 1 or 2 per axis")
+    return steps
+
+
+class _NonEmptySink(_Sink):
+    """N5Utils.saveNonEmptyBlock (J/SparkDownsample.java:176): the storage blocks of a saved block whose voxels are all
+    0 are not written, so they read back as 0 (PARITY_GAPS U2)."""
+
+    def __init__(self, store, is_zarr, block_size):
+        super().__init__(store, is_zarr, 0, 0)
+        self.bs = [int(v) for v in block_size]
+
+    def save(self, dataset, block, grid_pos):
+        for off, size, gpos in _storage_cells(((0, 0, 0), block.shape[::-1], grid_pos), self.bs):
+            part = block[off[2]:off[2] + size[2], off[1]:off[1] + size[1], off[0]:off[0] + size[0]]
+            if part.any():
+                super().save(dataset, np.ascontiguousarray(part), gpos)
+
+
+def _downsample_input(n5_path, storage, dataset):
+    """(store, is_zarr, dims xyz, block size xyz, dtype name, create(dataset, dims xyz)) of the input of `downsample`
+    (PARITY_GAPS U3); ``create`` makes a dataset with the input's block size, data type and compression."""
+    if storage.upper() == "ZARR":
+        store = bzarr.ZarrStore(n5_path)
+        m = store.array_meta(dataset)
+        shape = [int(v) for v in m["shape"]]
+        if not (len(shape) == 3 or (len(shape) == 5 and shape[:2] == [1, 1])):
+            raise ValueError(f"{dataset}: Zarr shape {shape} is neither (z, y, x) nor (1, 1, z, y, x)")
+        lead = shape[:-3]
+        return (store, True, shape[-3:][::-1], [int(v) for v in m["chunks"][-3:][::-1]],
+                np.dtype(m["dtype"]).newbyteorder("=").name,
+                lambda ds, dims: store.create_array_like(ds, dataset, lead + list(dims)[::-1]))
+    if storage.upper() != "N5":
+        raise ValueError(f"-s {storage} (N5 or ZARR)")
+    store = bn5.N5Store(n5_path)
+    a = store.dataset_attributes(dataset)
+    if len(a["dimensions"]) != 3:
+        raise ValueError(f"{dataset}: {len(a['dimensions'])}-D N5 dataset, downsample takes 3-D ones")
+    if a["compression"]["type"] not in ("raw", "gzip", "zstd"):
+        raise NotImplementedError(f"{dataset}: N5 compression {a['compression']['type']} (writable: raw, gzip, zstd)")
+    return (store, False, [int(v) for v in a["dimensions"]], [int(v) for v in a["blockSize"]], a["dataType"],
+            lambda ds, dims: store.set_attributes(ds, {"dimensions": list(dims), "blockSize": a["blockSize"],
+                                                       "dataType": a["dataType"], "compression": a["compression"]}))
+
+
+def downsample(n5_path, ctx: Context, dataset_in, datasets_out, downsampling, storage="N5", block_scale=(1, 1, 1),
+               dry_run=False, shard=(0, 1), barrier=None, retries=5):
+    """`./downsample -i fused.n5 -di /ch0/s0 -do "/ch0/s1; /ch0/s2" -ds "2,2,1; 2,2,2" [-s N5|ZARR] [--blockScale 1,1,1]`
+    (J/SparkDownsample.java:60-190): pyramid levels for an existing dataset, e.g. the single one nonrigid-fusion writes.
+    Level l (``datasets_out[l-1]``) is ``downsampling[l-1]`` applied to level l-1 (``dataset_in`` for l = 1) by the
+    device 2x step (bs_downsample, LazyHalfPixelDownsample2x per axis whose step is 2; parse_downsample_steps).  Each
+    output gets the input's blockSize, dataType and compression and dims in_dims // step (:126-139); it is computed in
+    blocks of Grid.create(out dims, blockSize * block_scale, blockSize) (:141-147) and storage blocks that come out all
+    0 are not written (saveNonEmptyBlock, :176).  When those compute blocks also cover whole storage blocks of the next
+    levels, the next levels are derived from each one while it is on the device instead of re-read from the container.
+
+    N5 3-D datasets and Zarr arrays of shape (z, y, x) or (1, 1, z, y, x) -- the layout `nonrigid_fusion(...,
+    storage="ZARR")` writes; any other shape raises ValueError.  uint8, uint16 and float32; other types raise
+    NotImplementedError.  A step count that differs from the output count, or an output dim below 1, raises ValueError.
+
+    Multi-GPU: rank 0 creates the datasets; rank r of w (``shard``) takes blocks [r::w] of each level and ``barrier()``
+    (required when w > 1) runs before each level, so that the level it reads is complete.  ``dry_run`` returns the
+    planned [(dataset, dims xyz)] and writes nothing.  Returns the list of datasets written."""
+    if isinstance(datasets_out, str):
+        datasets_out = [s.strip() for s in datasets_out.split(";") if s.strip()]
+    datasets_out = list(datasets_out)
+    steps = parse_downsample_steps(downsampling)
+    if len(steps) != len(datasets_out):
+        raise ValueError(f"{len(datasets_out)} output dataset(s) for {len(steps)} downsampling step(s): give as many "
+                         f"-do as -ds")
+    if len({dataset_in.strip("/")} | {d.strip("/") for d in datasets_out}) != len(datasets_out) + 1:
+        raise ValueError(f"-di {dataset_in} / -do {datasets_out}: every dataset must be a different one")
+    rank, world = shard
+    if world > 1 and barrier is None:
+        raise ValueError("downsample with more than one rank needs barrier(): rank 0 creates the datasets first")
+    store, is_zarr, dims, bs, dt, create = _downsample_input(n5_path, storage, dataset_in)
+    if dt not in DOWNSAMPLE_DTYPES:
+        raise NotImplementedError(f"downsample of {dt} dataset {dataset_in} (bs_downsample takes uint8, uint16, float32)")
+    levels = [dict(dataset=dataset_in, dimensions=dims, relativeDownsampling=[1, 1, 1])]
+    for ds, step in zip(datasets_out, steps):
+        cur = [levels[-1]["dimensions"][d] // step[d] for d in range(3)]
+        if min(cur) < 1:
+            raise ValueError(f"{ds}: {levels[-1]['dimensions']} // {list(step)} = {cur} has an empty axis")
+        levels.append(dict(dataset=ds, dimensions=cur, relativeDownsampling=list(step)))
+    plan = [(lv["dataset"], tuple(lv["dimensions"])) for lv in levels[1:]]
+    if dry_run:
+        return plan
+
+    if rank == 0:
+        for lv in levels[1:]:
+            create(lv["dataset"], lv["dimensions"])
+    compute = [bs[d] * int(block_scale[d]) for d in range(3)]
+    # the levels after s1 whose storage blocks every compute block of s1 covers whole stay on the device
+    resident, acc = 1, [1, 1, 1]
+    while resident < len(steps):
+        acc = [acc[d] * steps[resident][d] for d in range(3)]
+        if any(compute[d] % (acc[d] * bs[d]) for d in range(3)):
+            break
+        resident += 1
+    # the barrier before level 1 also lets every rank in once rank 0 has created the datasets
+    _pyramid_from_stored(ctx, [(_NonEmptySink(store, is_zarr, bs), levels, np.dtype(dt))], 1, compute, bs, shard,
+                         retries, barrier, resident)
+    return datasets_out
+
+
+# --------------------------------------------------------------------------------------------- clear-interestpoints
+def clear_interestpoints(xml_path, correspondences_only=False, dry_run=False):
+    """`./clear-interestpoints -x dataset.xml [--correspondencesOnly] [--dryRun]` (J/ClearInterestPoints.java): returns
+    {view: {label: (interest points, correspondences)}} of every view with interest points in the XML, counted before
+    anything is cleared.  Default: <ViewInterestPoints> is emptied, the XML saved (with a ~1 backup) and the whole
+    `interestpoints.n5` next to it removed.  ``correspondences_only``: every view's and label's correspondences become
+    the empty list (PARITY_GAPS N1: {0} data, empty idMap); the points and the XML stay.  ``dry_run``: counts only."""
+    data = SpimData2.load(xml_path)
+    base = os.path.join(os.path.dirname(os.path.abspath(xml_path)), data.root.findtext("BasePath") or ".")
+    root = os.path.join(base, "interestpoints.n5")
+    store = bn5.N5Store(root) if os.path.isdir(root) else None
+
+    def count(path):
+        dims = store.get_attributes(path).get("dimensions", [0]) if store is not None else [0]
+        return int(dims[1]) if len(dims) == 2 else 0
+
+    report = {}
+    for v, labels in sorted(data.interest_points().items()):
+        report[v] = {lab: (count(e["path"].rstrip("/") + "/interestpoints/loc"),
+                          count(e["path"].rstrip("/") + "/correspondences/data"))
+                     for lab, e in sorted(labels.items())}
+    if dry_run:
+        return report
+    if correspondences_only:
+        store = store or bn5.N5Store(root, create=True)
+        for v, labels in sorted(data.interest_points().items()):
+            for e in labels.values():
+                store.write_correspondences(e["path"], [])
+    else:
+        data.clear_interest_points()
+        data.save(xml_path)
+        shutil.rmtree(root, ignore_errors=True)
+    return report
+
+
+# --------------------------------------------------------------------------------------------- clear-registrations
+def clear_registrations(xml_path, keep=None, remove=None, view_selection=None, dry_run=False):
+    """`./clear-registrations -x dataset.xml (--keep N | --remove N) [view selection] [--dryRun]`
+    (J/ClearRegistrations.java): ``remove`` N drops the first N <ViewTransform>s of each selected view (the most
+    recently applied, e.g. a solve), ``keep`` N drops from the front until N remain; a view with fewer is not an error.
+    Exactly one of them, >= 0, or ValueError.  ``view_selection``: keyword arguments of SpimData2.select_views (default
+    all views; PARITY_GAPS U5).  The XML is saved (with a ~1 backup) unless ``dry_run``.  Returns {view: [(name,
+    3 x 4 affine)]} of the removed transforms, first removed first."""
+    if (keep is None) == (remove is None) or (keep is not None and int(keep) < 0) or (remove is not None and int(remove) < 0):
+        raise ValueError("Please specify --keep OR --remove as >=0.")
+    data = SpimData2.load(xml_path)
+    views = data.select_views(**view_selection) if view_selection else data.view_ids()
+    removed = {}
+    for v in views:
+        n = len(data.registrations[v])
+        drop = min(int(remove), n) if remove is not None else max(n - int(keep), 0)
+        removed[v] = [data.remove_first_registration(v) for _ in range(drop)]
+    if not dry_run:
+        data.save(xml_path)
+    return removed
+
+
+# --------------------------------------------------------------------------------------------- transform-points
+# TransformPoints keeps a CSV line when its trimmed text matches [\p{Space}*[-]*\d+\.?\d*\p{Space}*\,?]+ -- in Java
+# one character class (the nested [-] is a union): whitespace, '*', '-', digits, '+', '.', '?' and ','
+_CSV_POINT = re.compile(r"[ \t\n\x0b\f\r*\-0-9+.?,]+")
+_JAVA_TRIM = "".join(chr(c) for c in range(33))                 # String.trim strips every char <= ' '
+
+
+def _csv_doubles(text):
+    """Import.csvStringToDoubleArray: split at ',' (trailing empty fields dropped, as String.split does), parse each."""
+    parts = text.split(",")
+    while parts and parts[-1] == "":
+        parts.pop()
+    return [float(p.strip(_JAVA_TRIM)) for p in parts]
+
+
+def transform_points(xml_path, view, points=None, csv_in=None, csv_out=None):
+    """`./transform-points -x dataset.xml -vi '0,5' [--csvIn in.csv] [-p x,y,z ...] [--csvOut out.csv]`
+    (J/TransformPoints.java): map pixel coordinates of ``view`` ((tp, setup) or 'tp,setup') to world coordinates with
+    its full registration model.  Points come from ``csv_in`` -- only lines whose trimmed text matches upstream's
+    character-class pattern; others, such as `1e-5` or text, are ignored (PARITY_GAPS U6) -- and then from ``points``
+    (`-p` strings 'x,y,z' or triples).  A point takes the first three values of its line.  No points raises ValueError.
+    Writes `x,y,z` lines in Java's Double.toString format (java_double, PARITY_GAPS U7) to ``csv_out``, or to stdout.
+    Returns the (n, 3) float64 world coordinates."""
+    rows = []
+    if csv_in is not None:
+        with open(csv_in) as f:
+            for line in f.read().splitlines():
+                s = line.strip(_JAVA_TRIM)
+                if s and _CSV_POINT.fullmatch(s):
+                    rows.append(_csv_doubles(s))
+    for p in points or ():
+        if isinstance(p, str):
+            if p.strip(_JAVA_TRIM):
+                rows.append(_csv_doubles(p))
+        else:
+            rows.append([float(v) for v in p])
+    if not rows:
+        raise ValueError("No points defined (use either --csv and/or -p), stopping.")
+    if any(len(r) < 3 for r in rows):
+        raise ValueError(f"a point needs x,y,z: {next(r for r in rows if len(r) < 3)}")
+    data = SpimData2.load(xml_path)
+    v = tuple(int(t) for t in view.split(",")) if isinstance(view, str) else tuple(int(t) for t in view)
+    if v not in data.registrations:
+        raise ValueError(f"view {v} (timepoint, setup) is not in {xml_path}")
+    M = data.model(*v)
+    X = np.array([r[:3] for r in rows], dtype=np.float64)
+    # AffineTransform3D.apply, term by term in its order
+    W = np.stack([X[:, 0] * M[i, 0] + X[:, 1] * M[i, 1] + X[:, 2] * M[i, 2] + M[i, 3] for i in range(3)], axis=1)
+    lines = [",".join(java_double(c) for c in w) for w in W]
+    if csv_out is None:
+        for line in lines:
+            print(line)
+    else:
+        with open(csv_out, "w") as f:
+            f.writelines(line + "\n" for line in lines)
+    return W

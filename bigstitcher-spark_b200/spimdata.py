@@ -148,6 +148,15 @@ class SpimData2:
                 return
         raise KeyError(f"no ViewRegistration for {view}")
 
+    def remove_first_registration(self, view):
+        """Drop the view's <ViewTransform> at index 0 (the one applied last, e.g. the latest solve); returns its
+        (name, 3 x 4 affine).  The view must have one."""
+        for vr in self.root.find("ViewRegistrations").findall("ViewRegistration"):
+            if (int(vr.get("timepoint")), int(vr.get("setup"))) == tuple(view):
+                vr.remove(vr.find("ViewTransform"))
+                return self.registrations[tuple(view)].pop(0)
+        raise KeyError(f"no ViewRegistration for {view}")
+
     def view_ids(self):
         return sorted(self.registrations)
 
@@ -359,6 +368,12 @@ class SpimData2:
             entries[(int(tp), int(setup), label)] = f
         for k in sorted(entries):
             vip.append(entries[k])
+
+    def clear_interest_points(self):
+        """Remove every <ViewInterestPointsFile> (all labels of all views); <ViewInterestPoints> stays, empty."""
+        vip = self.root.find("ViewInterestPoints")
+        for f in (list(vip) if vip is not None else []):
+            vip.remove(f)
 
     # ------------------------------------------------------------------ bounding boxes
     def bounding_boxes(self):

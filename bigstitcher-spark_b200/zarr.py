@@ -9,8 +9,9 @@ through zstd.py).
 The reader also takes 5-D arrays written by other tools (the `bdv.multimg.zarr` input of every command): dtypes in
 any byte order ('<', '>', '|'), both dimension separators ('/' and '.', the Zarr v2 default), compressors null, zstd,
 gzip and zlib, and a missing chunk reads as the array's fill_value.  Any other codec (blosc, ...) raises
-NotImplementedError naming it.  ``read_multiscales`` turns an OME-NGFF 0.4 `multiscales` group into integer mipmap
-factors.  Host-side plumbing only.
+NotImplementedError naming it.  3-D (z, y, x) arrays (what `downsample` reads and writes besides the 5-D ones) are
+read and written by the same methods: their chunk index is the spatial part of (t, c, z, y, x).  ``read_multiscales``
+turns an OME-NGFF 0.4 `multiscales` group into integer mipmap factors.  Host-side plumbing only.
 """
 from __future__ import annotations
 
@@ -100,16 +101,27 @@ class ZarrStore:
             raise KeyError(f"{path} is not a Zarr array")
         return m
 
+    def create_array_like(self, path, like, shape):
+        """An array of ``shape`` with the chunks, dtype, compressor, fill value, order, filters and dimension separator
+        of the array ``like`` of this store.  Compressors other than null, zstd and gzip raise NotImplementedError."""
+        m = dict(self.array_meta(like), shape=[int(v) for v in shape])
+        cid = (m.get("compressor") or {}).get("id")
+        if cid not in (None, "zstd", "gzip"):
+            raise NotImplementedError(f"Zarr compressor {cid!r} (writable: null, zstd, gzip)")
+        self._write_json(path, ".zarray", m)
+
     def _chunk_path(self, path, idx_tczyx, meta=None):
-        sep = (meta or self.array_meta(path)).get("dimension_separator") or "."
-        key = sep.join(str(int(i)) for i in idx_tczyx)
+        m = meta or self.array_meta(path)
+        sep = m.get("dimension_separator") or "."
+        # a 3-D (z, y, x) array takes the spatial part of the (t, c, z, y, x) index
+        key = sep.join(str(int(i)) for i in tuple(idx_tczyx)[-len(m["shape"]):])
         return os.path.join(self.root, path.strip("/"), *key.split("/"))
 
     def write_chunk(self, path, idx_tczyx, block_zyx: np.ndarray):
         """block_zyx: the valid [z,y,x] part of one chunk; padded to the full chunk shape.  A full chunk already in
         the array's byte order is written as it is."""
         m = self.array_meta(path)
-        cz, cy, cx = m["chunks"][2:]
+        cz, cy, cx = m["chunks"][-3:]
         sdt = np.dtype(m["dtype"])
         if block_zyx.shape == (cz, cy, cx) and block_zyx.dtype == sdt and block_zyx.flags["C_CONTIGUOUS"]:
             payload = block_zyx.tobytes()
@@ -133,7 +145,7 @@ class ZarrStore:
         if m.get("order", "C") != "C":
             raise NotImplementedError(f"Zarr order {m['order']!r} of {path}")
         p = self._chunk_path(path, idx_tczyx, m)
-        cz, cy, cx = m["chunks"][2:]
+        cz, cy, cx = m["chunks"][-3:]
         dt = _np_dtype(m)
         if not os.path.exists(p):
             return np.full((cz, cy, cx), m.get("fill_value") or 0, dtype=dt)
@@ -146,8 +158,8 @@ class ZarrStore:
         [z,y,x] super-block into chunks starting at chunk index {gx,gy,gz} of channel c, timepoint t."""
         m = self.array_meta(path)
         gx, gy, gz, c, t = (int(v) for v in grid_offset_xyzct)
-        sz, sy, sx = m["shape"][2:]
-        cz, cy, cx = m["chunks"][2:]
+        sz, sy, sx = m["shape"][-3:]
+        cz, cy, cx = m["chunks"][-3:]
         vz, vy, vx = volume_zyx.shape
         for kz in range(-(-vz // cz)):
             for ky in range(-(-vy // cy)):
@@ -162,8 +174,8 @@ class ZarrStore:
     def read_region(self, path, min_xyz, size_xyz, c=0, t=0):
         """[z, y, x] array of the interval [min, min + size) of channel c / timepoint t (zero outside the array)."""
         m = self.array_meta(path)
-        sz, sy, sx = m["shape"][2:]
-        cz, cy, cx = m["chunks"][2:]
+        sz, sy, sx = m["shape"][-3:]
+        cz, cy, cx = m["chunks"][-3:]
         mn = [int(v) for v in min_xyz]
         n = [int(v) for v in size_xyz]
         out = np.zeros(n[::-1], dtype=_np_dtype(m))
@@ -184,8 +196,8 @@ class ZarrStore:
 
     def read_volume(self, path, c=0, t=0):
         m = self.array_meta(path)
-        sz, sy, sx = m["shape"][2:]
-        cz, cy, cx = m["chunks"][2:]
+        sz, sy, sx = m["shape"][-3:]
+        cz, cy, cx = m["chunks"][-3:]
         out = np.zeros((sz, sy, sx), dtype=_np_dtype(m))
         for iz in range(-(-sz // cz)):
             for iy in range(-(-sy // cy)):
