@@ -16,6 +16,7 @@
   clear_interestpoints    J/ClearInterestPoints.java              (points + correspondences, or correspondences only)
   clear_registrations     J/ClearRegistrations.java               (drop the latest <ViewTransform>s)
   transform_points        J/TransformPoints.java                  (view pixel coordinates -> world, host only)
+  split_images            J/SplitDatasets.java                    (overlapping sub-views, split loader, fake points)
 
 Every command reads its images through viewsource.py, so `bdv.n5` and `bdv.multimg.zarr` datasets both work.
 
@@ -36,7 +37,7 @@ from . import n5 as bn5
 from . import zarr as bzarr
 from . import matching as bm
 from . import intensity as bint
-from . import native, solver as bsolver, stitching as bst, viewsource as bvs
+from . import native, solver as bsolver, split as bsplit, stitching as bst, viewsource as bvs
 from .native import Context
 from .spimdata import SpimData2, fusion_project
 
@@ -1694,3 +1695,140 @@ def transform_points(xml_path, view, points=None, csv_in=None, csv_out=None):
         with open(csv_out, "w") as f:
             f.writelines(line + "\n" for line in lines)
     return W
+
+
+# --------------------------------------------------------------------------------------------- split-images
+def _ip_base(xml_path, data):
+    return os.path.join(os.path.dirname(os.path.abspath(xml_path)), data.root.findtext("BasePath") or ".")
+
+
+def _read_view_points(store, group):
+    """(ids int64 (n,), loc float64 (n, 3), intensities float32 (n,) or None) of one label group of interestpoints.n5."""
+    if store is None or "dimensions" not in store.get_attributes(group + "/interestpoints/loc"):
+        return np.zeros(0, dtype=np.int64), np.zeros((0, 3)), None
+    ids = store.read_list(group + "/interestpoints/id").reshape(-1).astype(np.int64)
+    loc = store.read_list(group + "/interestpoints/loc").astype(np.float64).reshape(-1, 3)
+    inten = None
+    if "dimensions" in store.get_attributes(group + "/intensities"):
+        inten = store.read_list(group + "/intensities").reshape(-1).astype(np.float32)
+    return ids, loc, inten
+
+
+def _write_view_points(store, group, ids, loc, inten=None):
+    shutil.rmtree(os.path.join(store.root, group), ignore_errors=True)     # no stale correspondences under it
+    store.set_attributes(group + "/interestpoints", IP_N5_GROUP_ATTRIBUTES)
+    store.write_list(group + "/interestpoints/id", np.asarray(ids, dtype=np.uint64).reshape(-1, 1), IP_N5_BLOCK_LENGTH, "zstd")
+    store.write_list(group + "/interestpoints/loc", np.asarray(loc, dtype=np.float64).reshape(-1, 3), IP_N5_BLOCK_LENGTH,
+                     "zstd")
+    if inten is not None:
+        store.write_list(group + "/intensities", np.asarray(inten, dtype=np.float32).reshape(-1, 1), IP_N5_BLOCK_LENGTH,
+                         "zstd")
+
+
+def split_images(xml_path, target_image_size, target_overlap, xml_out=None, disable_optimization=False,
+                 fake_interest_points=False, fip_density=100.0, fip_min_num_points=20, fip_max_num_points=500,
+                 fip_error=0.5, fip_exclusion_radius=20.0, fip_label="splitPoints", assign_illuminations=False,
+                 display_result=False, dry_run=False):
+    """`./split-images -x dataset.xml -tis 512,512,256 -to 32,32,32 [-xo out.xml] [--disableOptimization] [-fip
+    [--fipDensity 100] [--fipMinNumPoints 20] [--fipMaxNumPoints 500] [--fipError 0.5] [--fipExclusionRadius 20]]
+    [--assignIlluminations] [--dryRun]` (J/SplitDatasets.java:74-168): cut every view into overlapping sub-views so
+    that match-interestpoints + solver can give each piece its own model, and write the project of the pieces to
+    ``xml_out`` (default: the input, with a ~1 backup).  Sizes are "x,y,z" strings or triples.
+
+    The target size and overlap are rounded up to multiples of the step m, per axis the lcm of every view's mipmap
+    factors; an overlap larger than the size, or equal to it on an axis that has to be split, raises ValueError.  The
+    boxes and the new project follow split.intervals / split.split_project.  The new views are read through a
+    `split.viewerimgloader` wrapping the input's loader (viewsource.SplitViews), so every command reads them.
+
+    Interest points carry over: each sub-view gets, per label of its parent, the points inside its closed box shifted
+    by -min, ids and intensities kept, written to interestpoints.n5 next to ``xml_out``; correspondences are dropped
+    (re-run matching).  ``fake_interest_points`` (`-fip`) adds split.fake_points between overlapping sub-views of one
+    view, with their correspondences, as label ``fip_label``, which must not exist yet (ValueError).
+
+    ``display_result`` (a GUI) raises NotImplementedError; ``dry_run`` returns the plan and writes nothing.  Returns
+    dict(step=m, size=s, overlap=o, views={new setup: (old setup, min xyz, max xyz)}, fake_points={(tp, new a, new b):
+    count})."""
+    if display_result:
+        raise NotImplementedError("split-images --displayResult (the BigStitcher GUI) is not available")
+    size = bsplit.parse_size(target_image_size, "targetImageSize")
+    overlap = bsplit.parse_size(target_overlap, "targetOverlap")
+    data = SpimData2.load(xml_path)
+    src = bvs.open_views(data)
+    missing = data.missing_views()
+    present = [v for v in data.view_ids() if v not in missing]
+    m = bsplit.min_step(src, present)
+    s = tuple(bsplit.closest_larger_divisible(size[d], m[d]) for d in range(3))
+    o = tuple(bsplit.closest_larger_divisible(overlap[d], m[d]) for d in range(3))
+    if any(o[d] > s[d] for d in range(3)):
+        raise ValueError(f"overlap {o} cannot be bigger than size {s}.")
+    plan, boxes_of = {}, {}
+    for old in sorted(data.setups):
+        boxes_of[old] = bsplit.boxes(data.setups[old].size, s, o, m, not disable_optimization)
+        for k, (mn, mx) in enumerate(boxes_of[old]):
+            plan[len(plan)] = (old, mn, mx, k)
+    new_of = {(p[0], p[3]): nid for nid, p in plan.items()}
+    xml_out = xml_out or xml_path
+    new = bsplit.split_project(data, plan, assign_illuminations, xml_out)
+
+    # ---- every parent's points are read before anything is written: new setup ids reuse old ones
+    ips = data.interest_points()
+    if fake_interest_points and any(fip_label in labels for labels in ips.values()):
+        raise ValueError(f"interest point label '{fip_label}' already exists; choose another --fipLabel")
+    root_in = os.path.join(_ip_base(xml_path, data), "interestpoints.n5")
+    store_in = bn5.N5Store(root_in) if os.path.isdir(root_in) else None
+    parent_points = {}                        # (tp, old) -> {label: (ids, loc, intensities, params)}
+    for v, labels in sorted(ips.items()):
+        if v in missing:
+            continue
+        parent_points[v] = {lab: _read_view_points(store_in, e["path"].rstrip("/")) + (e["params"],)
+                            for lab, e in sorted(labels.items())}
+
+    carried = {}                              # (label, params) -> {new view: (group, ids, loc, intensities)}
+    for (tp, old), labels in parent_points.items():
+        for k, (mn, mx) in enumerate(boxes_of[old]):
+            nv = (tp, new_of[(old, k)])
+            for lab, (ids, loc, inten, params) in labels.items():
+                inside = np.all((loc >= mn) & (loc <= mx), axis=1)
+                carried.setdefault((lab, params), {})[nv] = (
+                    f"tpId_{tp}_viewSetupId_{nv[1]}/{lab}", ids[inside], loc[inside] - mn,
+                    None if inten is None else inten[inside])
+
+    fakes_out, fake_counts, fake_results = {}, {}, {}
+    if fake_interest_points:
+        for (tp, old) in present:
+            labels = parent_points.get((tp, old), {})
+            existing = np.concatenate([p[1] for p in labels.values()]) if labels else np.zeros((0, 3))
+            fakes, pairs = bsplit.fake_points(tp, old, boxes_of[old], existing, fip_density, fip_min_num_points,
+                                              fip_max_num_points, fip_error, fip_exclusion_radius)
+            for i, pts in fakes.items():
+                fakes_out[(tp, new_of[(old, i)])] = pts - boxes_of[old][i][0]
+            for (i, j), got in pairs.items():
+                va, vb = (tp, new_of[(old, i)]), (tp, new_of[(old, j)])
+                fake_counts[(tp, va[1], vb[1])] = len(got)
+                fake_results[(va, fip_label, vb, fip_label)] = np.asarray(got, dtype=np.int64).reshape(-1, 2)
+
+    result = dict(step=m, size=s, overlap=o, views={nid: (p[0], tuple(int(v) for v in p[1]), tuple(int(v) for v in p[2]))
+                                                    for nid, p in plan.items()}, fake_points=fake_counts)
+    if dry_run:
+        return result
+
+    if carried or fakes_out:
+        store = bn5.N5Store(os.path.join(_ip_base(xml_out, new), "interestpoints.n5"), create=True)
+        for (lab, params), views in sorted(carried.items()):
+            for group, ids, loc, inten in views.values():
+                _write_view_points(store, group, ids, loc, inten)
+            new.set_interest_points(lab, params, {v: g[0] for v, g in views.items()})
+        if fakes_out:
+            groups = {}
+            for v, pts in sorted(fakes_out.items()):
+                groups[v] = f"tpId_{v[0]}_viewSetupId_{v[1]}/{fip_label}"
+                _write_view_points(store, groups[v], np.arange(len(pts)), pts)
+            holder = type("FakePoints", (), dict(world={(v, fip_label): None for v in groups}, corr={}))
+            write_match_correspondences(store, holder, sorted(groups), [fip_label], fake_results, clear=True)
+            new.set_interest_points(fip_label, (
+                f"Fake points for image splitting: density={_java(float(fip_density))}, "
+                f"minPoints={int(fip_min_num_points)}, maxPoints={int(fip_max_num_points)}, error={_java(float(fip_error))}, "
+                f"excludeRadius={_java(float(fip_exclusion_radius))}"), groups)
+    os.makedirs(os.path.dirname(os.path.abspath(xml_out)), exist_ok=True)
+    new.save(xml_out)
+    return result

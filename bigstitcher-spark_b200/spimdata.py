@@ -6,7 +6,9 @@ extensions) -- the fields the two hot paths consume and produce:
   * ViewRegistrations: ordered <ViewTransform type="affine"> lists; list index 0 is applied LAST
     (J/ClearRegistrations.java:80-99), so model = T0 * T1 * ... * Tn
   * ImageLoader format="bdv.n5" path (J/SparkResaveN5.java:424-433), or format="bdv.multimg.zarr" (AllenOMEZarrLoader,
-    :434-445): the container root plus one <zgroup> per view with its group path and (channel, timepoint) indices
+    :434-445): the container root plus one <zgroup> per view with its group path and (channel, timepoint) indices,
+    or format="split.viewerimgloader" (split-images): one of those loaders plus the box of an old setup per new setup
+  * <MissingViews> and the <Attributes> entries of <ViewSetups> (tile names and locations, illuminations)
   * <StitchingResults><PairwiseResult view_setup_a/b tp_a/b> shift (12 doubles), correlation, hash,
     overlap_boundingbox (6 doubles)                                   (J/SparkPairwiseStitching.java:284-301,328-390)
   * <ViewInterestPoints><ViewInterestPointsFile timepoint setup label params>path of the label's group in
@@ -18,12 +20,15 @@ Host-side plumbing only.  Everything else in the file is preserved verbatim on s
 """
 from __future__ import annotations
 
+import copy
 import os
 import shutil
 import xml.etree.ElementTree as ET
 from dataclasses import dataclass, field
 
 import numpy as np
+
+SPLIT_LOADER = "split.viewerimgloader"
 
 
 @dataclass
@@ -74,21 +79,33 @@ class SpimData2:
             tps.add(tp)
         self.timepoints = sorted(tps)
 
-    def image_loader(self):
-        """(format, absolute container path) of the ImageLoader element."""
+    def _loader_element(self, nested=False):
         il = self.root.find("SequenceDescription").find("ImageLoader")
+        return il.find("ImageLoader") if nested else il
+
+    @staticmethod
+    def _container_node(il):
+        for tag in ("n5", "zarr", "hdf5"):
+            if il.find(tag) is not None:
+                return il.find(tag)
+        return None
+
+    def image_loader(self, nested=False):
+        """(format, absolute container path) of the ImageLoader element; ``nested``: of the loader a
+        `split.viewerimgloader` wraps."""
+        il = self._loader_element(nested)
         fmt = il.get("format")
-        node = il.find("n5") if il.find("n5") is not None else (il.find("zarr") if il.find("zarr") is not None else il.find("hdf5"))
+        node = self._container_node(il)
         p = node.text.strip() if node is not None else None
         if p is not None and node.get("type", "relative") == "relative" and self.path:
             base = self.root.findtext("BasePath") or "."
             p = os.path.normpath(os.path.join(os.path.dirname(os.path.abspath(self.path)), base, p))
         return fmt, p
 
-    def zarr_groups(self):
+    def zarr_groups(self, nested=False):
         """The views of a `bdv.multimg.zarr` loader: {(tp, setup): (group path, channel index, timepoint index)}.
         Element and attribute names are recalled from XmlIoAllenOMEZarrLoader (PARITY_GAPS R1)."""
-        il = self.root.find("SequenceDescription").find("ImageLoader")
+        il = self._loader_element(nested)
         out = {}
         zg = il.find("zgroups")
         for g in (zg.findall("zgroup") if zg is not None else []):
@@ -118,6 +135,92 @@ class SpimData2:
         seq.insert(list(seq).index(old) if old is not None else 0, il)
         if old is not None:
             seq.remove(old)
+
+    # ------------------------------------------------------------------ split image loader (split-images)
+    def split_setups(self):
+        """The sub-views of a `split.viewerimgloader`: {new setup: (old setup, min int64[3], max int64[3])}, the box
+        inclusive, in pixels of the old setup; {} for any other loader.  Element names are recalled from
+        XmlIoSplitViewerImgLoader (PARITY_GAPS P4)."""
+        il = self._loader_element()
+        if il.get("format") != SPLIT_LOADER:
+            return {}
+        out = {}
+        for d in il.find("SetupIds").findall("SetupIdDefinition"):
+            box = [np.array([int(v) for v in d.findtext(k).split()], dtype=np.int64) for k in ("min", "max")]
+            out[int(d.findtext("NewId"))] = (int(d.findtext("OldId")), box[0], box[1])
+        return out
+
+    def set_split_image_loader(self, nested, container, definitions, xml_path=None):
+        """Replace the ImageLoader by a `split.viewerimgloader` wrapping a copy of ``nested`` (a `bdv.n5` or
+        `bdv.multimg.zarr` <ImageLoader> element whose container lies at the absolute path ``container``); a relative
+        container path is re-based onto the BasePath of the XML at ``xml_path`` (default: where this one was loaded
+        from).  ``definitions``: {new setup: (old setup, min xyz, max xyz)}, old setups being those of the nested
+        loader."""
+        inner = copy.deepcopy(nested)
+        node = self._container_node(inner)
+        if node is not None and node.get("type", "relative") == "relative":
+            node.text = self._loader_path(container, xml_path)
+        seq = self.root.find("SequenceDescription")
+        old = seq.find("ImageLoader")
+        il = ET.Element("ImageLoader", format=SPLIT_LOADER)
+        il.append(inner)
+        ids = ET.SubElement(il, "SetupIds")
+        for new, (o, mn, mx) in sorted(definitions.items()):
+            d = ET.SubElement(ids, "SetupIdDefinition")
+            ET.SubElement(d, "NewId").text = str(int(new))
+            ET.SubElement(d, "OldId").text = str(int(o))
+            ET.SubElement(d, "min").text = " ".join(str(int(v)) for v in mn)
+            ET.SubElement(d, "max").text = " ".join(str(int(v)) for v in mx)
+        seq.insert(list(seq).index(old) if old is not None else 0, il)
+        if old is not None:
+            seq.remove(old)
+
+    # ------------------------------------------------------------------ missing views, attribute entries
+    def missing_views(self):
+        """The (tp, setup) of every <MissingViews><View>."""
+        mv = self.root.find("SequenceDescription").find("MissingViews")
+        return {(int(v.get("timepoint")), int(v.get("setup"))) for v in (mv.findall("View") if mv is not None else [])}
+
+    def set_missing_views(self, views):
+        seq = self.root.find("SequenceDescription")
+        mv = seq.find("MissingViews")
+        if mv is None:
+            mv = ET.SubElement(seq, "MissingViews")
+        for v in list(mv):
+            mv.remove(v)
+        for tp, setup in sorted(views):
+            ET.SubElement(mv, "View", timepoint=str(int(tp)), setup=str(int(setup)))
+
+    def attribute_entries(self, name):
+        """{id: dict(name=str, location=float64[3] or None)} of <ViewSetups><Attributes name=``name``>; None when the
+        element is absent."""
+        for a in self.root.find("SequenceDescription").find("ViewSetups").findall("Attributes"):
+            if a.get("name") == name:
+                out = {}
+                for e in a:
+                    loc = e.findtext("location")
+                    out[int(e.findtext("id"))] = dict(name=e.findtext("name"),
+                                                      location=None if loc is None else np.array([float(v) for v in loc.split()]))
+                return out
+        return None
+
+    def set_attribute_entries(self, name, entries):
+        """Rebuild <Attributes name=``name``> from {id: dict(name=, location=)} (entries in id order)."""
+        vss = self.root.find("SequenceDescription").find("ViewSetups")
+        old = next((a for a in vss.findall("Attributes") if a.get("name") == name), None)
+        a = ET.Element("Attributes", name=name)
+        for i, e in sorted(entries.items()):
+            el = ET.SubElement(a, name.capitalize())
+            ET.SubElement(el, "id").text = str(int(i))
+            if e.get("name") is not None:
+                ET.SubElement(el, "name").text = str(e["name"])
+            if e.get("location") is not None:
+                ET.SubElement(el, "location").text = _fmt(e["location"])
+        if old is not None:
+            vss.insert(list(vss).index(old), a)
+            vss.remove(old)
+        else:
+            vss.append(a)
 
     def save(self, path: str | None = None, backup: bool = True):
         path = path or self.path

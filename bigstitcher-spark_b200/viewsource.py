@@ -8,12 +8,16 @@ levels of every view.  Two loaders are read (Import / the BDV image loaders the 
     from the levels' `scale` transformations (zarr.read_multiscales).
 
 Mipmap transforms follow the half-pixel convention of MipmapTransforms.getMipmapTransformDefault for both
-(zarr.mipmap_transform_default).  Any other loader raises NotImplementedError.  Host-side plumbing only.
+(zarr.mipmap_transform_default).  A `split.viewerimgloader` (split-images) wraps either of them: its views are boxes
+of the wrapped views (SplitViews).  Any other loader raises NotImplementedError.  Host-side plumbing only.
 """
 from __future__ import annotations
 
+import numpy as np
+
 from . import n5 as bn5
 from . import zarr as bzarr
+from .spimdata import SPLIT_LOADER
 
 
 def open_views(data):
@@ -23,6 +27,12 @@ def open_views(data):
         return N5Views(path)
     if fmt == "bdv.multimg.zarr":
         return ZarrViews(path, data.zarr_groups())
+    if fmt == SPLIT_LOADER:
+        fmt, path = data.image_loader(nested=True)
+        if fmt == "bdv.n5":
+            return SplitViews(N5Views(path), data.split_setups())
+        if fmt == "bdv.multimg.zarr":
+            return SplitViews(ZarrViews(path, data.zarr_groups(nested=True)), data.split_setups())
     raise NotImplementedError(f"ImageLoader format {fmt}")
 
 
@@ -89,3 +99,58 @@ class ZarrViews:
     def read_region(self, view, level, min_xyz, size_xyz):
         (_, c, t), levels = self._view(view)
         return self.store.read_region(levels[level]["path"], min_xyz, size_xyz, c, t)
+
+
+class SplitViews:
+    """The sub-views split-images defines (`split.viewerimgloader`): view (tp, new setup) is the box [min, max] of view
+    (tp, old setup) of the wrapped N5Views / ZarrViews.  Level l with factors f is the parent's level-l window from
+    min / f to min(floor(max / f), parent dims - 1); min is a multiple of every factor, so the parent's half-pixel
+    mipmap transforms stay exact.  Voxels outside the window read as zero, like those outside a dataset."""
+    format = SPLIT_LOADER
+
+    def __init__(self, inner, definitions):
+        self.inner = inner
+        self.store = inner.store
+        self.definitions = definitions           # {new setup: (old setup, min xyz, max xyz)}
+
+    def _parent(self, view):
+        old, _, _ = self.definitions[int(view[1])]
+        return (int(view[0]), old)
+
+    def _window(self, view, level):
+        """(parent view, window min, window size) of a level."""
+        old, mn, mx = self.definitions[int(view[1])]
+        parent = (int(view[0]), old)
+        f = self.inner.mipmap_info(parent)[0][level]
+        pdims = self.inner.level_dims(parent, level)
+        lo = [int(mn[d]) // int(f[d]) for d in range(3)]
+        hi = [min(int(mx[d]) // int(f[d]), int(pdims[d]) - 1) for d in range(3)]
+        return parent, lo, [hi[d] - lo[d] + 1 for d in range(3)]
+
+    def mipmap_info(self, view):
+        return self.inner.mipmap_info(self._parent(view))
+
+    def level_dims(self, view, level):
+        return tuple(self._window(view, level)[2])
+
+    def level_dtype(self, view, level) -> str:
+        return self.inner.level_dtype(self._parent(view), level)
+
+    def read_volume(self, view, level=0):
+        parent, lo, size = self._window(view, level)
+        return self.inner.read_region(parent, level, lo, size)
+
+    def read_region(self, view, level, min_xyz, size_xyz):
+        parent, lo, dims = self._window(view, level)
+        mn = [int(v) for v in min_xyz]
+        sz = [int(v) for v in size_xyz]
+        a = [max(mn[d], 0) for d in range(3)]                       # the part inside the sub-view
+        b = [min(mn[d] + sz[d], dims[d]) for d in range(3)]
+        if any(b[d] <= a[d] for d in range(3)):
+            return np.zeros(sz[::-1], dtype=self.level_dtype(view, level))
+        part = self.inner.read_region(parent, level, [lo[d] + a[d] for d in range(3)], [b[d] - a[d] for d in range(3)])
+        if a == mn and b == [mn[d] + sz[d] for d in range(3)]:
+            return part
+        out = np.zeros(sz[::-1], dtype=part.dtype)
+        out[a[2] - mn[2]:b[2] - mn[2], a[1] - mn[1]:b[1] - mn[1], a[0] - mn[0]:b[0] - mn[0]] = part
+        return out
