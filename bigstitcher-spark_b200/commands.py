@@ -1011,18 +1011,47 @@ def _nonrigid_chunk(ctx, src, chunk, bb_min, fuse, nviews, vdims, params, cpd):
 
 
 # --------------------------------------------------------------------------------------------- match-interestpoints
-def match_pairs(view_dims, registrations, view_ids, view_reg="OVERLAPPING_ONLY"):
-    """M2: the view pairs (A, B) of one timepoint, A < B in (tp, setup) order; OVERLAPPING_ONLY keeps the pairs whose
-    closed transformed bounding boxes intersect, ALL_AGAINST_ALL keeps every pair."""
+# -rtp / --registrationTP: which timepoints are registered against each other (J/abstractcmdline/AbstractRegistration.java)
+REGISTRATION_TPS = ("TIMEPOINTS_INDIVIDUALLY", "TO_REFERENCE_TIMEPOINT", "ALL_TO_ALL", "ALL_TO_ALL_WITH_RANGE")
+
+
+def reference_timepoint(view_ids, reference_tp=None):
+    """--referenceTP (J/abstractcmdline/AbstractRegistration.java:95-104): the timepoint of the first view in (tp, setup)
+    order by default; a given timepoint must be the timepoint of one of ``view_ids``."""
+    views = sorted(view_ids)
+    if reference_tp is None:
+        return int(views[0][0])
+    if int(reference_tp) not in {v[0] for v in views}:
+        raise ValueError("Specified reference timepoint is not part of the ViewIds that are processed.")
+    return int(reference_tp)
+
+
+def match_pairs(view_dims, registrations, view_ids, view_reg="OVERLAPPING_ONLY", registration_tp="TIMEPOINTS_INDIVIDUALLY",
+                reference_tp=None, range_tp=5):
+    """M2, M10: the view pairs (A, B), A < B in (tp, setup) order, that the -rtp constellation forms:
+    TIMEPOINTS_INDIVIDUALLY pairs views of one timepoint, ALL_TO_ALL every two views, ALL_TO_ALL_WITH_RANGE views whose
+    timepoint ids are at most ``range_tp`` apart, TO_REFERENCE_TIMEPOINT the pairs with at least one view at
+    ``reference_tp`` (default: the first view's timepoint).  Then OVERLAPPING_ONLY keeps the pairs whose closed
+    transformed bounding boxes (each view under its own registration) intersect, ALL_AGAINST_ALL keeps every pair."""
     vr = view_reg.upper()
     if vr not in ("OVERLAPPING_ONLY", "ALL_AGAINST_ALL"):
         raise ValueError(f"-vr {view_reg}")
+    rtp = registration_tp.upper()
+    if rtp not in REGISTRATION_TPS:
+        raise NotImplementedError(f"-rtp {registration_tp} is not implemented")
+    if int(range_tp) < 0:
+        raise ValueError(f"--rangeTP {range_tp}: the range must not be negative")
     views = sorted(view_ids)
+    ref = reference_timepoint(views, reference_tp) if views else None
+    formed = {"TIMEPOINTS_INDIVIDUALLY": lambda ta, tb: ta == tb,
+              "ALL_TO_ALL": lambda ta, tb: True,
+              "ALL_TO_ALL_WITH_RANGE": lambda ta, tb: abs(ta - tb) <= int(range_tp),
+              "TO_REFERENCE_TIMEPOINT": lambda ta, tb: ref in (ta, tb)}[rtp]
     boxes = {v: bf.transformed_bounding_box(view_dims[v], registrations[v]) for v in views}
     pairs = []
     for i, a in enumerate(views):
         for b in views[i + 1:]:
-            if a[0] != b[0]:
+            if not formed(a[0], b[0]):
                 continue
             if vr == "ALL_AGAINST_ALL" or np.all(np.minimum(boxes[a][1], boxes[b][1]) >= np.maximum(boxes[a][0], boxes[b][0])):
                 pairs.append((a, b))
@@ -1094,19 +1123,22 @@ def match_interestpoints(xml_path, ctx: Context, labels, method, significance=3.
                          ransac_max_error=None, ransac_min_inlier_ratio=0.1, ransac_min_num_inliers=12,
                          ransac_multi_consensus=False, registration_tp="TIMEPOINTS_INDIVIDUALLY", group_tiles=False,
                          group_illums=False, group_channels=False, split_timepoints=False, view_selection=None,
-                         dry_run=False, shard=(0, 1), allgather=None):
+                         dry_run=False, shard=(0, 1), allgather=None, reference_tp=None, range_tp=5):
     """`./match-interestpoints -x dataset.xml -l beads -m PRECISE_TRANSLATION [-s 3.0] [-r 1] [-n 3] [--searchRadius r]
     [--clearCorrespondences] [--matchAcrossLabels] [-ipfr ALL|OVERLAPPING_ONLY] [-vr OVERLAPPING_ONLY|ALL_AGAINST_ALL]
-    [-tm AFFINE] [-rm RIGID] [--lambda 0.1] [-rit 10000] [-rme 5.0] [-rmir 0.1] [-rmni 12]`, the non-grouped branch of
-    J/SparkGeometricDescriptorMatching.java:161-342 and the save at :512-545: for every task (view pair x label pair)
-    the points are read from interestpoints.n5 and mapped to world (M1), optionally filtered to the partner's box (M3);
+    [-tm AFFINE] [-rm RIGID] [--lambda 0.1] [-rit 10000] [-rme 5.0] [-rmir 0.1] [-rmni 12]
+    [-rtp TIMEPOINTS_INDIVIDUALLY|TO_REFERENCE_TIMEPOINT|ALL_TO_ALL|ALL_TO_ALL_WITH_RANGE] [--referenceTP t]
+    [--rangeTP 5]`, the non-grouped branch of J/SparkGeometricDescriptorMatching.java:161-342 and the save at :512-545:
+    the view pairs are those of the -rtp constellation (``match_pairs``; across timepoints for every name but
+    TIMEPOINTS_INDIVIDUALLY); for every task (view pair x label pair) the points are read from interestpoints.n5 and
+    mapped to world (M1), optionally filtered to the partner's box (M3);
     descriptors and the exhaustive A -> B search run on the device (bs_descriptors_build / bs_descriptors_match), the
     ratio test (M6), RANSAC and its filter (M7, M8) on the host; the inliers become correspondences of both views (M9),
     written for every selected view x label unless ``dry_run``.  The XML is not touched.
     Returns {(viewA, labelA, viewB, labelB): int64 (K, 2) id pairs} for every task.
 
     Multi-GPU: rank r of w (``shard``) takes tasks[r::w]; ``allgather(obj) -> [obj of every rank]`` merges the results
-    and rank 0 writes.  FAST_ROTATION, FAST_TRANSLATION, ICP, grouping, -rtp other than TIMEPOINTS_INDIVIDUALLY and
+    and rank 0 writes.  FAST_ROTATION, FAST_TRANSLATION, ICP, grouping, an -rtp name other than the four above and
     -rmc raise NotImplementedError."""
     m = method.upper()
     if m in ("FAST_ROTATION", "FAST_TRANSLATION", "ICP"):
@@ -1115,7 +1147,7 @@ def match_interestpoints(xml_path, ctx: Context, labels, method, significance=3.
         raise ValueError(f"-m {method}")
     for flag, on in (("--groupTiles", group_tiles), ("--groupIllums", group_illums), ("--groupChannels", group_channels),
                      ("--splitTimepoints", split_timepoints), ("-rmc", ransac_multi_consensus),
-                     (f"-rtp {registration_tp}", registration_tp.upper() != "TIMEPOINTS_INDIVIDUALLY")):
+                     (f"-rtp {registration_tp}", registration_tp.upper() not in REGISTRATION_TPS)):
         if on:
             raise NotImplementedError(f"match-interestpoints {flag} is not implemented")
     ipfr = interestpoints_for_reg.upper()
@@ -1139,7 +1171,8 @@ def match_interestpoints(xml_path, ctx: Context, labels, method, significance=3.
     views = sorted(data.select_views(**view_selection) if view_selection else data.view_ids())
     regs = {v: data.model(*v) for v in views}
     vdims = {v: tuple(int(d) for d in data.setups[v[1]].size) for v in views}
-    tasks = match_tasks(match_pairs(vdims, regs, views, view_reg), labels, match_across_labels)
+    tasks = match_tasks(match_pairs(vdims, regs, views, view_reg, registration_tp, reference_tp, range_tp), labels,
+                        match_across_labels)
     base = os.path.join(os.path.dirname(os.path.abspath(xml_path)), data.root.findtext("BasePath") or ".")
     store = bn5.N5Store(os.path.join(base, "interestpoints.n5"))
     ips = _MatchPoints(store, views, labels, regs)
@@ -1185,22 +1218,24 @@ def solver(xml_path, ctx: Context, source, labels=None, label_weights=None, meth
            transformation_model="AFFINE", regularization_model="RIGID", regularization_lambda=0.1, max_error=5.0,
            max_iterations=10000, max_plateau_width=200, relative_threshold=3.5, absolute_threshold=7.0, fixed_views=None,
            disable_fixed_views=False, group_tiles=None, group_illums=None, group_channels=None, split_timepoints=None,
-           registration_tp="TIMEPOINTS_INDIVIDUALLY", view_selection=None, dry_run=False):
+           registration_tp="TIMEPOINTS_INDIVIDUALLY", view_selection=None, dry_run=False, reference_tp=None):
     """`./solver -x dataset.xml -s STITCHING|IP [-l beads [-lw 1.0]] [--method ONE_ROUND_SIMPLE|ONE_ROUND_ITERATIVE]
     [-tm AFFINE] [-rm RIGID] [--lambda 0.1] [--maxError 5.0] [--maxIterations 10000] [--maxPlateauwidth 200]
     [--relativeThreshold 3.5] [--absoluteThreshold 7.0] [-fv 'tp,setup' | --disableFixedViews] [--groupTiles]
-    [--groupIllums] [--groupChannels] [--splitTimepoints] [--dryRun]` (J/Solver.java:161-432): global optimisation of
-    the stored stitching results or interest-point correspondences.  The matches are built and the tiles pre-aligned on
-    the host; the relaxation runs on the device (bs_solve_tiles).  Every view of a solved tile gets the tile's model as
+    [--groupIllums] [--groupChannels] [--splitTimepoints]
+    [-rtp TIMEPOINTS_INDIVIDUALLY|TO_REFERENCE_TIMEPOINT|ALL_TO_ALL|ALL_TO_ALL_WITH_RANGE] [--referenceTP t] [--dryRun]`
+    (J/Solver.java:161-432): global optimisation of the stored stitching results or interest-point correspondences.
+    The matches are built and the tiles pre-aligned on the host; the relaxation runs on the device (bs_solve_tiles).  Every view of a solved tile gets the tile's model as
     a new first <ViewTransform>; the XML is saved (with a ~1 backup) unless ``dry_run``.  Returns dict(models={view:
     3 x 4}, removed=[(views A, views B)] (ONE_ROUND_ITERATIVE), stats) -- stats holds iterations, the final error,
-    skipped fits, stale stitching results and the views without links, which keep their registration.
+    skipped fits, stale stitching results and the views without links, which keep their registration.  -rtp only
+    chooses the automatic fixed views (``solver.fixed_views_auto``); every stored link between selected views is used.
 
-    TWO_ROUND_SIMPLE / TWO_ROUND_ITERATIVE and -rtp other than TIMEPOINTS_INDIVIDUALLY raise NotImplementedError."""
+    TWO_ROUND_SIMPLE / TWO_ROUND_ITERATIVE and an -rtp name other than the four above raise NotImplementedError."""
     return bsolver.run(xml_path, ctx, source, labels, label_weights, method, transformation_model, regularization_model,
                        regularization_lambda, max_error, max_iterations, max_plateau_width, relative_threshold,
                        absolute_threshold, fixed_views, disable_fixed_views, group_tiles, group_illums, group_channels,
-                       split_timepoints, registration_tp, view_selection, dry_run)
+                       split_timepoints, registration_tp, view_selection, dry_run, reference_tp)
 
 
 # --------------------------------------------------------------------------------------------- resave

@@ -56,6 +56,20 @@ def tile_keys(data: SpimData2, views, group_tiles=False, group_illums=False, gro
     return keys
 
 
+def fixed_views_auto(views, registration_tp="TIMEPOINTS_INDIVIDUALLY", reference_tp=None):
+    """The fixed views when neither -fv nor --disableFixedViews is given (assembleFixedAuto, J/Solver.java:674-717), out
+    of the views in (tp, setup) order: TIMEPOINTS_INDIVIDUALLY fixes the first view of every timepoint,
+    TO_REFERENCE_TIMEPOINT only the first view at ``reference_tp``, ALL_TO_ALL and ALL_TO_ALL_WITH_RANGE only the first
+    view."""
+    rtp = registration_tp.upper()
+    if rtp == "TIMEPOINTS_INDIVIDUALLY":
+        return {min(v for v in views if v[0] == tp) for tp in sorted({v[0] for v in views})}
+    if rtp == "TO_REFERENCE_TIMEPOINT":
+        at_ref = [v for v in views if v[0] == reference_tp]
+        return {min(at_ref)} if at_ref else set()
+    return {min(views)}
+
+
 def stitching_matches(data: SpimData2, tile_of, views):
     """Matches of the stored stitching results (J/Solver.java:398-432): results whose hash differs from the hash of the
     first views' current registrations are stale and dropped; every other result (A, B, R, r, overlap box) gives the 8
@@ -280,15 +294,16 @@ def run(xml_path, ctx, source, labels=None, label_weights=None, method="ONE_ROUN
         regularization_model="RIGID", regularization_lambda=0.1, max_error=5.0, max_iterations=10000,
         max_plateau_width=200, relative_threshold=3.5, absolute_threshold=7.0, fixed_views=None,
         disable_fixed_views=False, group_tiles=None, group_illums=None, group_channels=None, split_timepoints=None,
-        registration_tp="TIMEPOINTS_INDIVIDUALLY", view_selection=None, dry_run=False):
+        registration_tp="TIMEPOINTS_INDIVIDUALLY", view_selection=None, dry_run=False, reference_tp=None):
     from . import n5 as bn5
-    from .commands import _InterestPoints
+    from .commands import REGISTRATION_TPS, _InterestPoints, reference_timepoint
     m = method.upper()
     if m not in METHODS:
         raise ValueError(f"--method {method}")
     if m.startswith("TWO_ROUND"):
         raise NotImplementedError(f"solver --method {m} is not implemented")
-    if registration_tp.upper() != "TIMEPOINTS_INDIVIDUALLY":
+    rtp = registration_tp.upper()
+    if rtp not in REGISTRATION_TPS:
         raise NotImplementedError(f"solver -rtp {registration_tp} is not implemented")
     src = source.upper()
     if src not in ("STITCHING", "IP"):
@@ -296,6 +311,7 @@ def run(xml_path, ctx, source, labels=None, label_weights=None, method="ONE_ROUN
     model = bm.Model(transformation_model, regularization_model, regularization_lambda)
     data = SpimData2.load(xml_path)
     views = sorted(data.select_views(**view_selection) if view_selection else data.view_ids())
+    ref = reference_timepoint(views, reference_tp)
     if src == "IP":
         labels = list(labels or [])
         if not labels:
@@ -336,7 +352,7 @@ def run(xml_path, ctx, source, labels=None, label_weights=None, method="ONE_ROUN
     elif fixed_views:
         fixed_v = {tuple(int(x) for x in (f.split(",") if isinstance(f, str) else f)) for f in fixed_views}
     else:
-        fixed_v = {min(v for v in views if v[0] == tp) for tp in sorted({v[0] for v in views})}
+        fixed_v = fixed_views_auto(views, rtp, ref)
     prob.fixed = np.zeros(prob.n_tiles, dtype=np.int32)
     for v in fixed_v:
         if v in tile_of:
