@@ -367,12 +367,7 @@ def _fuse_volume_blockwise(ctx, data, src, sink, meta, levels, view_ids, fusion_
     if coeffs is not None:
         # corrected sources are float32 whole-view volumes (the windowed fusion kernel reads uint16 windows only)
         windowed_ok = False
-        path, storage, group, dataset = coeffs
-        for v in view_ids:
-            c = bint.read_coefficients(path, storage, group, dataset, v)
-            if c is None:
-                raise ValueError(f"no intensity coefficients for view (timepoint {v[0]}, setup {v[1]}) in {path} "
-                                 f"({bint.coefficient_dataset(group, v, dataset)})")
+        for v, c in bint.view_coefficients(*coeffs, view_ids).items():
             factors, mts = src.mipmap_info(v)
             correction[v] = (c, mts[info[v]["level"]], tuple(int(d) for d in data.setups[v[1]].size))
     content = ft in (native.FUSE_AVG_CONTENT, native.FUSE_AVG_BLEND_CONTENT)
@@ -890,7 +885,8 @@ class _InterestPoints:
 def nonrigid_fusion(xml_path, ctx: Context, out_path, n5_dataset, interest_points, storage="N5",
                     block_size=(128, 128, 128), block_scale=(2, 2, 1), data_type="FLOAT32", min_intensity=None,
                     max_intensity=None, view_selection=None, bdv=None, xml_out=None, bounding_box=None, dry_run=False,
-                    shard=(0, 1), retries=5, blocks_per_call=16):
+                    shard=(0, 1), retries=5, blocks_per_call=16, intensity_n5_path=None, intensity_n5_storage=None,
+                    intensity_n5_group="", intensity_n5_dataset="intensity"):
     """`./nonrigid-fusion -x dataset.xml -o fused.n5 -d /ch0/s0 -ip beads [-ip nuclei] [-s N5|ZARR] [--blockSize ...]
     [--blockScale 2,2,1] [-p FLOAT32|UINT16|UINT8 --minIntensity --maxIntensity]` (J/SparkNonRigidFusion.java:124-446):
     the maximal bounding box of the selected views becomes dataset ``n5_dataset`` (Zstandard, attribute offset = bb.min);
@@ -898,6 +894,13 @@ def nonrigid_fusion(xml_path, ctx: Context, out_path, n5_dataset, interest_point
     device with per-view moving-least-squares grids fitted to the corresponding interest points of the ``-ip`` labels
     (bs_nonrigid_fuse_blocks, AVG_BLEND, control points every 10 px) and saved; blocks no view reaches are not written.
     Returns the list of written grid positions.  ZARR output is the (t, c, z, y, x) array with singleton t and c.
+
+    ``intensity_n5_path`` (`--intensityN5Path`, with `--intensityN5Storage` / `--intensityN5Group` /
+    `--intensityN5Dataset`, as affine-fusion takes them; upstream nonrigid-fusion has no such option, PARITY_GAPS N6):
+    the coefficients solve-intensities wrote.  Every staged s0 source window is corrected on the device to float32
+    (bs_intensity_apply at the window's full-resolution position, before the n-linear resampling) and fused from that.
+    The coefficients of every selected view are read before the output dataset is created, so a selected view without
+    a coefficient dataset raises ValueError and leaves nothing behind.  None: nothing changes.
 
     ``--bdv`` / ``-xo``, named ``-b`` bounding boxes, multi-GPU sharding and ``--dryRun`` raise NotImplementedError."""
     for flag, on in (("--bdv", bdv is not None), ("-xo", xml_out is not None), ("-b", bounding_box is not None),
@@ -917,6 +920,10 @@ def nonrigid_fusion(xml_path, ctx: Context, out_path, n5_dataset, interest_point
     views = sorted(data.select_views(**view_selection) if view_selection else data.view_ids())
     regs = {v: data.model(*v) for v in views}
     vdims = {v: tuple(int(d) for d in data.setups[v[1]].size) for v in views}
+    coeffs = None
+    if intensity_n5_path is not None:
+        coeffs = bint.view_coefficients(intensity_n5_path, intensity_n5_storage, intensity_n5_group,
+                                        intensity_n5_dataset, views)
     lo = np.full(3, np.iinfo(np.int64).max, dtype=np.int64)
     hi = np.full(3, np.iinfo(np.int64).min, dtype=np.int64)
     for v in views:
@@ -969,7 +976,7 @@ def nonrigid_fusion(xml_path, ctx: Context, out_path, n5_dataset, interest_point
             for c0 in range(0, len(todo), blocks_per_call):
                 chunk = todo[c0:c0 + blocks_per_call]
                 try:
-                    outs = _nonrigid_chunk(ctx, src, chunk, lo, fuse, nviews, vdims, params, cpd)
+                    outs = _nonrigid_chunk(ctx, src, chunk, lo, fuse, nviews, vdims, params, cpd, coeffs)
                 except native.BsError:
                     failed.extend(chunk)
                     continue
@@ -980,9 +987,11 @@ def nonrigid_fusion(xml_path, ctx: Context, out_path, n5_dataset, interest_point
     return written
 
 
-def _nonrigid_chunk(ctx, src, chunk, bb_min, fuse, nviews, vdims, params, cpd):
+def _nonrigid_chunk(ctx, src, chunk, bb_min, fuse, nviews, vdims, params, cpd, coeffs=None):
     """Fuse a list of super-blocks that share their views.  Each view's source window is the range its control-point
-    grids map to over the chunk (+2 px for the n-linear taps), read from level s0 and uploaded as a windowed view."""
+    grids map to over the chunk (+2 px for the n-linear taps), read from level s0 and uploaded as a windowed view.
+    ``coeffs`` ({view: (a, b)}): each window is replaced by its float32 correction (s0 is full resolution, so the
+    window voxel l sits at q = window_min + l)."""
     mins = [tuple(int(v) for v in bb_min + np.asarray(off, dtype=np.int64)) for off, _, _ in chunk]
     sizes = [tuple(int(v) for v in size) for _, size, _ in chunk]
     staged, gviews = [], []
@@ -1000,6 +1009,12 @@ def _nonrigid_chunk(ctx, src, chunk, bb_min, fuse, nviews, vdims, params, cpd):
             if np.any(whi < wlo):
                 continue                                  # the view's grids never reach its pixels in this chunk
             h = ctx.volume_upload(src.read_region(v, 0, wlo, whi - wlo + 1))
+            if coeffs is not None:
+                try:
+                    hc = ctx.intensity_apply(h, vdims[v], np.eye(3, 4), *coeffs[v], window_min_xyz=wlo)
+                finally:
+                    ctx.volume_free(h)
+                h = hc
             staged.append(h)
             gviews.append(dict(nv, vol_handle=h, window_min=tuple(int(x) for x in wlo)))
         if not gviews:

@@ -1,5 +1,5 @@
 """Intensity correction: the host side of `match-intensities`, `solve-intensities` and the coefficient input of
-`affine-fusion --intensityN5Path`.
+`affine-fusion --intensityN5Path` and `nonrigid-fusion --intensityN5Path`.
 
   match-intensities   J/SparkIntensityMatching.java:84-190 (IntensityCorrection.matchRansac per view pair)
   solve-intensities   J/IntensitySolver.java:50-123      (IntensityCorrection.solve, writeCoefficients)
@@ -344,6 +344,21 @@ def read_coefficients(path, storage, group, dataset, view):
     with open(os.path.join(path, ds, "0", "0", "0", "0"), "rb") as f:
         arr = np.frombuffer(f.read(), dtype=np.dtype(m["dtype"])).astype(np.float64).reshape(2, nz, ny, nx)
     return arr[0].copy(), arr[1].copy()
+
+
+def view_coefficients(path, storage, group, dataset, views):
+    """{view: (a, b)} of every view in ``views``, read before anything is fused (`--intensityN5Path`, with
+    `--intensityN5Storage` / `--intensityN5Group` / `--intensityN5Dataset`).  ``storage`` None: guessed from the path
+    (guess_storage, HDF5 raises NotImplementedError).  A view without a coefficient dataset raises ValueError."""
+    storage = guess_storage(path, storage)
+    out = {}
+    for v in views:
+        c = read_coefficients(path, storage, group, dataset, v)
+        if c is None:
+            raise ValueError(f"no intensity coefficients for view (timepoint {v[0]}, setup {v[1]}) in {path} "
+                             f"({coefficient_dataset(group, v, dataset)})")
+        out[v] = c
+    return out
 
 
 def check_coefficients_size(stored, wanted):

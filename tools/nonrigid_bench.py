@@ -7,7 +7,13 @@ control-point x point evaluations per second of k_mls_grid, fused Gvoxel/s of k_
 time (N5 source reads, uploads, zstd output included), the card name and power limit read in the same run, and,
 labelled as a CPU figure, the float64 oracle on one bounded super-block.  The dataset goes to a temporary directory.
 
-    python tools/nonrigid_bench.py [--tiles 4x2] [--size 512x512x256] [--beads 3000] [--out result.json]
+``--intensity``: instead, write seeded 8x8x8-cell intensity coefficients for every tile and run the command without and
+with them (`intensity_n5_path`), alternating, ``--repeats`` times each after one warm-up run of each.  Reports the
+seconds end to end of every run, then one profiled run of each with the device time and launch count of
+"intensity_apply" next to "mls_grid" and "nonrigid_fuse", and the card name and power limit.
+
+    python tools/nonrigid_bench.py [--tiles 4x2] [--size 512x512x256] [--beads 3000] [--intensity [--repeats 3]]
+                                   [--out result.json]
 """
 import argparse
 import json
@@ -98,11 +104,54 @@ def make_dataset(tmp, tiles_xy, size, n_beads, seed=5):
     return xml, sum(len(v) for v in pts.values())
 
 
+def intensity_runs(ctx, xml, tmp, repeats, res, seed=9):
+    """nonrigid-fusion without and with seeded coefficients (a in [0.8, 1.2], b in [-20, 20] per cell), alternating."""
+    import shutil
+    from bsgpu import commands, intensity as bint, spimdata
+    views = spimdata.SpimData2.load(xml).view_ids()
+    rng = np.random.default_rng(seed)
+    co = {v: (rng.uniform(0.8, 1.2, (8, 8, 8)), rng.uniform(-20.0, 20.0, (8, 8, 8))) for v in views}
+    cpath = os.path.join(tmp, "coeff.n5")
+    bint.write_coefficients(cpath, "N5", "", "intensity", co)
+    modes = {"plain": {}, "intensity": dict(intensity_n5_path=cpath)}
+
+    def run(mode):
+        out = os.path.join(tmp, f"{mode}.n5")
+        t0 = time.perf_counter()
+        blocks = commands.nonrigid_fusion(xml, ctx, out, "fused/s0", ["beads"], data_type="UINT16", min_intensity=0.0,
+                                          max_intensity=2000.0, **modes[mode])
+        ctx.synchronize()
+        s = time.perf_counter() - t0
+        shutil.rmtree(out)
+        return s, len(blocks)
+
+    for mode in modes:                                   # first calls: module load, allocations
+        run(mode)
+    secs = {mode: [] for mode in modes}
+    for _ in range(repeats):
+        for mode in modes:
+            s, n = run(mode)
+            secs[mode].append(round(s, 2))
+            res[f"{mode}_blocks_written"] = n
+    for mode in modes:
+        res[f"{mode}_command_s"] = secs[mode]
+        res[f"{mode}_command_s_median"] = float(np.median(secs[mode]))
+        ctx.profile_enable(True)
+        ctx.profile_reset()
+        run(mode)
+        for tag in ("mls_grid", "nonrigid_fuse", "intensity_apply"):
+            ms, n = ctx.profile_get(tag)
+            res[f"{mode}_{tag}_ms"], res[f"{mode}_{tag}_launches"] = round(ms, 2), n
+        ctx.profile_enable(False)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--tiles", default="4x2")
     ap.add_argument("--size", default="512x512x256")
     ap.add_argument("--beads", type=int, default=3000)
+    ap.add_argument("--intensity", action="store_true")
+    ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     tiles = tuple(int(v) for v in a.tiles.split("x"))
@@ -116,6 +165,11 @@ def main():
         xml, n_points = make_dataset(tmp, tiles, size, a.beads)
         res["dataset_s"] = round(time.perf_counter() - t0, 1)
         res["points_total"] = n_points
+        if a.intensity:
+            with bsgpu.Context(0) as ctx:
+                intensity_runs(ctx, xml, tmp, a.repeats, res)
+            emit(res, a.out)
+            return
         with bsgpu.Context(0) as ctx:
             evals = [0]
             voxels = [0]
@@ -168,10 +222,14 @@ def main():
         res["cpu_oracle_block"] = "x".join(str(v) for v in bsz)
         res["cpu_oracle_s"] = round(cpu_s, 2)
         res["cpu_oracle_mvoxel_per_s"] = round(float(np.prod(bsz)) / cpu_s / 1e6, 4)
+    emit(res, a.out)
+
+
+def emit(res, out):
     line = json.dumps(res)
     print(line)
-    if a.out:
-        with open(a.out, "w") as f:
+    if out:
+        with open(out, "w") as f:
             f.write(line + "\n")
 
 
