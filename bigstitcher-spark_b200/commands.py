@@ -39,7 +39,7 @@ from . import matching as bm
 from . import intensity as bint
 from . import native, solver as bsolver, split as bsplit, stitching as bst, viewsource as bvs
 from .native import Context
-from .spimdata import SpimData2, fusion_project
+from .spimdata import FILEMAP_LOADER, SpimData2, fusion_project
 
 
 def stitching(xml_path, ctx: Context, downsampling=(2, 2, 1), peaks_to_check=5, disable_subpixel=False,
@@ -1423,9 +1423,11 @@ def resave(xml_path, ctx: Context, xml_out=None, n5=False, out_path=None, block_
     xml_out = xml_out or xml_path
     if out_path is None:
         out_path = os.path.join(os.path.dirname(os.path.abspath(xml_out)), "dataset.n5" if n5 else "dataset.ome.zarr")
-    a, b = os.path.realpath(out_path), os.path.realpath(src.store.root)
-    if a == b or a.startswith(b + os.sep) or b.startswith(a + os.sep):
-        raise ValueError(f"resave output {out_path} overlaps the input container {src.store.root}; choose another -o / -xo")
+    a = os.path.realpath(out_path)
+    for root in src.roots:
+        b = os.path.realpath(root)
+        if a == b or a.startswith(b + os.sep) or b.startswith(a + os.sep):
+            raise ValueError(f"resave output {out_path} overlaps the input container {root}; choose another -o / -xo")
     bs = [int(v) for v in block_size]
     compute = [bs[d] * int(block_scale[d]) for d in range(3)]
     if downsampling is None:     # N5ApiTools.mipMapInfoToDownsamplings(proposeMipmaps(...)): one pyramid for all views
@@ -1795,7 +1797,8 @@ def split_images(xml_path, target_image_size, target_overlap, xml_out=None, disa
     (re-run matching).  ``fake_interest_points`` (`-fip`) adds split.fake_points between overlapping sub-views of one
     view, with their correspondences, as label ``fip_label``, which must not exist yet (ValueError).
 
-    ``display_result`` (a GUI) raises NotImplementedError; ``dry_run`` returns the plan and writes nothing.  Returns
+    A TIFF dataset (`spimreconstruction.filemap2`) raises NotImplementedError before anything is written: resave it
+    first.  ``display_result`` (a GUI) raises NotImplementedError; ``dry_run`` returns the plan and writes nothing.  Returns
     dict(step=m, size=s, overlap=o, views={new setup: (old setup, min xyz, max xyz)}, fake_points={(tp, new a, new b):
     count})."""
     if display_result:
@@ -1804,6 +1807,9 @@ def split_images(xml_path, target_image_size, target_overlap, xml_out=None, disa
     overlap = bsplit.parse_size(target_overlap, "targetOverlap")
     data = SpimData2.load(xml_path)
     src = bvs.open_views(data)
+    if src.format == FILEMAP_LOADER:
+        raise NotImplementedError("split-images of a TIFF dataset (spimreconstruction.filemap2): resave it to N5 or "
+                                  "OME-ZARR first")
     missing = data.missing_views()
     present = [v for v in data.view_ids() if v not in missing]
     m = bsplit.min_step(src, present)

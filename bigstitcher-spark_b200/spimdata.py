@@ -7,7 +7,8 @@ extensions) -- the fields the two hot paths consume and produce:
     (J/ClearRegistrations.java:80-99), so model = T0 * T1 * ... * Tn
   * ImageLoader format="bdv.n5" path (J/SparkResaveN5.java:424-433), or format="bdv.multimg.zarr" (AllenOMEZarrLoader,
     :434-445): the container root plus one <zgroup> per view with its group path and (channel, timepoint) indices,
-    or format="split.viewerimgloader" (split-images): one of those loaders plus the box of an old setup per new setup
+    or format="split.viewerimgloader" (split-images): one of those loaders plus the box of an old setup per new setup,
+    or format="spimreconstruction.filemap2" (TIFF stacks): one <FileMapping> of a file, series and channel per view
   * <MissingViews> and the <Attributes> entries of <ViewSetups> (tile names and locations, illuminations)
   * <StitchingResults><PairwiseResult view_setup_a/b tp_a/b> shift (12 doubles), correlation, hash,
     overlap_boundingbox (6 doubles)                                   (J/SparkPairwiseStitching.java:284-301,328-390)
@@ -29,6 +30,7 @@ from dataclasses import dataclass, field
 import numpy as np
 
 SPLIT_LOADER = "split.viewerimgloader"
+FILEMAP_LOADER = "spimreconstruction.filemap2"
 
 
 @dataclass
@@ -132,6 +134,44 @@ class SpimData2:
                 ET.SubElement(zg, "zgroup", setup=str(setup), tp=str(tp), path=gpath, indicies=f"[{int(c)}, {int(t)}]")
         elif fmt != "bdv.n5":
             raise ValueError(f"ImageLoader format {fmt}")
+        seq.insert(list(seq).index(old) if old is not None else 0, il)
+        if old is not None:
+            seq.remove(old)
+
+    # ------------------------------------------------------------------ TIFF files (the automatic loader)
+    def file_mappings(self):
+        """The views of a `spimreconstruction.filemap2` loader: {(tp, setup): (absolute file path, series, channel)};
+        relative paths resolve against the BasePath.  Element names are recalled from XmlIoFileMapImgLoaderLOCI2
+        (PARITY_GAPS T1).  A z-grouped loader (one file per plane) raises NotImplementedError."""
+        il = self._loader_element()
+        for e in il:
+            if e.tag.lower() == "zgrouped" and (e.text or "").strip().lower() == "true":
+                raise NotImplementedError(f"ImageLoader {il.get('format')}: ZGrouped (one file per z-plane); "
+                                          "only files holding whole stacks are read")
+        base = os.path.join(os.path.dirname(os.path.abspath(self.path or ".")), self.root.findtext("BasePath") or ".")
+        out = {}
+        files = il.find("files")
+        for m in (files.findall("FileMapping") if files is not None else []):
+            f = m.find("file")
+            p = f.text.strip()
+            if f.get("type", "relative") == "relative":
+                p = os.path.normpath(os.path.join(base, p))
+            out[(int(m.get("timepoint")), int(m.get("view_setup")))] = (p, int(m.get("series", 0)),
+                                                                        int(m.get("channel", 0)))
+        return out
+
+    def set_file_map_loader(self, mappings, xml_path=None):
+        """Replace the ImageLoader by a `spimreconstruction.filemap2` one: ``mappings`` = {(tp, setup): (file path,
+        series, channel)}, each path written relative to the BasePath of the XML at ``xml_path`` (default: where this
+        one was loaded from)."""
+        seq = self.root.find("SequenceDescription")
+        old = seq.find("ImageLoader")
+        il = ET.Element("ImageLoader", format=FILEMAP_LOADER)
+        files = ET.SubElement(il, "files")
+        for (tp, setup), (path, series, channel) in sorted(mappings.items()):
+            m = ET.SubElement(files, "FileMapping", view_setup=str(int(setup)), timepoint=str(int(tp)),
+                              series=str(int(series)), channel=str(int(channel)))
+            ET.SubElement(m, "file", type="relative").text = self._loader_path(path, xml_path)
         seq.insert(list(seq).index(old) if old is not None else 0, il)
         if old is not None:
             seq.remove(old)

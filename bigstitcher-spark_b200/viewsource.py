@@ -1,23 +1,27 @@
 """The image data of a SpimData2 dataset, whichever container holds it: volume and region reads and the mipmap
-levels of every view.  Two loaders are read (Import / the BDV image loaders the reference opens through the XML):
+levels of every view.  Three loaders are read (Import / the BDV image loaders the reference opens through the XML):
 
   * `bdv.n5` -- BDV-N5: `setup{s}/timepoint{t}/s{l}` 3-D datasets, mipmap factors from the setup's
     `downsamplingFactors` attribute;
   * `bdv.multimg.zarr` -- AllenOMEZarrLoader (J/SparkResaveN5.java:434-445): one OME-NGFF multiscale group per view,
     levels "0", "1", ... of 5-D (t, c, z, y, x) arrays read at the view's (channel, timepoint) indices, mipmap factors
-    from the levels' `scale` transformations (zarr.read_multiscales).
+    from the levels' `scale` transformations (zarr.read_multiscales);
+  * `spimreconstruction.filemap2` -- TIFF stacks as BigStitcher's automatic loader defines them: per view a file,
+    a series and a channel (SpimData2.file_mappings), read by tiff.py, one level (TiffViews).
 
 Mipmap transforms follow the half-pixel convention of MipmapTransforms.getMipmapTransformDefault for both
-(zarr.mipmap_transform_default).  A `split.viewerimgloader` (split-images) wraps either of them: its views are boxes
-of the wrapped views (SplitViews).  Any other loader raises NotImplementedError.  Host-side plumbing only.
+(zarr.mipmap_transform_default).  A `split.viewerimgloader` (split-images) wraps an N5 or OME-ZARR one: its views are
+boxes of the wrapped views (SplitViews).  Any other loader raises NotImplementedError.  ``roots`` of every view source
+lists the containers or files it reads.  Host-side plumbing only.
 """
 from __future__ import annotations
 
 import numpy as np
 
 from . import n5 as bn5
+from . import tiff as btiff
 from . import zarr as bzarr
-from .spimdata import SPLIT_LOADER
+from .spimdata import FILEMAP_LOADER, SPLIT_LOADER
 
 
 def open_views(data):
@@ -27,6 +31,8 @@ def open_views(data):
         return N5Views(path)
     if fmt == "bdv.multimg.zarr":
         return ZarrViews(path, data.zarr_groups())
+    if fmt == FILEMAP_LOADER:
+        return TiffViews(data.file_mappings())
     if fmt == SPLIT_LOADER:
         fmt, path = data.image_loader(nested=True)
         if fmt == "bdv.n5":
@@ -41,6 +47,7 @@ class N5Views:
 
     def __init__(self, root):
         self.store = bn5.N5Store(root)
+        self.roots = [root]
 
     def mipmap_info(self, view):
         """(factors [(fx, fy, fz)] per level, mipmap transforms 3 x 4 per level) of a view."""
@@ -69,6 +76,7 @@ class ZarrViews:
 
     def __init__(self, root, groups):
         self.store = bzarr.ZarrStore(root)
+        self.roots = [root]
         self.groups = groups                     # {(tp, setup): (group path, channel index, timepoint index)}
         self._levels = {}
 
@@ -101,6 +109,58 @@ class ZarrViews:
         return self.store.read_region(levels[level]["path"], min_xyz, size_xyz, c, t)
 
 
+class TiffViews:
+    """TIFF stacks (`spimreconstruction.filemap2`): view (tp, setup) is channel ``channel`` of series ``series`` of its
+    file, at frame tp when the series has more than one frame and at frame 0 for every timepoint when it has one
+    (PARITY_GAPS T2).  One level, full resolution.  Files are opened on first use and kept open."""
+    format = FILEMAP_LOADER
+
+    def __init__(self, mappings):
+        self.mappings = mappings                 # {(tp, setup): (file path, series, channel)}
+        self.roots = sorted({m[0] for m in mappings.values()})
+        self._files = {}
+
+    def _view(self, view):
+        """(Series, channel, frame) of a view."""
+        key = (int(view[0]), int(view[1]))
+        if key not in self.mappings:
+            raise KeyError(f"view {key} has no <FileMapping> in the ImageLoader")
+        path, series, channel = self.mappings[key]
+        if path not in self._files:
+            self._files[path] = btiff.TiffFile(path)
+        all_series = self._files[path].series()
+        if series >= len(all_series):
+            raise ValueError(f"view {key}: {path} has {len(all_series)} series, not series {series}")
+        s = all_series[series]
+        frame = key[0] if s.frames > 1 else 0
+        if channel >= s.channels or frame >= s.frames:
+            raise ValueError(f"view {key}: series {series} of {path} has {s.channels} channels and {s.frames} frames; "
+                             f"channel {channel}, frame {frame} asked")
+        return s, channel, frame
+
+    def mipmap_info(self, view):
+        return [(1, 1, 1)], [bzarr.mipmap_transform_default((1, 1, 1))]
+
+    def _level0(self, view, level):
+        if int(level) != 0:
+            raise ValueError(f"view {tuple(view)}: a TIFF view has only level 0, not level {level}")
+        return self._view(view)
+
+    def level_dims(self, view, level):
+        return self._level0(view, level)[0].dims
+
+    def level_dtype(self, view, level) -> str:
+        return self._level0(view, level)[0].dtype.name
+
+    def read_volume(self, view, level=0):
+        s, c, t = self._level0(view, level)
+        return s.read_volume(c, t)
+
+    def read_region(self, view, level, min_xyz, size_xyz):
+        s, c, t = self._level0(view, level)
+        return s.read_region(min_xyz, size_xyz, c, t)
+
+
 class SplitViews:
     """The sub-views split-images defines (`split.viewerimgloader`): view (tp, new setup) is the box [min, max] of view
     (tp, old setup) of the wrapped N5Views / ZarrViews.  Level l with factors f is the parent's level-l window from
@@ -111,6 +171,7 @@ class SplitViews:
     def __init__(self, inner, definitions):
         self.inner = inner
         self.store = inner.store
+        self.roots = inner.roots
         self.definitions = definitions           # {new setup: (old setup, min xyz, max xyz)}
 
     def _parent(self, view):
