@@ -135,10 +135,6 @@ void bs_destroy(bs_ctx* ctx) {
     bs_match_free(ctx);
     bs_intensity_free(ctx);
     bs_comm_free(ctx);
-    if (ctx->fuse_ring_dev) cudaFree(ctx->fuse_ring_dev);
-    if (ctx->fuse_ring_host) cudaFreeHost(ctx->fuse_ring_host);
-    for (int i = 0; i < bs_ctx::kFuseSlots; ++i)
-        if (ctx->fuse_slot_ev[i]) cudaEventDestroy(ctx->fuse_slot_ev[i]);
     if (ctx->fuse_out) cudaFree(ctx->fuse_out);
     if (ctx->fuse_plan) cudaFree(ctx->fuse_plan);
     cudaStreamDestroy(ctx->copy_stream);

@@ -79,15 +79,6 @@ struct bs_ctx {
     std::map<std::string, bs_prof_entry> prof_entries;
     std::vector<bs_pending_event> prof_pending;
     bs_pcm_workspace ws;
-    // ring of descriptor slots (pinned host mirror + device copy): a fusion call never has to
-    // synchronise the stream just to hand its view list to the kernel
-    static constexpr int kFuseSlots = 16;
-    void* fuse_ring_host = nullptr;
-    void* fuse_ring_dev = nullptr;
-    size_t fuse_slot_bytes = 0;
-    int fuse_next_slot = 0;
-    cudaEvent_t fuse_slot_ev[kFuseSlots] = {};
-    bool fuse_slot_used[kFuseSlots] = {};
     void* fuse_plan = nullptr;        // per-tile view lists of the current fusion call
     size_t fuse_plan_cap = 0;
     void* fuse_out = nullptr;         // device staging for host outputs
@@ -156,6 +147,13 @@ int bs_volume_acquire(bs_ctx* ctx, bs_volume& v);
 void bs_pcm_workspace_free(bs_ctx* ctx);
 // fuse_tma.cu
 void bs_fuse2_free(bs_ctx* ctx);
+// Staging of one fusion call's tables (views, blocks, LUT, ...) into device memory on ctx->stream.
+// bs_fuse_tables_reserve waits until the next pinned host slot is no longer read by an earlier copy and
+// returns it (*host, `bytes` long, 16-byte aligned) with the device address the tables will have (*dev);
+// bs_fuse_tables_commit queues the copy.  The device buffer is shared by all calls, so the kernels that read
+// the tables must be queued on ctx->stream before the next call's commit.
+int bs_fuse_tables_reserve(bs_ctx* ctx, size_t bytes, void** host, const void** dev);
+int bs_fuse_tables_commit(bs_ctx* ctx);
 // the driver's cuTensorMapEncodeTiled, or NULL when the driver does not provide it
 PFN_cuTensorMapEncodeTiled_v12000 bs_tensor_map_encoder();
 void bs_dog_free(bs_ctx* ctx);
@@ -167,7 +165,12 @@ void bs_match_free(bs_ctx* ctx);
 void bs_intensity_free(bs_ctx* ctx);
 // comm.cu
 void bs_comm_free(bs_ctx* ctx);
-// fuse.cu: generic tile kernel for one block into a device buffer (ctx->mu held by the caller)
+// fuse.cu: generic tile kernel for one block into a device buffer (ctx->mu held by the caller; arguments
+// validated by bs_fuse_validate and bs_fuse_validate_blocks)
 int bs_fuse_legacy_block(bs_ctx* ctx, const bs_view* views, int n_views, const long long block_min[3],
                          const long long block_size[3], const bs_fuse_params* params, void* out_dev);
+// the argument checks shared by every fusion entry point
 int bs_fuse_validate(bs_ctx* ctx, const bs_view* views, int n_views, const bs_fuse_params* p);
+int bs_fuse_validate_blocks(bs_ctx* ctx, int nb, const long long* bmin, const long long* bsize, const bs_fuse_params* p);
+// a block extent the fusion kernels' int sizes can hold
+static inline bool bs_fuse_block_dim_ok(long long n) { return n > 0 && n <= 0x7fffffffLL; }

@@ -40,7 +40,6 @@ struct FuseArgs {
     void* out;
     float* acc_wi;         // accumulate mode
     float* acc_w;
-    int no_stage;          // debug: force the global-gather path (env BS_FUSE_NO_STAGE)
     const struct TilePlan* plan;   // per-tile view lists from fuse_plan_kernel (or nullptr)
 };
 
@@ -210,7 +209,7 @@ __global__ void fuse_plan_kernel(const FuseViewDev* __restrict__ views, int nvie
     int count = 0, overflow = 0;
     for (int vi = 0; vi < nviews; ++vi) {
         ViewTile t;
-        if (!make_view_tile(views[vi], cx0, cy0, cz0, ex, ey, ez, linear && a.no_stage == 0, t)) continue;
+        if (!make_view_tile(views[vi], cx0, cy0, cz0, ex, ey, ez, linear, t)) continue;
         if (count < FUSE_PLAN_MAXV) p.v[count++] = t;
         else overflow = 1;
     }
@@ -344,7 +343,7 @@ fuse_kernel(const FuseViewDev* __restrict__ views, int nviews, FuseArgs a) {
             // cull: threads over the views of this chunk
             for (int vi = chunk + tid; vi < min(nviews, chunk + FUSE_CHUNK); vi += NT) {
                 ViewTile t;
-                if (make_view_tile(views[vi], cx0, cy0, cz0, ex, ey, ez, LINEAR && a.no_stage == 0, t))
+                if (make_view_tile(views[vi], cx0, cy0, cz0, ex, ey, ez, LINEAR, t))
                     s_active[atomicAdd(&s_nactive, 1)] = vi;
             }
             __syncthreads();
@@ -359,7 +358,7 @@ fuse_kernel(const FuseViewDev* __restrict__ views, int nviews, FuseArgs a) {
             }
             __syncthreads();
             for (int ai = tid; ai < nact; ai += NT)
-                make_view_tile(views[s_active[ai]], cx0, cy0, cz0, ex, ey, ez, LINEAR && a.no_stage == 0, s_vt[ai]);
+                make_view_tile(views[s_active[ai]], cx0, cy0, cz0, ex, ey, ez, LINEAR, s_vt[ai]);
             __syncthreads();
         }
 
@@ -484,40 +483,31 @@ int bs_fuse_validate(bs_ctx* ctx, const bs_view* views, int n_views, const bs_fu
     return BS_OK;
 }
 
+int bs_fuse_validate_blocks(bs_ctx* ctx, int nb, const long long* bmin, const long long* bsize, const bs_fuse_params* p) {
+    if (!bmin || !bsize || !p) return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse: NULL argument");
+    if (nb < 0) return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse_blocks: n_blocks < 0");
+    for (int b = 0; b < nb; ++b)
+        for (int d = 0; d < 3; ++d)
+            if (!bs_fuse_block_dim_ok(bsize[3 * b + d]))
+                return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse: bad block_size[%d]=%lld", d, bsize[3 * b + d]);
+    return BS_OK;
+}
+
 struct FusePrepared {
     FuseArgs args;
     int nviews;
-    int slot;
     const FuseViewDev* views_dev;
 };
 
-// validate + upload view descriptors (and the cosine table); fills args except out pointers
+// upload the view descriptors (and the cosine table) of validated arguments; fills args except out pointers.
+// Rejects what only this kernel cannot take: windowed views and content volumes that do not match their view.
 static int fuse_prepare(bs_ctx* ctx, const bs_view* views, int n_views, const long long block_min[3],
                         const long long block_size[3], const bs_fuse_params* p, FusePrepared* prep) {
-    if (!views && n_views > 0) return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse: views is NULL");
-    if (!block_min || !block_size || !p) return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse: NULL argument");
-    if (n_views < 0) return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse: n_views < 0");
-    for (int d = 0; d < 3; ++d)
-        if (block_size[d] <= 0 || block_size[d] > 0x7fffffffLL)
-            return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse: bad block_size[%d]=%lld", d, block_size[d]);
-    if (p->fusion_type < BS_FUSE_AVG || p->fusion_type > BS_FUSE_CLOSEST_PIXEL_WINS)
-        return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse: unknown fusion_type %d", p->fusion_type);
-    if (p->interpolation != 0 && p->interpolation != 1)
-        return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse: interpolation must be 0 or 1");
-    if (p->out_dtype != BS_DTYPE_F32 && p->out_dtype != BS_DTYPE_U16 && p->out_dtype != BS_DTYPE_U8)
-        return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse: bad out_dtype %d", p->out_dtype);
-    if (p->blend_lut_n < 0 || p->blend_lut_n > FUSE_MAX_LUT)
-        return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse: blend_lut_n out of range [0,%d]", FUSE_MAX_LUT);
-    if (p->out_dtype != BS_DTYPE_F32 && !(p->max_intensity > p->min_intensity))
-        return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse: max_intensity must exceed min_intensity");
     const bool need_content = p->fusion_type == BS_FUSE_AVG_CONTENT || p->fusion_type == BS_FUSE_AVG_BLEND_CONTENT;
 
     std::vector<FuseViewDev> hv((size_t)n_views);
     for (int i = 0; i < n_views; ++i) {
-        auto it = ctx->vols.find(views[i].vol_handle);
-        if (it == ctx->vols.end())
-            return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse: view %d has unknown vol_handle %llu", i, views[i].vol_handle);
-        bs_volume& vol = it->second;
+        bs_volume& vol = ctx->vols.find(views[i].vol_handle)->second;
         { int rc = bs_volume_acquire(ctx, vol); if (rc) return rc; }
         if (views[i].full_dims[0] > 0)
             return bs_set_error(ctx, BS_ERR_UNSUPPORTED, "bs_fuse: windowed views need uint16 sources with x size a multiple of 8, "
@@ -541,54 +531,32 @@ static int fuse_prepare(bs_ctx* ctx, const bs_view* views, int n_views, const lo
             d.range[k] = views[i].blend_range[k];
         }
     }
+    // the table: the LUT, then the view descriptors
     const size_t lut_bytes = (size_t)(FUSE_MAX_LUT + 2) * sizeof(float);
-    const size_t need = lut_bytes + hv.size() * sizeof(FuseViewDev);
-    if (need > ctx->fuse_slot_bytes) {
-        size_t sb = 1 << 16;
-        while (sb < need) sb <<= 1;
-        BS_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        if (ctx->fuse_ring_dev) cudaFree(ctx->fuse_ring_dev);
-        if (ctx->fuse_ring_host) cudaFreeHost(ctx->fuse_ring_host);
-        ctx->fuse_ring_dev = ctx->fuse_ring_host = nullptr;
-        ctx->fuse_slot_bytes = 0;
-        BS_CUDA(ctx, cudaMalloc(&ctx->fuse_ring_dev, sb * bs_ctx::kFuseSlots));
-        BS_CUDA(ctx, cudaHostAlloc(&ctx->fuse_ring_host, sb * bs_ctx::kFuseSlots, cudaHostAllocDefault));
-        for (int i = 0; i < bs_ctx::kFuseSlots; ++i) {
-            ctx->fuse_slot_used[i] = false;
-            if (!ctx->fuse_slot_ev[i])
-                BS_CUDA(ctx, cudaEventCreateWithFlags(&ctx->fuse_slot_ev[i], cudaEventDisableTiming));
-        }
-        ctx->fuse_slot_bytes = sb;
-    }
-    const int slot = ctx->fuse_next_slot;
-    ctx->fuse_next_slot = (slot + 1) % bs_ctx::kFuseSlots;
-    if (ctx->fuse_slot_used[slot]) BS_CUDA(ctx, cudaEventSynchronize(ctx->fuse_slot_ev[slot]));
-    unsigned char* hslot = (unsigned char*)ctx->fuse_ring_host + (size_t)slot * ctx->fuse_slot_bytes;
-    unsigned char* dslot = (unsigned char*)ctx->fuse_ring_dev + (size_t)slot * ctx->fuse_slot_bytes;
-    float* lut = (float*)hslot;
+    void* host = nullptr;
+    const void* dev = nullptr;
+    int rc = bs_fuse_tables_reserve(ctx, lut_bytes + hv.size() * sizeof(FuseViewDev), &host, &dev);
+    if (rc) return rc;
+    float* lut = (float*)host;
     const int n = p->blend_lut_n;
     if (n > 0) {
         for (int i = 0; i <= n; ++i) lut[i] = (float)((std::cos((1.0 - (double)i / n) * M_PI) + 1.0) / 2.0);
         lut[n + 1] = lut[n];
     }
-    if (!hv.empty()) memcpy(hslot + lut_bytes, hv.data(), hv.size() * sizeof(FuseViewDev));
-    BS_CUDA(ctx, cudaMemcpyAsync(dslot, hslot, need, cudaMemcpyHostToDevice, ctx->stream));
-    prep->slot = slot;
-    prep->views_dev = (const FuseViewDev*)(dslot + lut_bytes);
+    if (!hv.empty()) memcpy((unsigned char*)host + lut_bytes, hv.data(), hv.size() * sizeof(FuseViewDev));
+    rc = bs_fuse_tables_commit(ctx);
+    if (rc) return rc;
+    prep->views_dev = (const FuseViewDev*)((const unsigned char*)dev + lut_bytes);
 
     FuseArgs& a = prep->args;
     memset(&a, 0, sizeof(a));
     for (int d = 0; d < 3; ++d) { a.bmin[d] = block_min[d]; a.size[d] = (int)block_size[d]; }
     a.fusion_type = p->fusion_type;
     a.lut_n = n;
-    a.lut = (const float*)dslot;
+    a.lut = (const float*)dev;
     a.ctop = p->out_dtype == BS_DTYPE_U8 ? 255.0 : 65535.0;
     a.cmin = p->min_intensity;
     a.cscale = p->out_dtype == BS_DTYPE_F32 ? 1.0 : a.ctop / (p->max_intensity - p->min_intensity);
-    {
-        const char* e = getenv("BS_FUSE_NO_STAGE");
-        a.no_stage = (e && *e && *e != '0') ? 1 : 0;
-    }
     prep->nviews = n_views;
     return BS_OK;
 }
@@ -619,9 +587,8 @@ static int fuse_launch(bs_ctx* ctx, const FusePrepared& prep, const bs_fuse_para
     const bool lin = p->interpolation == 1;
     FuseArgs a2 = a;
     {
-        const char* e = getenv("BS_FUSE_NO_PLAN");
         const long long ntiles = (long long)grid.x * grid.y * grid.z;
-        if (!(e && *e && *e != '0') && prep.nviews > 0 && ntiles * (long long)sizeof(TilePlan) <= (256LL << 20)) {
+        if (prep.nviews > 0 && ntiles * (long long)sizeof(TilePlan) <= (256LL << 20)) {
             int rc = bs_ensure_dev(ctx, &ctx->fuse_plan, &ctx->fuse_plan_cap, (size_t)ntiles * sizeof(TilePlan));
             if (rc) return rc;
             a2.plan = (const TilePlan*)ctx->fuse_plan;
@@ -644,8 +611,6 @@ static int fuse_launch(bs_ctx* ctx, const FusePrepared& prep, const bs_fuse_para
         }
     }
     BS_CUDA(ctx, cudaGetLastError());
-    BS_CUDA(ctx, cudaEventRecord(ctx->fuse_slot_ev[prep.slot], ctx->stream));
-    ctx->fuse_slot_used[prep.slot] = true;
     return BS_OK;
 }
 
@@ -687,8 +652,11 @@ int bs_fuse_accumulate(bs_ctx* ctx, const bs_view* views, int n_views, const lon
         return bs_set_error(ctx, BS_ERR_UNSUPPORTED,
                             "bs_fuse_accumulate: only the weighted-average fusion types reduce by sum");
     BS_CUDA(ctx, cudaSetDevice(ctx->device));
+    int rc = bs_fuse_validate_blocks(ctx, 1, block_min, block_size, params);
+    if (!rc) rc = bs_fuse_validate(ctx, views, n_views, params);
+    if (rc) return rc;
     FusePrepared prep;
-    int rc = fuse_prepare(ctx, views, n_views, block_min, block_size, params, &prep);
+    rc = fuse_prepare(ctx, views, n_views, block_min, block_size, params, &prep);
     if (rc) return rc;
     prep.args.acc_wi = sum_wi_dev;
     prep.args.acc_w = sum_w_dev;

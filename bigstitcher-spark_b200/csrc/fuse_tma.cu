@@ -151,10 +151,10 @@ __device__ __forceinline__ void tmap_acquire(const CUtensorMap* tm) {
     asm volatile("fence.proxy.tensormap::generic.acquire.gpu [%0], 128;" ::"l"(tm) : "memory");
 }
 
-// The per-call tables (views, blocks, candidates, work records) travel from a mapped pinned buffer to device memory
-// by this kernel, NOT by cudaMemcpyAsync: a DMA copy would queue on the host->device copy engine behind every tile
-// upload already in flight (bs_volume_upload_async), and the plan / fusion kernels of the first blocks would wait for
-// ALL of the step's uploads.
+// The per-call tables of both fusion paths (here: views, blocks, candidates, work records; fuse.cu: LUT and views)
+// travel from a mapped pinned buffer to device memory by this kernel (bs_fuse_tables_commit), NOT by
+// cudaMemcpyAsync: a DMA copy would queue on the host->device copy engine behind every tile upload already in flight
+// (bs_volume_upload_async), and the plan / fusion kernels of the first blocks would wait for ALL of the step's uploads.
 __global__ void fuse_meta_copy_kernel(uint4* __restrict__ dst, const uint4* __restrict__ src_mapped, int n16) {
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n16; i += gridDim.x * blockDim.x) dst[i] = src_mapped[i];
 }
@@ -1022,12 +1022,16 @@ bool ensure_tmaps(bs_ctx* ctx, bs_volume& vol) {
 }
 
 struct Fuse2Ws {
+    // per-call tables of both fusion paths (bs_fuse_tables_reserve / _commit): a ring of mapped pinned host slots,
+    // each busy until the copy that reads it has run (meta_ev), and one device buffer
     static constexpr int kRing = 4;
-    void* meta_host[kRing] = {};      // pinned staging of one call's tables
+    void* meta_host[kRing] = {};
     size_t meta_host_cap[kRing] = {};
     cudaEvent_t meta_ev[kRing] = {};
     bool meta_used[kRing] = {};
     int next = 0;
+    int reserved = 0;                 // the slot of the last reserve and its size (a multiple of 16 bytes)
+    size_t reserved_bytes = 0;
     void* meta_dev = nullptr; size_t meta_dev_cap = 0;
     void* hdr = nullptr; size_t hdr_cap = 0;
     void* pool = nullptr; size_t pool_cap = 0;
@@ -1065,15 +1069,13 @@ constexpr size_t smem_bytes(bool general) {
            (size_t)NTEAMS * 2 * NST_T * WT_N * sizeof(float) + 1024;
 }
 
+// arguments validated by bs_fuse_validate
 bool eligible(bs_ctx* ctx, const bs_view* views, int n_views, const bs_fuse_params* p) {
-    const char* e = getenv("BS_FUSE_LEGACY");
-    if (e && *e && *e != '0') return false;
     const bool content = p->fusion_type == BS_FUSE_AVG_CONTENT || p->fusion_type == BS_FUSE_AVG_BLEND_CONTENT;
     if (!(p->fusion_type == BS_FUSE_AVG || p->fusion_type == BS_FUSE_AVG_BLEND || content)) return false;
     if (p->interpolation != 1 || p->blend_lut_n != 0) return false;
     for (int i = 0; i < n_views; ++i) {
         auto it = ctx->vols.find(views[i].vol_handle);
-        if (it == ctx->vols.end()) return false;   // the legacy path reports the error
         if (!ensure_tmaps(ctx, it->second)) return false;
         if (content) {
             // content weights ride along in the translation kernel only: whole (non-windowed) views, identity linear part
@@ -1156,10 +1158,6 @@ int fuse2_launch(bs_ctx* ctx, const bs_view* views, int n_views, int nb, const l
             d.whi[r] = hi + pad;
         }
     }
-    {
-        const char* e = getenv("BS_FUSE_GENERAL");
-        if (e && *e && *e != '0') general = true;
-    }
     // ---- blocks, candidates, work records, pool bound
     std::vector<BlockDev> hb((size_t)nb);
     std::vector<int> cand;
@@ -1224,43 +1222,25 @@ int fuse2_launch(bs_ctx* ctx, const bs_view* views, int n_views, int nb, const l
     const size_t off_cand = align_up(off_blocks + hb.size() * sizeof(BlockDev), 64);
     const size_t off_work = align_up(off_cand + cand.size() * sizeof(int), 64);
     const size_t meta_bytes = align_up(off_work + work.size() * sizeof(WorkRec), 64) + 64;
-    const int slot = W->next;
-    W->next = (slot + 1) % Fuse2Ws::kRing;
-    if (!W->meta_ev[slot]) BS_CUDA(ctx, cudaEventCreateWithFlags(&W->meta_ev[slot], cudaEventDisableTiming));
-    if (W->meta_used[slot]) BS_CUDA(ctx, cudaEventSynchronize(W->meta_ev[slot]));
-    if (W->meta_host_cap[slot] < meta_bytes) {
-        if (W->meta_host[slot]) cudaFreeHost(W->meta_host[slot]);
-        W->meta_host[slot] = nullptr;
-        W->meta_host_cap[slot] = 0;
-        const size_t cap = align_up(meta_bytes * 2, 1 << 16);
-        BS_CUDA(ctx, cudaHostAlloc(&W->meta_host[slot], cap, cudaHostAllocMapped));
-        W->meta_host_cap[slot] = cap;
-    }
-    int rc = bs_ensure_dev(ctx, &W->meta_dev, &W->meta_dev_cap, align_up(meta_bytes * 2, 1 << 16));
-    if (rc) return rc;
-    rc = bs_ensure_dev(ctx, &W->hdr, &W->hdr_cap, align_up((size_t)ntiles_total * sizeof(TileHdr) * 5 / 4, 1 << 16));
+    int rc = bs_ensure_dev(ctx, &W->hdr, &W->hdr_cap, align_up((size_t)ntiles_total * sizeof(TileHdr) * 5 / 4, 1 << 16));
     if (rc) return rc;
     rc = bs_ensure_dev(ctx, &W->pool, &W->pool_cap, align_up((size_t)std::max<long long>(pool_need, 1) * sizeof(ViewItem) * 5 / 4, 1 << 16));
     if (rc) return rc;
     if (!W->ctr) BS_CUDA(ctx, cudaMalloc((void**)&W->ctr, 64));
-    unsigned char* mh = (unsigned char*)W->meta_host[slot];
+    void* host = nullptr;
+    const void* dev = nullptr;
+    rc = bs_fuse_tables_reserve(ctx, meta_bytes, &host, &dev);
+    if (rc) return rc;
+    unsigned char* mh = (unsigned char*)host;
     if (!hv.empty()) memcpy(mh + off_views, hv.data(), hv.size() * sizeof(ViewDev));
     memcpy(mh + off_blocks, hb.data(), hb.size() * sizeof(BlockDev));
     if (!cand.empty()) memcpy(mh + off_cand, cand.data(), cand.size() * sizeof(int));
     memcpy(mh + off_work, work.data(), work.size() * sizeof(WorkRec));
-    {
-        void* mh_dev = nullptr;
-        BS_CUDA(ctx, cudaHostGetDevicePointer(&mh_dev, mh, 0));
-        const int n16 = (int)((meta_bytes + 15) / 16);
-        bs_launch_scope scope(ctx, "fuse_meta");
-        fuse_meta_copy_kernel<<<std::min(64, (n16 + 255) / 256), 256, 0, ctx->stream>>>((uint4*)W->meta_dev, (const uint4*)mh_dev, n16);
-    }
-    BS_CUDA(ctx, cudaGetLastError());
-    BS_CUDA(ctx, cudaEventRecord(W->meta_ev[slot], ctx->stream));
-    W->meta_used[slot] = true;
+    rc = bs_fuse_tables_commit(ctx);
+    if (rc) return rc;
     BS_CUDA(ctx, cudaMemsetAsync(W->ctr, 0, 64, ctx->stream));
 
-    const unsigned char* md = (const unsigned char*)W->meta_dev;
+    const unsigned char* md = (const unsigned char*)dev;
     const ViewDev* dviews = (const ViewDev*)(md + off_views);
     const BlockDev* dblocks = (const BlockDev*)(md + off_blocks);
     const int use_blend = (p->fusion_type == BS_FUSE_AVG_BLEND || p->fusion_type == BS_FUSE_AVG_BLEND_CONTENT) ? 1 : 0;
@@ -1303,10 +1283,7 @@ int fuse2_launch(bs_ctx* ctx, const bs_view* views, int n_views, int nb, const l
     a.hdr = (const TileHdr*)W->hdr;
     a.pool = (const ViewItem*)W->pool;
     a.use_blend = use_blend;
-    {
-        const char* e = getenv("BS_FUSE_NO_XYAFF");
-        a.xyaff = (xyaff && !(e && *e && *e != '0')) ? 1 : 0;
-    }
+    a.xyaff = xyaff ? 1 : 0;
     a.work_ctr = W->ctr + 2;
     a.nwork = (int)work.size();
     a.ctop = p->out_dtype == BS_DTYPE_U8 ? 255.0 : 65535.0;
@@ -1341,16 +1318,6 @@ __global__ void fuse_bswap_kernel(void* data, size_t n, int es) {
     }
 }
 
-int validate_blocks(bs_ctx* ctx, int nb, const long long* bmin, const long long* bsize, const bs_fuse_params* p) {
-    if (!bmin || !bsize || !p) return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse: NULL argument");
-    if (nb < 0) return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse_blocks: n_blocks < 0");
-    for (int b = 0; b < nb; ++b)
-        for (int d = 0; d < 3; ++d)
-            if (bsize[3 * b + d] <= 0 || bsize[3 * b + d] > 0x7fffffffLL)
-                return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse: bad block_size[%d]=%lld", d, bsize[3 * b + d]);
-    return BS_OK;
-}
-
 // device outputs; chooses the TMA kernels or the generic tile kernel
 int fuse_blocks_dev(bs_ctx* ctx, const bs_view* views, int n_views, int nb, const long long* bmin, const long long* bsize,
                     const bs_fuse_params* p, void* const* outs_dev) {
@@ -1373,6 +1340,48 @@ int fuse_blocks_dev(bs_ctx* ctx, const bs_view* views, int n_views, int nb, cons
 }
 
 }  // namespace
+
+int bs_fuse_tables_reserve(bs_ctx* ctx, size_t bytes, void** host, const void** dev) {
+    Fuse2Ws* W = ws_of(ctx);
+    bytes = align_up(bytes, 16);
+    const int slot = W->next;
+    W->next = (slot + 1) % Fuse2Ws::kRing;
+    if (!W->meta_ev[slot]) BS_CUDA(ctx, cudaEventCreateWithFlags(&W->meta_ev[slot], cudaEventDisableTiming));
+    if (W->meta_used[slot]) BS_CUDA(ctx, cudaEventSynchronize(W->meta_ev[slot]));
+    const size_t cap = align_up(bytes * 2, 1 << 16);
+    if (W->meta_host_cap[slot] < bytes) {
+        if (W->meta_host[slot]) cudaFreeHost(W->meta_host[slot]);
+        W->meta_host[slot] = nullptr;
+        W->meta_host_cap[slot] = 0;
+        BS_CUDA(ctx, cudaHostAlloc(&W->meta_host[slot], cap, cudaHostAllocMapped));
+        W->meta_host_cap[slot] = cap;
+    }
+    if (W->meta_dev_cap < bytes) {   // bs_ensure_dev lets the kernels reading the old buffer finish first
+        int rc = bs_ensure_dev(ctx, &W->meta_dev, &W->meta_dev_cap, cap);
+        if (rc) return rc;
+    }
+    W->reserved = slot;
+    W->reserved_bytes = bytes;
+    *host = W->meta_host[slot];
+    *dev = W->meta_dev;
+    return BS_OK;
+}
+
+int bs_fuse_tables_commit(bs_ctx* ctx) {
+    Fuse2Ws* W = ws_of(ctx);
+    const int slot = W->reserved;
+    void* src = nullptr;
+    BS_CUDA(ctx, cudaHostGetDevicePointer(&src, W->meta_host[slot], 0));
+    const int n16 = (int)(W->reserved_bytes / 16);
+    {
+        bs_launch_scope scope(ctx, "fuse_meta");
+        fuse_meta_copy_kernel<<<std::min(64, (n16 + 255) / 256), 256, 0, ctx->stream>>>((uint4*)W->meta_dev, (const uint4*)src, n16);
+    }
+    BS_CUDA(ctx, cudaGetLastError());
+    BS_CUDA(ctx, cudaEventRecord(W->meta_ev[slot], ctx->stream));
+    W->meta_used[slot] = true;
+    return BS_OK;
+}
 
 void bs_fuse2_free(bs_ctx* ctx) {
     Fuse2Ws* W = (Fuse2Ws*)ctx->fuse2;
@@ -1400,7 +1409,7 @@ int bs_fuse_blocks(bs_ctx* ctx, const bs_view* views, int n_views, int n_blocks,
                    const long long* block_size, const bs_fuse_params* params, void* const* outs, int out_on_device) {
     if (!ctx) return BS_ERR_ARG;
     std::lock_guard<std::mutex> lk(ctx->mu);
-    int rc = validate_blocks(ctx, n_blocks, block_min, block_size, params);
+    int rc = bs_fuse_validate_blocks(ctx, n_blocks, block_min, block_size, params);
     if (rc) return rc;
     if (n_blocks > 0 && !outs) return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse_blocks: outs is NULL");
     for (int b = 0; b < n_blocks; ++b)
@@ -1481,7 +1490,7 @@ int bs_fuse_block_to_volume(bs_ctx* ctx, const bs_view* views, int n_views, cons
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
         for (int d = 0; d < 3; ++d)
-            if (block_size[d] <= 0 || block_size[d] > 0x7fffffffLL)
+            if (!bs_fuse_block_dim_ok(block_size[d]))
                 return bs_set_error(ctx, BS_ERR_ARG, "bs_fuse_block_to_volume: bad block_size");
         BS_CUDA(ctx, cudaSetDevice(ctx->device));
         BS_CUDA(ctx, cudaMalloc(&dev, (size_t)block_size[0] * block_size[1] * block_size[2] * bs_out_elem_size(params->out_dtype)));

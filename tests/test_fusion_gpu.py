@@ -400,20 +400,23 @@ def test_oblique_rotation_uses_the_fully_general_kernel(ctx):
     assert np.count_nonzero(want) > 0.6 * want.size
 
 
-def test_xy_affine_path_equals_generic_path(ctx, monkeypatch):
+def test_xy_affine_path_equals_generic_path(ctx):
     """Rotation about z + xy scale: the z-marching xy-affine tiles and the per-voxel generic tiles agree to rounding."""
     views = _scene(seed=34, n=3, shape=(72, 80, 96), rot=0.5)
     S = np.diag([1.01, 0.99, 1.0, 1.0])
     views = [(v, (S @ np.vstack([M, [0, 0, 0, 1]]))[:3]) for v, M in views]
-    handles = [ctx.volume_upload(v) for v, _ in views]
+    # xy-affine tiles run only when EVERY view of the call is xy-affine: a uint16 view (x size a multiple of 8, so
+    # the call stays on the TMA kernels) rotated about x and placed far outside the block is culled from every tile
+    # but sends the whole call to the per-voxel tiles
+    far = synth.translation((5000.0, 5000.0, 5000.0))
+    far = (np.vstack([far, [0, 0, 0, 1]]) @ np.vstack([synth.rot_x(0.7, center_xyz=(0, 8, 8)), [0, 0, 0, 1]]))[:3]
+    handles = [ctx.volume_upload(v) for v, _ in views] + [ctx.volume_upload(np.ones((16, 16, 16), np.uint16))]
     gv = []
-    for (vol, M), h in zip(views, handles):
+    for M, h in zip([M for _, M in views] + [far], handles):
         border, rng = fo.adjust_blending(M)
         gv.append(dict(src_to_world=M, vol_handle=h, blend_border=border, blend_range=rng))
-    a = ctx.fuse_block(gv, (0, 0, 0), (250, 80, 72))
-    monkeypatch.setenv("BS_FUSE_NO_XYAFF", "1")
+    a = ctx.fuse_block(gv[:-1], (0, 0, 0), (250, 80, 72))
     b = ctx.fuse_block(gv, (0, 0, 0), (250, 80, 72))
-    monkeypatch.delenv("BS_FUSE_NO_XYAFF")
     assert np.count_nonzero(a) > 0.6 * a.size
     err = np.abs(a - b) / np.maximum(np.abs(b), 250.0)
     assert err.max() < 2e-5
