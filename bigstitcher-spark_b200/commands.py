@@ -17,6 +17,7 @@
   clear_registrations     J/ClearRegistrations.java               (drop the latest <ViewTransform>s)
   transform_points        J/TransformPoints.java                  (view pixel coordinates -> world, host only)
   split_images            J/SplitDatasets.java                    (overlapping sub-views, split loader, fake points)
+  estimate_bounding_box   (no upstream command; BigStitcher's BoundingBoxMinFilterThreshold) (named box from the data)
 
 Every command reads its images through viewsource.py, so `bdv.n5` and `bdv.multimg.zarr` datasets both work.
 
@@ -106,6 +107,20 @@ def estimate_multires_pyramid(dims_xyz, anisotropy_factor=float("nan"), min_size
     return steps
 
 
+def views_bounding_box(data, view_ids, anisotropy_factor=float("nan")):
+    """The box of all ``view_ids`` (Import.getBoundingBox without a name, J/util/Import.java:39-66): the union of the
+    views' transformed bounding boxes (fusion.transformed_bounding_box) under their registrations, adjusted for
+    ``anisotropy_factor``.  (lo, hi) float64 [3] of whole world coordinates, both inclusive."""
+    lo = np.full(3, np.inf)
+    hi = np.full(3, -np.inf)
+    regs = bf.adjust_all_transforms({v: data.model(*v) for v in view_ids}, anisotropy_factor)
+    for v, M in regs.items():
+        bmin, bmax = bf.transformed_bounding_box(data.setups[v[1]].size, M)
+        lo = np.minimum(lo, bmin)
+        hi = np.maximum(hi, bmax)
+    return lo, hi
+
+
 def create_fusion_container(xml_path, out_path, block_size=(128, 128, 128), dtype="float32", min_intensity=None,
                             max_intensity=None, preserve_anisotropy=False, anisotropy_factor=float("nan"),
                             storage=None, downsamplings=(), multi_res=False, compression="zstd", bounding_box=None,
@@ -133,13 +148,7 @@ def create_fusion_container(xml_path, out_path, block_size=(128, 128, 128), dtyp
     data = SpimData2.load(xml_path)
     af = anisotropy_factor if preserve_anisotropy else float("nan")
     if bounding_box is None:
-        lo = np.full(3, np.inf)
-        hi = np.full(3, -np.inf)
-        regs = bf.adjust_all_transforms({v: data.model(*v) for v in data.view_ids()}, af)
-        for v, M in regs.items():
-            bmin, bmax = bf.transformed_bounding_box(data.setups[v[1]].size, M)
-            lo = np.minimum(lo, bmin)
-            hi = np.maximum(hi, bmax)
+        lo, hi = views_bounding_box(data, data.view_ids(), af)
     else:
         boxes = data.bounding_boxes()
         if bounding_box not in boxes:
@@ -692,12 +701,12 @@ def interestpoint_blocks(dims_xyz, block_size):
     return out
 
 
-def _check_device_memory(ctx, nbytes, what):
-    import torch
-    free, _ = torch.cuda.mem_get_info(ctx.device)
+def _check_device_memory(ctx, nbytes, what, command="detect-interestpoints",
+                         advice="use a larger --downsampleXY / --downsampleZ"):
+    free = ctx.memory_free()
     if nbytes > free:
-        raise MemoryError(f"detect-interestpoints: {what} needs {nbytes / 2**30:.2f} GiB on device {ctx.device}, "
-                          f"{free / 2**30:.2f} GiB are free; use a larger --downsampleXY / --downsampleZ")
+        raise MemoryError(f"{command}: {what} needs {nbytes / 2**30:.2f} GiB on device {ctx.device}, "
+                          f"{free / 2**30:.2f} GiB are free; {advice}")
 
 
 def _detect_view(ctx, src, view, level, remaining, mt, sigma, threshold, min_intensity, max_intensity, find_max,
@@ -1888,3 +1897,127 @@ def split_images(xml_path, target_image_size, target_overlap, xml_out=None, disa
     os.makedirs(os.path.dirname(os.path.abspath(xml_out)), exist_ok=True)
     new.save(xml_out)
     return result
+
+
+# --------------------------------------------------------------------------------------------- estimate-bounding-box
+BBOX_SLAB = 32                 # downsampled z-planes fused per call
+BBOX_BYTES_PER_VOXEL = 12      # fused volume, filter output and the filter's ping-pong buffer, float32 each
+
+
+def bounding_box_grid(lo, hi, ds):
+    """The downsampled grid over the world box [lo, hi] (PARITY_GAPS B2): (g_min, dims), int64 [3] each, with
+    g_min = floor(lo / ds), g_max = ceil(hi / ds) and dims = g_max - g_min + 1; voxel i is world point ds (g_min + i)."""
+    lo = np.asarray(lo, dtype=np.int64)
+    hi = np.asarray(hi, dtype=np.int64)
+    g_min = np.floor_divide(lo, ds)
+    return g_min, -np.floor_divide(-hi, ds) - g_min + 1
+
+
+def fuse_downsampled(ctx, data, src, view_ids, ds, g_min, dims, out):
+    """AVG_BLEND fusion of ``view_ids`` with n-linear interpolation, in float32, on the grid of bounding_box_grid
+    (PARITY_GAPS B2), written into ``out`` ([z, y, x] float32 of ``dims``: a device tensor, e.g. from
+    Context.volume_empty).  Each view's model is its registration scaled by 1 / ds (fusion.adjust_all_transforms) composed
+    with the mipmap level ViewUtil's best-resolution rule picks for it, blending from adjust_blending of that model.  The
+    grid is fused in slabs of BBOX_SLAB z-planes.  Each view's level volume is staged whole, once, as float32: that runs
+    the generic fusion kernel, because the uint16 TMA kernels sample models that magnify the source (ds > 1) at the
+    wrong voxels (DESIGN.md, estimate-bounding-box)."""
+    view_ids = sorted(view_ids)
+    regs = bf.adjust_all_transforms({v: data.model(*v) for v in view_ids}, downsampling=float(ds))
+    info = {}
+    for v in view_ids:
+        factors, mts = src.mipmap_info(v)
+        lvl = bf.best_mipmap_level(regs[v], factors, mts)
+        m = _compose(regs[v], mts[lvl])
+        info[v] = dict(level=lvl, dims=src.level_dims(v, lvl), model=m, blending=bf.adjust_blending(m))
+    vdims = {v: info[v]["dims"] for v in view_ids}
+    vregs = {v: info[v]["model"] for v in view_ids}
+    params = ctx.fuse_params("AVG_BLEND", 1, native.DTYPE_F32)
+    g_min = np.asarray(g_min, dtype=np.int64)
+    nx, ny, nz = (int(d) for d in dims)
+    staged = {}
+    try:
+        for z0 in range(0, nz, BBOX_SLAB):
+            sz = min(BBOX_SLAB, nz - z0)
+            lo = g_min + np.array([0, 0, z0])
+            hi = g_min + np.array([nx - 1, ny - 1, z0 + sz - 1])
+            views = []
+            for v in bf.find_overlapping_views(vdims, vregs, lo, hi, view_ids):
+                if v not in staged:
+                    staged[v] = ctx.volume_upload(src.read_volume(v, info[v]["level"]).astype(np.float32))
+                border, rng = info[v]["blending"]
+                views.append(dict(src_to_world=info[v]["model"], vol_handle=staged[v], blend_border=border,
+                                  blend_range=rng))
+            ctx.fuse_blocks(views, [tuple(int(x) for x in lo)], [(nx, ny, sz)], params, outs=[out[z0:z0 + sz]])
+    finally:
+        for h in staged.values():
+            ctx.volume_free(h)
+
+
+def estimate_bounding_box(xml_path, ctx: Context, name, background_intensity=5.0, discarded_object_size=25,
+                          downsampling=4, view_selection=None, dry_run=False):
+    """`./estimate-bounding-box -x dataset.xml -b name [--background 5] [--minObjectSize 25] [--downsampling 4]
+    [view selection] [--dryRun]`: the "automatic bounding box through image filtering" of BigStitcher's GUI (mvrecon
+    BoundingBoxMinFilterThreshold, recalled; PARITY_GAPS B1-B6), stored as the XML's <BoundingBoxDefinition> ``name``
+    for `create-fusion-container -b name`.  BigStitcher-Spark has no such command.  The defaults are the GUI's, recalled.
+
+    1. The selected views (``view_selection``: keyword arguments of SpimData2.select_views, default all) are fused at
+       1 / ``downsampling`` on the device (fuse_downsampled) over the box of those views (views_bounding_box).
+    2. t = mn + (mx - mn) ``background_intensity`` / 100 from the fused volume's min mn and max mx.
+    3. A box minimum filter of radius r = max(1, floor(``discarded_object_size`` / downsampling + 0.5)) on every axis
+       (bs_min_filter) removes objects narrower than about the size (beads); the box is clipped to the volume.
+    4. The voxels of the filtered volume above t (strictly) give an index box; one downsampled voxel is added on every
+       side, it is mapped back to world coordinates and intersected with the views' box.
+
+    The definition replaces any earlier one of that name; the XML is saved with a `~1` backup unless ``dry_run``.
+    Returns dict(min, max (world, inclusive), threshold, min_max (mn, mx), radius, dims (of the downsampled grid),
+    count (voxels above t)).  ValueError, with the XML untouched, for an empty name, a downsampling that is not an
+    integer >= 1, a background outside [0, 100], a negative object size, no selected views, and when no voxel is above
+    the threshold.  MemoryError, before anything is fused, when the device cannot hold 12 bytes per grid voxel plus the
+    float32 source levels."""
+    if not name:
+        raise ValueError("estimate-bounding-box: the bounding box needs a name (-b)")
+    if isinstance(downsampling, bool) or int(downsampling) != downsampling or downsampling < 1:
+        raise ValueError(f"estimate-bounding-box: --downsampling {downsampling} is not an integer >= 1")
+    if not 0.0 <= float(background_intensity) <= 100.0:
+        raise ValueError(f"estimate-bounding-box: --background {background_intensity} outside [0, 100]")
+    if not float(discarded_object_size) >= 0.0:
+        raise ValueError(f"estimate-bounding-box: --minObjectSize {discarded_object_size} is negative")
+    ds = int(downsampling)
+    data = SpimData2.load(xml_path)
+    views = data.select_views(**view_selection) if view_selection else data.view_ids()
+    if not views:
+        raise ValueError("estimate-bounding-box: no views selected")
+    lo, hi = (b.astype(np.int64) for b in views_bounding_box(data, views))
+    g_min, dims = bounding_box_grid(lo, hi, ds)
+    src = bvs.open_views(data)
+    source_bytes = 0
+    for v in views:
+        factors, mts = src.mipmap_info(v)
+        reg = bf.adjust_all_transforms({v: data.model(*v)}, downsampling=float(ds))[v]
+        source_bytes += 4 * int(np.prod(src.level_dims(v, bf.best_mipmap_level(reg, factors, mts))))
+    _check_device_memory(ctx, BBOX_BYTES_PER_VOXEL * int(np.prod(dims)) + source_bytes,
+                         f"the {dims[0]}x{dims[1]}x{dims[2]} grid at downsampling {ds}", "estimate-bounding-box",
+                         "use a larger --downsampling")
+    radius = max(1, int(math.floor(float(discarded_object_size) / ds + 0.5)))
+    fused, buf = ctx.volume_empty(dims)
+    handles = [fused]
+    try:
+        fuse_downsampled(ctx, data, src, views, ds, g_min, dims, buf)
+        mn, mx = ctx.volume_min_max(fused)
+        t = mn + (mx - mn) * float(background_intensity) / 100.0
+        handles.append(ctx.min_filter(fused, (radius, radius, radius)))
+        i_min, i_max, count = ctx.threshold_bbox(handles[-1], t)
+    finally:
+        for h in handles:
+            ctx.volume_free(h)
+        del buf
+    if count == 0:
+        raise ValueError(f"estimate-bounding-box: no voxel of the filtered fusion is above the threshold {t!r} "
+                         f"(min {mn!r}, max {mx!r}, --background {background_intensity}); the XML is unchanged")
+    bb_min = np.maximum(ds * (g_min + np.asarray(i_min, dtype=np.int64) - 1), lo)
+    bb_max = np.minimum(ds * (g_min + np.asarray(i_max, dtype=np.int64) + 1), hi)
+    data.set_bounding_box(name, bb_min, bb_max, replace=True)
+    if not dry_run:
+        data.save(xml_path)
+    return dict(min=[int(v) for v in bb_min], max=[int(v) for v in bb_max], threshold=t, min_max=(mn, mx),
+                radius=radius, dims=[int(v) for v in dims], count=int(count))

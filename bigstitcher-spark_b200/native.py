@@ -141,7 +141,7 @@ SYMBOLS = [
     "bs_descriptors_build", "bs_descriptors_free", "bs_descriptors_neighbors", "bs_descriptors_match",
     "bs_solve_tiles",
     "bs_intensity_pair_candidates", "bs_intensity_candidates_get", "bs_intensity_candidates_free", "bs_intensity_ransac",
-    "bs_intensity_apply",
+    "bs_intensity_apply", "bs_min_filter", "bs_volume_min_max", "bs_threshold_bbox",
 ]
 
 #: fixed parameters of the reference's non-rigid fusion (J/SparkNonRigidFusion.java:373-383): control-point distance
@@ -231,6 +231,9 @@ def load_library():
     lib.bs_intensity_candidates_free.argtypes = [vp, ull]
     lib.bs_intensity_ransac.argtypes = [vp, ull, ll, ip, dbl, P(dbl), P(dbl), P(ip)]
     lib.bs_intensity_apply.argtypes = [vp, ull, P(ll), P(ll), P(dbl), P(ip), P(dbl), P(dbl), P(ull)]
+    lib.bs_min_filter.argtypes = [vp, ull, P(ip), P(ull)]
+    lib.bs_volume_min_max.argtypes = [vp, ull, P(dbl)]
+    lib.bs_threshold_bbox.argtypes = [vp, ull, dbl, P(ll), P(ll), P(ll)]
     _lib = lib
     return lib
 
@@ -481,6 +484,19 @@ class Context:
         h = C.c_ulonglong()
         self._check(self.lib.bs_volume_wrap(self.h, p, dims, dtype, C.byref(h)))
         return h.value
+
+    def volume_empty(self, dims_xyz):
+        """A new resident float32 volume of uninitialised device memory, allocated by torch on this context's device
+        and wrapped (bs_volume_wrap).  Returns (handle, tensor [z, y, x]); the tensor owns the memory and must outlive
+        the handle."""
+        import torch
+        t = torch.empty(tuple(int(v) for v in dims_xyz)[::-1], dtype=torch.float32, device=f"cuda:{self.device}")
+        return self.volume_wrap(t, dims_xyz, DTYPE_F32), t
+
+    def memory_free(self) -> int:
+        """Free bytes on this context's device."""
+        import torch
+        return int(torch.cuda.mem_get_info(self.device)[0])
 
     def downsample(self, handle: int, factors_xyz) -> int:
         f = (C.c_int * 3)(*[int(v) for v in factors_xyz])
@@ -873,6 +889,28 @@ class Context:
         self._check(self.lib.bs_intensity_apply(self.h, handle, fd, wm, m, n, ca.ctypes.data_as(D), cb.ctypes.data_as(D),
                                                 C.byref(h)))
         return h.value
+
+    # -- estimate-bounding-box
+    def min_filter(self, handle: int, radius_xyz) -> int:
+        """New float32 volume: the minimum over the box of ``radius_xyz`` around every voxel, clipped to the volume
+        (NaN neighbours ignored) of a resident float32 volume."""
+        r = (C.c_int * 3)(*[int(v) for v in radius_xyz])
+        h = C.c_ulonglong()
+        self._check(self.lib.bs_min_filter(self.h, handle, r, C.byref(h)))
+        return h.value
+
+    def volume_min_max(self, handle: int):
+        """(min, max) of a resident float32 volume over its voxels that are not NaN; (nan, nan) when there are none."""
+        out = (C.c_double * 2)()
+        self._check(self.lib.bs_volume_min_max(self.h, handle, out))
+        return out[0], out[1]
+
+    def threshold_bbox(self, handle: int, t: float):
+        """(min_xyz, max_xyz, count) of the voxels of a resident float32 volume that are > ``t`` (compared in double);
+        (-1, -1, -1) twice and 0 when there are none."""
+        mn, mx, n = (C.c_longlong * 3)(), (C.c_longlong * 3)(), C.c_longlong()
+        self._check(self.lib.bs_threshold_bbox(self.h, handle, float(t), mn, mx, C.byref(n)))
+        return tuple(mn), tuple(mx), n.value
 
     @staticmethod
     def comm_unique_id() -> bytes:

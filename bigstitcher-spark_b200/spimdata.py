@@ -529,11 +529,16 @@ class SpimData2:
                                        for k in ("min", "max"))
         return out
 
-    def set_bounding_box(self, name, bb_min, bb_max):
-        """Append a <BoundingBoxDefinition> (earlier ones of the same name stay, and lose to this one on reading)."""
+    def set_bounding_box(self, name, bb_min, bb_max, replace=False):
+        """Append a <BoundingBoxDefinition> (earlier ones of the same name stay, and lose to this one on reading;
+        ``replace`` removes them instead)."""
         bbs = self.root.find("BoundingBoxes")
         if bbs is None:
             bbs = ET.SubElement(self.root, "BoundingBoxes")
+        if replace:
+            for b in bbs.findall("BoundingBoxDefinition"):
+                if b.get("name") == str(name):
+                    bbs.remove(b)
         b = ET.SubElement(bbs, "BoundingBoxDefinition", name=str(name))
         ET.SubElement(b, "min").text = " ".join(str(int(v)) for v in bb_min)
         ET.SubElement(b, "max").text = " ".join(str(int(v)) for v in bb_max)

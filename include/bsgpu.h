@@ -502,6 +502,24 @@ int bs_intensity_apply(bs_ctx* ctx, unsigned long long vol_handle, const long lo
                        const double level_to_full[12], const int n_cells[3], const double* coeff_a, const double* coeff_b,
                        unsigned long long* out_handle);
 
+/* ---------------------------------------------------------------- estimate-bounding-box
+ * The filter and reductions of mvrecon's BoundingBoxMinFilterThreshold on a resident FLOAT32 volume (the downsampled
+ * fusion).  Additive: the ABI version stays 107.  BS_ERR_ARG for an unknown handle, a volume that is not F32 or larger
+ * than 2^31 - 1 x 2^31 - 1 x 65535, a negative radius and NULL outputs. */
+
+/* out = the minimum over the box |q - p|_inf <= radius (per axis {x, y, z}), clipped to the volume (a mirror or border
+ * extension gives the same minimum); a NaN neighbour is ignored as by fminf (NaN only when the whole box is NaN).
+ * Computed as 1-D passes along x, then y, then z; min is exact, so the result is bit-identical to any evaluation order.
+ * A radius of 0 leaves that axis as it is.  New F32 volume handle; needs two volume-sized device buffers while it runs.
+ * Profile tag "min_filter". */
+int bs_min_filter(bs_ctx* ctx, unsigned long long vol_handle, const int radius[3], unsigned long long* out_handle);
+/* out = {min, max} over the voxels that are not NaN; both NaN when there are none.  Profile tag "min_max". */
+int bs_volume_min_max(bs_ctx* ctx, unsigned long long vol_handle, double out[2]);
+/* the voxels with (double)v > t: their count and the smallest / largest index per axis {x, y, z} (-1 and a count of 0
+ * when there are none).  Profile tag "threshold_bbox". */
+int bs_threshold_bbox(bs_ctx* ctx, unsigned long long vol_handle, double t, long long min[3], long long max[3],
+                      long long* count);
+
 #ifdef __cplusplus
 }
 #endif

@@ -813,3 +813,30 @@ JF(jlong, intensityApply)(JNIEnv* env, jclass, jlong ctx, jlong handle, jlongArr
     return failed(env, ctx, bs_intensity_apply(C(ctx), (unsigned long long)handle, fd, wm, m, n, ca.data(), cb.data(), &h))
                ? 0 : (jlong)h;
 }
+
+// ---------------------------------------------------------------------------------------- estimate-bounding-box
+// a new float32 volume: the box minimum of radius[3] {x, y, z} of a resident float32 volume (BoundingBoxMinFilterThreshold)
+JF(jlong, minFilter)(JNIEnv* env, jclass, jlong ctx, jlong handle, jintArray radius) {
+    jint r[3];
+    env->GetIntArrayRegion(radius, 0, 3, r);
+    const int rr[3] = {r[0], r[1], r[2]};
+    unsigned long long h = 0;
+    return failed(env, ctx, bs_min_filter(C(ctx), (unsigned long long)handle, rr, &h)) ? 0 : (jlong)h;
+}
+
+// out: double[2] {min, max} over the voxels that are not NaN
+JF(void, volumeMinMax)(JNIEnv* env, jclass, jlong ctx, jlong handle, jdoubleArray out) {
+    double mm[2];
+    if (failed(env, ctx, bs_volume_min_max(C(ctx), (unsigned long long)handle, mm))) return;
+    env->SetDoubleArrayRegion(out, 0, 2, mm);
+}
+
+// the voxels > t: min / max long[3] {x, y, z} (-1 when none); returns their count
+JF(jlong, thresholdBbox)(JNIEnv* env, jclass, jlong ctx, jlong handle, jdouble t, jlongArray min, jlongArray max) {
+    long long mn[3], mx[3], n = 0;
+    if (failed(env, ctx, bs_threshold_bbox(C(ctx), (unsigned long long)handle, t, mn, mx, &n))) return 0;
+    const jlong a[3] = {mn[0], mn[1], mn[2]}, b[3] = {mx[0], mx[1], mx[2]};
+    env->SetLongArrayRegion(min, 0, 3, a);
+    env->SetLongArrayRegion(max, 0, 3, b);
+    return (jlong)n;
+}

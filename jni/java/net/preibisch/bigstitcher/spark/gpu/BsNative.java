@@ -138,4 +138,11 @@ public final class BsNative
 	/** affine-fusion --intensityN5Path: a new float32 volume a(q) v + b(q) of a (windowed) level volume */
 	public static native long intensityApply( long ctx, long handle, long[] fullDims, long[] windowMin, double[] levelToFull,
 			int[] nCells, double[] coeffA, double[] coeffB );
+
+	/** estimate-bounding-box (BoundingBoxMinFilterThreshold): a new float32 volume, the box minimum of radius {x, y, z} */
+	public static native long minFilter( long ctx, long handle, int[] radius );
+	/** out = {min, max} of a float32 volume over its voxels that are not NaN */
+	public static native void volumeMinMax( long ctx, long handle, double[] out );
+	/** the voxels > t of a float32 volume: min / max {x, y, z} (-1 when none); returns their count */
+	public static native long thresholdBbox( long ctx, long handle, double t, long[] min, long[] max );
 }
