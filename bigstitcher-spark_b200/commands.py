@@ -18,6 +18,7 @@
   transform_points        J/TransformPoints.java                  (view pixel coordinates -> world, host only)
   split_images            J/SplitDatasets.java                    (overlapping sub-views, split loader, fake points)
   estimate_bounding_box   (no upstream command; BigStitcher's BoundingBoxMinFilterThreshold) (named box from the data)
+  extract_psfs            (no upstream command; BigStitcher's PSFExtraction) (per-view bead PSFs, TIFF + the XML)
 
 Every command reads its images through viewsource.py, so `bdv.n5` and `bdv.multimg.zarr` datasets both work.
 
@@ -38,7 +39,7 @@ from . import n5 as bn5
 from . import zarr as bzarr
 from . import matching as bm
 from . import intensity as bint
-from . import native, solver as bsolver, split as bsplit, stitching as bst, viewsource as bvs
+from . import native, solver as bsolver, split as bsplit, stitching as bst, tiff as btiff, viewsource as bvs
 from .native import Context
 from .spimdata import FILEMAP_LOADER, SpimData2, fusion_project
 
@@ -2021,3 +2022,162 @@ def estimate_bounding_box(xml_path, ctx: Context, name, background_intensity=5.0
         data.save(xml_path)
     return dict(min=[int(v) for v in bb_min], max=[int(v) for v in bb_max], threshold=t, min_max=(mn, mx),
                 radius=radius, dims=[int(v) for v in dims], count=int(count))
+
+
+# --------------------------------------------------------------------------------------------- extract-psfs
+PSF_DIR = "psfs"               # next to the XML (its base path), one TIFF per view
+PSF_SLAB_BYTES = 1 << 30       # largest s0 window of one run of points (psf_runs; one point's box may be larger)
+
+
+def psf_file_name(view):
+    """The TIFF of one view's PSF (PARITY_GAPS Q4)."""
+    return f"psf_t{int(view[0])}_vs{int(view[1])}.tif"
+
+
+def _psf_tap_boxes(loc, psf_size, full_dims):
+    """Per point, the inclusive box of every s0 voxel its PSF samples can touch: floor(p) - h - 1 .. floor(p) + h + 2
+    per axis (a voxel to spare for p + o rounding up), clipped to the view, where the border extension puts every tap
+    outside it.  Returns (lo, hi), int64 (n, 3) each."""
+    h = (np.asarray(psf_size, dtype=np.int64) - 1) // 2
+    full = np.asarray(full_dims, dtype=np.int64)
+    b = np.floor(np.asarray(loc, dtype=np.float64).reshape(-1, 3)).astype(np.int64)
+    return np.clip(b - h - 1, 0, full - 1), np.clip(b + h + 2, 0, full - 1)
+
+
+def psf_runs(loc, psf_size, full_dims, max_voxels):
+    """Runs of consecutive points (in the order given) with the window each needs, [(start, stop, window_min int64[3],
+    window_size int64[3])]: a run's window is the box of its points' tap boxes (_psf_tap_boxes), and a run ends before
+    the point that would make its window exceed ``max_voxels``."""
+    lo, hi = (a.tolist() for a in _psf_tap_boxes(loc, psf_size, full_dims))
+    out, start, wlo, whi = [], 0, None, None
+    for i in range(len(lo)):
+        if wlo is None:
+            wlo, whi = list(lo[i]), list(hi[i])
+            continue
+        nlo = [min(wlo[d], lo[i][d]) for d in range(3)]
+        nhi = [max(whi[d], hi[i][d]) for d in range(3)]
+        if math.prod(nhi[d] - nlo[d] + 1 for d in range(3)) > max_voxels:
+            out.append((start, i, np.array(wlo), np.array(whi) - wlo + 1))
+            start, wlo, whi = i, list(lo[i]), list(hi[i])
+        else:
+            wlo, whi = nlo, nhi
+    if wlo is not None:
+        out.append((start, len(lo), np.array(wlo), np.array(whi) - wlo + 1))
+    return out
+
+
+def psf_slabs(loc, psf_size, full_dims, max_voxels):
+    """The upload plan of one view (PARITY_GAPS Q2), [(start, stop, window_min, window_size)] over the points in the
+    order given (ascending id, the order of the float64 sum).  Ids need not follow space (`--maxSpots` numbers points by
+    intensity), so the runs of psf_runs can overlap and read the view many times over.  When their windows add up to
+    more than the box of all the points' taps, that box is read once instead, as one run of every point.  Either way
+    the plan reads at most that box, whatever the id order."""
+    runs = psf_runs(loc, psf_size, full_dims, max_voxels)
+    lo, hi = _psf_tap_boxes(loc, psf_size, full_dims)
+    if len(lo) == 0:
+        return runs
+    ulo, usize = lo.min(axis=0), hi.max(axis=0) - lo.min(axis=0) + 1
+    if sum(int(np.prod(r[3])) for r in runs) > int(np.prod(usize)):
+        return [(0, len(lo), ulo, usize)]
+    return runs
+
+
+def _psf_points(ips, view, label, all_points):
+    """(ascending ids, their full-resolution locations) of one view's points of ``label`` that extract-psfs averages
+    (PARITY_GAPS Q1): every point with ``all_points``, else those with at least one correspondence of that label."""
+    ids, loc = ips.ids[(view, label)], ips.loc[(view, label)]
+    order = np.argsort(ids, kind="stable")
+    ids, loc = ids[order], loc[order]
+    if not all_points:
+        rows, _ = ips.table[(view, label)]
+        keep = np.isin(ids, rows[:, 0].astype(np.int64))
+        ids, loc = ids[keep], loc[keep]
+    return ids, loc
+
+
+def extract_psfs(xml_path, ctx: Context, label, psf_size=(19, 19, 25), all_points=False, view_selection=None,
+                 xml_out=None, dry_run=False, shard=(0, 1), allgather=None):
+    """`./extract-psfs -x dataset.xml -l beads [--psfSize 19,19,25] [--allPoints] [view selection] [-xo out.xml]
+    [--dryRun]`: the point spread function of every selected view as the average of the full-resolution image around
+    its beads, BigStitcher's "Extract PSFs" (mvrecon PSFExtraction, recalled; PARITY_GAPS Q1-Q5), which multi-view
+    deconvolution reads.  BigStitcher-Spark has no such command.
+
+    1. Points: the label's `interestpoints/loc` of the view, full-resolution pixels as stored, in ascending id; only
+       the ids with a correspondence of that label (the beads the registration used) unless ``all_points``.
+    2. Every PSF voxel o in [-h, h] (h = (psf_size - 1) / 2, sizes {x, y, z}, odd) of every point p is the n-linear
+       sample at p + o of level s0 with border extension (PARITY_GAPS #37), summed over the points in float64 on the
+       device (bs_psf_accumulate), run of points by run of points (psf_slabs), each run's s0 window read and uploaded
+       on its own; the sum is carried from run to run, so it does not depend on the runs.  A view is read at most
+       once over the box of its points' taps, whatever the id order.
+    3. PSF = sum / number of points, as float32 [z, y, x]; not normalised.
+    4. Unless ``dry_run``: one float32 TIFF per view, `psfs/psf_t{tp}_vs{setup}.tif` under the base path of the XML
+       written (``xml_out``, default ``xml_path``), and its <PointSpreadFunction> in the XML (entries of other views
+       kept), saved with a `~1` backup.
+
+    Returns {(tp, setup): (psf float32 [z, y, x], number of points)}.  ValueError, with nothing written, for a size
+    that is not three odd integers >= 1, a label no view has, a selected view without the label, and a selected view
+    with no usable points.  MemoryError, before any view is extracted, when the device cannot hold the largest window
+    (the box of all a view's taps when its ids do not follow space).
+
+    Multi-GPU: rank r of w (``shard``) extracts views[r::w]; ``allgather(obj) -> [obj of every rank]`` merges the
+    results and rank 0 writes."""
+    size = tuple(psf_size)
+    if len(size) != 3 or any(isinstance(s, bool) or int(s) != s or s < 1 or int(s) % 2 == 0 for s in size):
+        raise ValueError(f"extract-psfs: --psfSize {psf_size} is not three odd integers >= 1")
+    size = tuple(int(s) for s in size)
+    data = SpimData2.load(xml_path)
+    views = data.select_views(**view_selection) if view_selection else data.view_ids()
+    listed = data.interest_points()
+    if not any(label in labels for labels in listed.values()):
+        raise ValueError(f"extract-psfs: no view has interest points labelled '{label}'")
+    missing = [v for v in views if label not in listed.get(v, {})]
+    if missing:
+        raise ValueError(f"extract-psfs: views {missing} have no interest points labelled '{label}'")
+    store = bn5.N5Store(os.path.join(_ip_base(xml_path, data), "interestpoints.n5"))
+    ips = _InterestPoints(store, views, [label], {v: data.model(*v) for v in views}, tables=True)
+    missing = [v for v in views if (v, label) not in ips.loc]
+    if missing:
+        raise ValueError(f"extract-psfs: interestpoints.n5 holds no points labelled '{label}' for views {missing}")
+    points = {v: _psf_points(ips, v, label, all_points)[1] for v in views}
+    empty = [v for v in views if len(points[v]) == 0]
+    if empty:
+        raise ValueError(f"extract-psfs: views {empty} have no " + ("" if all_points else "corresponding ") +
+                         f"interest points labelled '{label}'" + ("" if all_points else " (use --allPoints)"))
+    src = bvs.open_views(data)
+    rank, world = shard
+    plans, largest = {}, 0
+    for v in views[rank::world]:
+        full = src.level_dims(v, 0)
+        item = np.dtype(src.level_dtype(v, 0)).itemsize
+        plans[v] = (full, psf_slabs(points[v], size, full, max(1, PSF_SLAB_BYTES // item)))
+        largest = max([largest] + [int(np.prod(s[3])) * item for s in plans[v][1]])
+    _check_device_memory(ctx, largest + 8 * (math.prod(size) + 3 * max([len(points[v]) for v in plans] or [0])),
+                         f"an s0 window of {largest / 2**30:.2f} GiB", "extract-psfs",
+                         "free device memory, or extract fewer views per device")
+    results = {}
+    for v, (full, slabs) in plans.items():
+        total = np.zeros(size[::-1], dtype=np.float64)
+        for start, stop, wmin, wsize in slabs:
+            h = ctx.volume_upload(src.read_region(v, 0, tuple(int(x) for x in wmin), tuple(int(x) for x in wsize)))
+            try:
+                ctx.psf_accumulate(h, wmin, full, points[v][start:stop], size, total)
+            finally:
+                ctx.volume_free(h)
+        results[v] = ((total / len(points[v])).astype(np.float32), len(points[v]))
+    if world > 1:
+        merged = {}
+        for part in allgather(results):
+            merged.update(part)
+        results = {v: merged[v] for v in views if v in merged}
+        if rank != 0:
+            return results
+    if dry_run:
+        return results
+    out_xml = xml_out or xml_path
+    folder = os.path.join(_ip_base(out_xml, data), PSF_DIR)
+    os.makedirs(folder, exist_ok=True)
+    for v, (psf, _) in sorted(results.items()):
+        btiff.write_float32_stack(os.path.join(folder, psf_file_name(v)), psf)
+    data.set_point_spread_functions({v: psf_file_name(v) for v in results})
+    data.save(out_xml)
+    return results

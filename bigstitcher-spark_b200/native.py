@@ -141,7 +141,7 @@ SYMBOLS = [
     "bs_descriptors_build", "bs_descriptors_free", "bs_descriptors_neighbors", "bs_descriptors_match",
     "bs_solve_tiles",
     "bs_intensity_pair_candidates", "bs_intensity_candidates_get", "bs_intensity_candidates_free", "bs_intensity_ransac",
-    "bs_intensity_apply", "bs_min_filter", "bs_volume_min_max", "bs_threshold_bbox",
+    "bs_intensity_apply", "bs_min_filter", "bs_volume_min_max", "bs_threshold_bbox", "bs_psf_accumulate",
 ]
 
 #: fixed parameters of the reference's non-rigid fusion (J/SparkNonRigidFusion.java:373-383): control-point distance
@@ -234,6 +234,7 @@ def load_library():
     lib.bs_min_filter.argtypes = [vp, ull, P(ip), P(ull)]
     lib.bs_volume_min_max.argtypes = [vp, ull, P(dbl)]
     lib.bs_threshold_bbox.argtypes = [vp, ull, dbl, P(ll), P(ll), P(ll)]
+    lib.bs_psf_accumulate.argtypes = [vp, ull, P(ll), P(ll), P(dbl), ip, P(ip), P(dbl)]
     _lib = lib
     return lib
 
@@ -911,6 +912,24 @@ class Context:
         mn, mx, n = (C.c_longlong * 3)(), (C.c_longlong * 3)(), C.c_longlong()
         self._check(self.lib.bs_threshold_bbox(self.h, handle, float(t), mn, mx, C.byref(n)))
         return tuple(mn), tuple(mx), n.value
+
+    # -- extract-psfs
+    def psf_accumulate(self, handle: int, window_min_xyz, full_dims_xyz, points_xyz, psf_size_xyz, sum=None):
+        """Add, for every point in the order given, the n-linear samples (PARITY_GAPS #37, border extension of the
+        full view of size ``full_dims_xyz``) of the PSF box of odd size ``psf_size_xyz`` around the point to ``sum``
+        (float64 [sz, sy, sx], updated in place; zeros when None) and return it.  The resident volume is the window of
+        the view's full-resolution level that starts at ``window_min_xyz``; points are full-resolution pixels."""
+        s = [int(v) for v in psf_size_xyz]
+        if sum is None:
+            sum = np.zeros(s[::-1], dtype=np.float64)
+        if sum.dtype != np.float64 or not sum.flags.c_contiguous or sum.size != int(np.prod(s)):
+            raise ValueError(f"psf_accumulate: sum must be a C-contiguous float64 array of {s[::-1]}")
+        pts = np.ascontiguousarray(np.asarray(points_xyz, dtype=np.float64).reshape(-1, 3))
+        self._check(self.lib.bs_psf_accumulate(
+            self.h, handle, (C.c_longlong * 3)(*[int(v) for v in window_min_xyz]),
+            (C.c_longlong * 3)(*[int(v) for v in full_dims_xyz]), pts.ctypes.data_as(C.POINTER(C.c_double)), len(pts),
+            (C.c_int * 3)(*s), sum.ctypes.data_as(C.POINTER(C.c_double))))
+        return sum
 
     @staticmethod
     def comm_unique_id() -> bytes:

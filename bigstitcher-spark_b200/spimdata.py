@@ -543,6 +543,27 @@ class SpimData2:
         ET.SubElement(b, "min").text = " ".join(str(int(v)) for v in bb_min)
         ET.SubElement(b, "max").text = " ".join(str(int(v)) for v in bb_max)
 
+    # ------------------------------------------------------------------ point spread functions
+    def point_spread_functions(self):
+        """{(tp, setup): file name relative to `psfs/` next to the XML} of <PointSpreadFunctions> (mvrecon
+        XmlIoPointSpreadFunctions, recalled: <PointSpreadFunction timepoint= setup=><file>...</file>)."""
+        psfs = self.root.find("PointSpreadFunctions")
+        return {(int(p.get("timepoint")), int(p.get("setup"))): (p.findtext("file") or "").strip()
+                for p in (psfs.findall("PointSpreadFunction") if psfs is not None else [])}
+
+    def set_point_spread_functions(self, files):
+        """Add or replace the <PointSpreadFunction> of every view in ``files`` ({(tp, setup): file name}); the entries
+        of other views are kept.  Entries stay ordered by (timepoint, setup)."""
+        psfs = self.root.find("PointSpreadFunctions")
+        if psfs is None:
+            psfs = ET.SubElement(self.root, "PointSpreadFunctions")
+        entries = {**self.point_spread_functions(), **{(int(t), int(s)): str(f) for (t, s), f in files.items()}}
+        for p in list(psfs):
+            psfs.remove(p)
+        for (tp, setup), f in sorted(entries.items()):
+            p = ET.SubElement(psfs, "PointSpreadFunction", timepoint=str(tp), setup=str(setup))
+            ET.SubElement(p, "file").text = f
+
 
 # ---------------------------------------------------------------------------------------------
 def fusion_project(xml_path, dims_xyz, num_channels, num_timepoints, anisotropy_factor=None) -> SpimData2:

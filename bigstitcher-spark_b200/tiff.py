@@ -13,6 +13,8 @@ sample type) on the integer types.  Three layouts give the (c, z, t) planes of a
     `<TiffData IFD= FirstZ= FirstC= FirstT= PlaneCount=>` in the `DimensionOrder` of its `<Pixels>`, or, without
     `<TiffData>`, the IFDs that follow the planes of the series before it.
 
+Write: ``write_float32_stack``, an uncompressed float32 stack with an ImageJ description (the PSFs of extract-psfs).
+
 Anything else raises NotImplementedError naming the file and what it has (PARITY_GAPS T4).  Regions read only the
 pages, and the strips or tiles of those pages, that they touch; uncompressed rows are read straight into the output
 buffer, one read per run of adjacent rows.
@@ -335,3 +337,35 @@ def _read_plane(tf, page, shift, y0, y1, x0, x1, dst):
         s = _decode(tf, page, page.offsets[k] + shift, page.counts[k], n, w)
         a0, a1 = max(y0, k * rps), min(y1, k * rps + n)
         dst[a0 - y0:a1 - y0] = s[a0 - k * rps:a1 - k * rps, x0:x1]
+
+
+def write_float32_stack(path, vol):
+    """Write ``vol`` [z, y, x] as an uncompressed little-endian float32 TIFF: one page per z-plane, one strip per page,
+    and the ImageJ description `images=z slices=z` in the first page, so ImageJ / Fiji open it as a z-stack."""
+    vol = np.ascontiguousarray(vol, dtype="<f4")
+    if vol.ndim != 3 or 0 in vol.shape:
+        raise ValueError(f"write_float32_stack: a non-empty [z, y, x] volume, not shape {vol.shape}")
+    nz, h, w = vol.shape
+    desc = f"ImageJ=1.11a\nimages={nz}\nslices={nz}\nloop=false\n".encode("ascii") + b"\0"
+    plane = h * w * 4
+    data_at = 8 + len(desc) + len(desc) % 2            # word-aligned pixel data, so every IFD is word-aligned too
+    ifd_at = data_at + nz * plane
+    out = bytearray(struct.pack("<2sHI", b"II", 42, ifd_at))
+    out += desc + b"\0" * (len(desc) % 2)
+    out += vol.tobytes()
+    for z in range(nz):
+        entries = [(_WIDTH, 4, 1, w), (_LENGTH, 4, 1, h), (_BITS, 3, 1, 32), (_COMPRESSION, 3, 1, 1),
+                   (_PHOTOMETRIC, 3, 1, 1)]
+        if z == 0:
+            entries.append((_DESCRIPTION, 2, len(desc), 8))
+        entries += [(_STRIP_OFFSETS, 4, 1, data_at + z * plane), (_SAMPLES, 3, 1, 1), (_ROWS_PER_STRIP, 4, 1, h),
+                    (_STRIP_COUNTS, 4, 1, plane), (_SAMPLE_FORMAT, 3, 1, 3)]
+        here = len(out)
+        nxt = here + 2 + 12 * len(entries) + 4 if z + 1 < nz else 0
+        out += struct.pack("<H", len(entries))
+        for tag, typ, count, value in entries:
+            inline = struct.pack("<HH", value, 0) if typ == 3 else struct.pack("<I", value)   # SHORTs left-justified
+            out += struct.pack("<HHI", tag, typ, count) + inline
+        out += struct.pack("<I", nxt)
+    with open(path, "wb") as f:
+        f.write(bytes(out))

@@ -520,6 +520,20 @@ int bs_volume_min_max(bs_ctx* ctx, unsigned long long vol_handle, double out[2])
 int bs_threshold_bbox(bs_ctx* ctx, unsigned long long vol_handle, double t, long long min[3], long long max[3],
                       long long* count);
 
+/* ---------------------------------------------------------------- extract-psfs
+ * The bead average of mvrecon's PSFExtraction (recalled).  Additive: the ABI version stays 107.
+ *
+ * The resident volume (U8 / U16 / F32) is the window [window_min, window_min + dims) of a full-resolution view of size
+ * full_dims.  For every PSF voxel o in [-h, h] (h = (psf_size - 1) / 2, x fastest) and every point p, in the order
+ * given: sum[o] += (double) nlinear(p + o), where nlinear is bs_sample_nlinear's arithmetic (PARITY_GAPS #37: double
+ * weights, each corner term (float)(v w), summed in float) on the border extension of the FULL view; the caller's
+ * window must hold every tap that extension reaches.  sum: host [sz][sy][sx] doubles, read and written, so a caller
+ * that passes the points in several calls, in order, gets exactly the one-call result.  n = 0 leaves sum as it is.
+ * BS_ERR_ARG for an even or non-positive psf_size, n < 0, NULL pointers, an unknown handle, or a window outside
+ * full_dims.  Profile tag "psf". */
+int bs_psf_accumulate(bs_ctx* ctx, unsigned long long vol_handle, const long long window_min[3],
+                      const long long full_dims[3], const double* points_xyz, int n, const int psf_size[3], double* sum);
+
 #ifdef __cplusplus
 }
 #endif

@@ -840,3 +840,30 @@ JF(jlong, thresholdBbox)(JNIEnv* env, jclass, jlong ctx, jlong handle, jdouble t
     env->SetLongArrayRegion(max, 0, 3, b);
     return (jlong)n;
 }
+
+// ------------------------------------------------------------------------------------------------ extract-psfs
+// windowMin / fullDims long[3] {x, y, z}, points double[3n] {x, y, z}, psfSize int[3]; sum double[sz * sy * sx]
+// (x fastest), read and added to (PSFExtraction's bead average before the division by n)
+JF(void, psfAccumulate)(JNIEnv* env, jclass, jlong ctx, jlong handle, jlongArray windowMin, jlongArray fullDims,
+                        jdoubleArray points, jintArray psfSize, jdoubleArray sum) {
+    jlong w[3], f[3];
+    jint s[3];
+    env->GetLongArrayRegion(windowMin, 0, 3, w);
+    env->GetLongArrayRegion(fullDims, 0, 3, f);
+    env->GetIntArrayRegion(psfSize, 0, 3, s);
+    const long long wm[3] = {w[0], w[1], w[2]}, fd[3] = {f[0], f[1], f[2]};
+    const int ps[3] = {s[0], s[1], s[2]};
+    const jint n = env->GetArrayLength(points) / 3;
+    std::vector<jdouble> p((size_t)n * 3);
+    env->GetDoubleArrayRegion(points, 0, n * 3, p.data());
+    const jsize ns = env->GetArrayLength(sum);
+    std::vector<jdouble> acc((size_t)ns);
+    env->GetDoubleArrayRegion(sum, 0, ns, acc.data());
+    if ((long long)ns != (long long)ps[0] * ps[1] * ps[2]) {
+        jclass ex = env->FindClass("java/lang/IllegalArgumentException");
+        if (ex) env->ThrowNew(ex, "psfAccumulate: sum must hold psfSize[0] * psfSize[1] * psfSize[2] doubles");
+        return;
+    }
+    if (failed(env, ctx, bs_psf_accumulate(C(ctx), (unsigned long long)handle, wm, fd, p.data(), n, ps, acc.data()))) return;
+    env->SetDoubleArrayRegion(sum, 0, ns, acc.data());
+}

@@ -145,4 +145,9 @@ public final class BsNative
 	public static native void volumeMinMax( long ctx, long handle, double[] out );
 	/** the voxels > t of a float32 volume: min / max {x, y, z} (-1 when none); returns their count */
 	public static native long thresholdBbox( long ctx, long handle, double t, long[] min, long[] max );
+
+	/** extract-psfs (PSFExtraction): add the n-linear PSF box of psfSize {x, y, z} (odd) around every point {x, y, z} of
+	 *  a (windowed) full-resolution view volume to sum (psfSize[2] * psfSize[1] * psfSize[0] doubles, x fastest) */
+	public static native void psfAccumulate( long ctx, long handle, long[] windowMin, long[] fullDims, double[] points,
+			int[] psfSize, double[] sum );
 }
