@@ -822,6 +822,17 @@ __device__ __forceinline__ void col540_tw(float2* tw, const float2* __restrict__
 // Every wait is bounded: when a wait expires, its thread records the kernel's code in *err and the CTA stops
 // without writing; the other CTAs see *err and stop as well, and the host turns the code into an error.
 #define PCM_HANDOFF_POLLS (1u << 24)
+// Role probe (tools/pcm_kernel_times.py --probe), compiled in only with -DPCM_XY_PROBE: per CTA of the fused
+// kernel, thread 0's nanoseconds in hand-off waits and from its start to its end, read back after each launch.
+#ifdef PCM_XY_PROBE
+#define PCM_PROBE_CTAS 1024
+__device__ unsigned long long pcm_xy_probe[2 * PCM_PROBE_CTAS];   // [cta][wait ns, total ns]
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+#endif
 struct Handoff {
     int* ready = nullptr;   // [Pz]; nullptr in the standalone kernels, where every hook below is a no-op
     int* done = nullptr;    // [Pz]
@@ -839,6 +850,13 @@ __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
 // one thread: poll *c until it reaches `full`; false when the poll budget is spent or another wait has expired
 __device__ __forceinline__ bool handoff_wait(const int* c, int full, const Handoff& h) {
     unsigned int ns = 32;
+#ifdef PCM_XY_PROBE
+    const unsigned long long t0 = globaltimer_ns();
+    struct Acc {
+        unsigned long long t0;
+        __device__ ~Acc() { pcm_xy_probe[2 * blockIdx.x] += globaltimer_ns() - t0; }
+    } acc{t0};
+#endif
     for (unsigned int i = 0; i < PCM_HANDOFF_POLLS; ++i) {
         if (ld_acquire_gpu(c) >= full) {
             __threadfence();   // the whole CTA reads the plane after the barrier that follows
@@ -855,6 +873,12 @@ __device__ __forceinline__ bool handoff_wait(const int* c, int full, const Hando
 __device__ __forceinline__ bool handoff_ready(const Handoff& h, int z) {
     return !h.ready || handoff_wait(h.ready + z, h.ready_full, h);
 }
+// consumer, one look without waiting: plane z is complete
+__device__ __forceinline__ bool handoff_ready_now(const Handoff& h, int z) {
+    if (ld_acquire_gpu(h.ready + z) < h.ready_full) return false;
+    __threadfence();
+    return true;
+}
 // producer: plane z may be stored into (plane z - window has been read out)
 __device__ __forceinline__ bool handoff_window(const Handoff& h, int z) {
     return !h.ready || z < h.window || handoff_wait(h.done + z - h.window, h.done_full, h);
@@ -869,73 +893,63 @@ __device__ __forceinline__ void handoff_publish(const Handoff& h, int z, int n) 
 __device__ __forceinline__ void handoff_consume(const Handoff& h, int z, int n) {
     if (h.ready) atomicAdd(h.done + z, n);
 }
+__device__ __forceinline__ bool mbar_try_wait(unsigned long long* bar, unsigned int parity) {
+    unsigned int done;
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
+        "selp.u32 %0, 1, 0, p;\n"
+        "}\n"
+        : "=r"(done)
+        : "r"(smem_u32(bar)), "r"(parity)
+        : "memory");
+    return done != 0;
+}
+// the phase of `bar` with this parity has completed, within the poll budget of the hand-off waits; with watch, also
+// false as soon as another wait has expired
+__device__ __forceinline__ bool mbar_wait_bounded(unsigned long long* bar, unsigned int parity, const Handoff& h,
+                                                  bool watch) {
+    for (unsigned int i = 0; i < PCM_HANDOFF_POLLS; ++i) {
+        if (mbar_try_wait(bar, parity)) return true;
+        if (watch && *(volatile int*)h.err) return false;
+    }
+    atomicCAS(h.err, 0, h.code);
+    return false;
+}
 // f(z, n) for each plane z of Py lines that lines [l0, l1) touch, with the n lines that fall into it
 template <class Fn>
 __device__ __forceinline__ void for_planes(int l0, int l1, int Py, Fn&& f) {
     for (int z = l0 / Py; z * Py < l1; ++z) f(z, min(l1, (z + 1) * Py) - max(l0, z * Py));
 }
 
-// Forward y FFT, in place, of tiles t, t + stride, ... < n_tiles on F (RegFft2<20, 27>), ptr(t) the tile's first
-// element.  X0 holds two exchange buffers (one barrier per tile); the next tile's loads go out into the stage-1
-// registers once stage 1 has written them out (in the fused roles after the barrier, which carries the hand-off
-// wait), and are in flight under stage 2 and the stores.
-//   Y_ALONE     k_fft_col540
-//   Y_CONSUMER  y role of k_fft_xy_col540: a tile's loads wait for its plane; thread 0 counts a tile as taken
-//               after its own stage 1, before it waits for the next tile's plane, so a tile's count never waits on
-//               a later plane; the spectra go to DRAM as streaming (evict-first) stores so as not to push the x
-//               output that is still waiting out of L2
-enum { Y_ALONE, Y_CONSUMER };
-template <class F, int MODE, class Ptr>
-__device__ __forceinline__ void col540_y_tiles(float2* X0, float2* tw, const float2* __restrict__ tw_g, int t, int stride,
-                                               int n_tiles, long long estride, int tiles_per_plane, Ptr ptr,
-                                               const Handoff& h) {
-    static_assert(F::N == 540, "RegFft2<20, 27>");
-    bool ok = true;
-    if (MODE == Y_CONSUMER && threadIdx.x == 0 && t < n_tiles) ok = handoff_ready(h, t / tiles_per_plane);
-    if (MODE == Y_CONSUMER && __syncthreads_or(!ok)) return;
-    typename F::In v;
-    if (t < n_tiles) F::load(v, ptr(t), estride);
-    col540_tw(tw, tw_g);
-    __syncthreads();
-    for (int it = 0; t < n_tiles; t += stride, ++it) {
-        float2* x = X0 + (it & 1) * F::XSIZE;
-        F::stage1(v, x, tw);
-        const int tn = t + stride;
-        if (MODE == Y_ALONE) {
-            if (tn < n_tiles) F::load(v, ptr(tn), estride);
-            __syncthreads();
-        } else {
-            if (threadIdx.x == 0) {
-                handoff_consume(h, t / tiles_per_plane, 1);
-                if (tn < n_tiles) ok = handoff_ready(h, tn / tiles_per_plane);
-            }
-            if (__syncthreads_or(!ok)) return;
-            if (tn < n_tiles) F::load(v, ptr(tn), estride);   // the next tile's plane is complete from here on
-        }
-        F::stage2(x, [&](const float2 (&w)[27], int, int k1, int c) {
-            float2* g = ptr(t);
-            if (MODE == Y_CONSUMER) {
-                float2* p = g + (long long)k1 * estride + c;
-#pragma unroll
-                for (int k2 = 0; k2 < 27; ++k2) __stcs(p + (long long)(20 * k2) * estride, w[k2]);
-            } else {
-                F::store(w, g, estride, k1, c);
-            }
-        });
-    }
-}
-
-// forward y FFT in place, tiles of both spectra (p.n_tiles = tiles_x * n_other * n_img)
+// forward y FFT in place, tiles of both spectra (p.n_tiles = tiles_x * n_other * n_img).  Two exchange buffers (one
+// barrier per tile); the next tile's loads go out into the stage-1 registers once stage 1 has written them out, and
+// are in flight under stage 2 and the stores.
 __global__ void __launch_bounds__(COL540_NT, 1) k_fft_col540(const __grid_constant__ StridedPipeArgs p) {
     const StridedArgs& a = p.s;
     float2* tw = bs_sm;
+    float2* X0 = bs_sm + Col540::N;
     auto tile_ptr = [&](int t) -> float2* {
         const int tx = t % p.tiles_x, r = t / p.tiles_x;
         const int o = r % p.n_other, im = r / p.n_other;
         return (im ? a.b : a.a) + (size_t)o * a.ostride + (size_t)tx * COL540_TC;
     };
-    col540_y_tiles<Col540, Y_ALONE>(bs_sm + Col540::N, tw, a.tw, blockIdx.x, gridDim.x, p.n_tiles, a.estride, 1, tile_ptr,
-                                    Handoff());
+    int t = blockIdx.x;
+    Col540::In v;
+    if (t < p.n_tiles) Col540::load(v, tile_ptr(t), a.estride);
+    col540_tw(tw, a.tw);
+    __syncthreads();
+    for (int it = 0; t < p.n_tiles; t += gridDim.x, ++it) {
+        float2* x = X0 + (it & 1) * Col540::XSIZE;
+        Col540::stage1(v, x, tw);
+        const int tn = t + gridDim.x;
+        if (tn < p.n_tiles) Col540::load(v, tile_ptr(tn), a.estride);
+        __syncthreads();
+        Col540::stage2(x, [&](const float2 (&w)[27], int, int k1, int c) {
+            Col540::store(w, tile_ptr(t), a.estride, k1, c);
+        });
+    }
 }
 
 // z cross-power: forward z FFT of A and B, unit-magnitude normalisation and conj(A) * B, then the forward FFT of
@@ -1339,8 +1353,16 @@ __global__ void __launch_bounds__(COL540X_NT, 1) k_fft_x_c2r_col540(const __grid
 // the lines each tile stores per plane; the others run y tiles (540 rows x 16 columns) plane-major: the 17 column
 // tiles of A and of B of plane z, then plane z + 1.  A y tile waits until its plane has all Py lines.
 // The y role runs Col540X (RegFft2<20, 27> on 448 threads, one stage-1 item per thread): each item computes what
-// k_fft_col540's does, so the spectra are bit-identical to the five-pass chain's.  It uses the x role's largest
-// shared-memory regions as its two exchange buffers.
+// k_fft_col540's does, so the spectra are bit-identical to the five-pass chain's.
+// Its tiles reach shared memory by tensor-map copies (XY_YBOXES boxes of 32 floats x 180 rows x 1 plane), as in
+// k_fft_xpower_col540, into a ring of three buffers: tile i of the CTA lands in buffer i % 3 and completes phase
+// i / 3 of that buffer's mbarrier.  Stage 1 runs in place on the staged tile, stage 2 reads it back and stores the
+// spectrum with streaming (evict-first) stores, so as not to push the x output that is still waiting out of L2.
+// After the barrier that ends tile i's stage 1, buffer (i + 2) % 3 is free and thread 0 issues the copies that
+// are not out yet: tile i + 1 once its plane is complete (it waits for that), then tile i + 2 if one look finds
+// its plane complete (else at the next tile).  So up to two copies are in flight under stage 2 and the stores, and
+// no copy goes out for a plane that is not complete.  Thread 0 counts tile i as taken after its own stage 1 of it,
+// before that barrier, so a tile's count never waits on a later plane.
 // Forward progress: all CTAs are co-resident (cooperative launch, one CTA per SM).  Each role takes its tiles in
 // ascending plane order.  A y tile waits only on x tiles of its own plane (its count in done[] waits on nothing), and
 // an x tile waits only on y tiles `window` >= 2 planes behind the last plane it stores into.  So the lowest plane p
@@ -1348,30 +1370,111 @@ __global__ void __launch_bounds__(COL540X_NT, 1) k_fft_x_c2r_col540(const __grid
 // and every earlier tile of each CTA is in a plane no higher.
 // The inverse pair (y, then x C2R) fused the same way measured slower than the two kernels (DESIGN.md), so it
 // stays two launches.
+#define XY_YBOXES 3
+static_assert(Col540X::N % XY_YBOXES == 0 && Col540X::N / XY_YBOXES <= 256, "a TMA box has at most 256 rows");
 struct XYCol540Args {
+    CUtensorMap tm[2];   // the two half spectra as [Pz][Py][2 pitch] floats
     XR2CCol540Args x;
     const float2* tw_y;
     int kx;   // CTAs of the x role
     Handoff h;
 };
+// the y role's shared memory: three tile buffers, the twiddles, one mbarrier per buffer
+constexpr size_t XY_YSMEM = (3 * (size_t)Col540X::XSIZE + Col540X::N) * sizeof(float2) + 3 * sizeof(unsigned long long);
+static_assert(XY_YSMEM <= PCM_SMEM_MAX, "y role shared memory");
+
+// Tiles t0, t0 + stride, ... of the y role
+__device__ __forceinline__ void xy_y_tiles(const XYCol540Args& P, int t0, int stride) {
+    const XR2CArgs& a = P.x.x;
+    const Handoff& h = P.h;
+    constexpr int rows = Col540X::N / XY_YBOXES;
+    float2* X0 = bs_sm;   // the copies need 128-byte aligned targets: buffers first
+    float2* tw = X0 + 3 * Col540X::XSIZE;
+    unsigned long long* bars = reinterpret_cast<unsigned long long*>(tw + Col540X::N);
+    const int tiles_x = a.pitch / COL540_TC, per_plane = 2 * tiles_x;
+    const long long ostride = (long long)a.Py * a.pitch;
+    const int n = max(0, (a.Pz * per_plane - t0 + stride - 1) / stride);   // this CTA's tiles
+    auto plane = [&](int i) { return (t0 + i * stride) / per_plane; };
+    // thread 0: copy tile i into buffer i % 3, once its plane is known to be complete.  The proxy fences order the
+    // acquire of the plane before the copy's global reads, and the generic-proxy accesses to the buffer before the
+    // barrier that released it ahead of the copy's writes.
+    auto fetch = [&](int i) {
+        const int u = t0 + i * stride, z = u / per_plane, j = u - z * per_plane, im = j / tiles_x;
+        float2* dst = X0 + (i % 3) * Col540X::XSIZE;
+        asm volatile("fence.proxy.async.global;" ::: "memory");
+        fence_proxy_async_smem();
+        mbar_expect_tx(&bars[i % 3], Col540X::XSIZE * sizeof(float2));
+#pragma unroll
+        for (int k = 0; k < XY_YBOXES; ++k)
+            tma_load_3d(dst + k * rows * COL540_TC, &P.tm[im], (j - im * tiles_x) * 2 * COL540_TC, k * rows, z,
+                        &bars[i % 3]);
+    };
+    int issued = 0;   // thread 0: tiles [0, issued) have been copied
+    // thread 0, with tiles [0, i) read out: wait for tiles [i, issued) to land, so that no copy outlives the CTA
+    auto drain = [&](int i) {
+        for (; i < issued; ++i) mbar_wait_bounded(&bars[i % 3], (i / 3) & 1u, h, false);
+    };
+    if (threadIdx.x == 0) {
+        for (int b = 0; b < 3; ++b) mbar_init(&bars[b], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    col540_tw(tw, P.tw_y);
+    __syncthreads();
+    bool ok = true;
+    if (threadIdx.x == 0 && n > 0) {
+        ok = handoff_ready(h, plane(0));
+        if (ok) fetch(issued++);
+        if (ok && n > 1 && handoff_ready_now(h, plane(1))) fetch(issued++);
+    }
+    if (__syncthreads_or(!ok)) {
+        if (threadIdx.x == 0) drain(0);
+        return;
+    }
+    Col540X::In v;
+    for (int i = 0; i < n; ++i) {
+        float2* X = X0 + (i % 3) * Col540X::XSIZE;
+        if (ok) ok = mbar_wait_bounded(&bars[i % 3], (i / 3) & 1u, h, true);
+        if (ok) {
+            Col540X::load_shared(v, X);
+            Col540X::stage1(v, X, tw);
+            if (threadIdx.x == 0) handoff_consume(h, plane(i), 1);
+        }
+        // X's stage 1 is complete; tile i - 1's stage 2 has read buffer (i + 2) % 3 out
+        if (__syncthreads_or(!ok)) {
+            if (threadIdx.x == 0) drain(i);
+            return;
+        }
+        if (threadIdx.x == 0) {
+            if (issued == i + 1 && i + 1 < n) {
+                ok = handoff_ready(h, plane(i + 1));
+                if (ok) fetch(issued++);
+            }
+            if (ok && issued == i + 2 && i + 2 < n && handoff_ready_now(h, plane(i + 2))) fetch(issued++);
+        }
+        const int u = t0 + i * stride, z = u / per_plane, j = u - z * per_plane, im = j / tiles_x;
+        float2* g = a.spec[im] + z * ostride + (j - im * tiles_x) * COL540_TC;
+        Col540X::stage2(X, [&](const float2 (&w)[27], int, int k1, int c) {
+            float2* p = g + (long long)k1 * a.pitch + c;
+#pragma unroll
+            for (int k2 = 0; k2 < 27; ++k2) __stcs(p + (long long)(20 * k2) * a.pitch, w[k2]);
+        });
+    }
+}
 
 __global__ void __launch_bounds__(COL540X_NT, 1) k_fft_xy_col540(const __grid_constant__ XYCol540Args P) {
+#ifdef PCM_XY_PROBE
+    struct Total {
+        unsigned long long t0 = globaltimer_ns();
+        __device__ ~Total() {
+            if (threadIdx.x == 0) pcm_xy_probe[2 * blockIdx.x + 1] += globaltimer_ns() - t0;
+        }
+    } total;
+#endif
     if ((int)blockIdx.x < P.kx) {
         x_r2c_col540_tiles(P.x, blockIdx.x, P.kx, P.h);
         return;
     }
-    const XR2CArgs& a = P.x.x;
-    float2* X0 = bs_sm;                                           // r2c's X and Y regions
-    float2* tw = X0 + Col540X::XSIZE + COL540_TC * COL540_XLP;   // r2c's twiddle region
-    static_assert(COL540_TC * COL540_XLP >= Col540X::XSIZE, "exchange buffers");
-    const int tiles_x = a.pitch / COL540_TC, per_plane = 2 * tiles_x;
-    const long long ostride = (long long)a.Py * a.pitch;
-    auto ptr = [&](int u) -> float2* {
-        const int z = u / per_plane, j = u - z * per_plane, im = j / tiles_x;
-        return a.spec[im] + z * ostride + (j - im * tiles_x) * COL540_TC;
-    };
-    col540_y_tiles<Col540X, Y_CONSUMER>(X0, tw, P.tw_y, blockIdx.x - P.kx, gridDim.x - P.kx, a.Pz * per_plane, a.pitch,
-                                        per_plane, ptr, P.h);
+    xy_y_tiles(P, blockIdx.x - P.kx, gridDim.x - P.kx);
 }
 
 
@@ -2318,6 +2421,21 @@ static int set_smem(bs_ctx* ctx, const void* fn) {
     return BS_OK;
 }
 
+// 3-D tensor maps (float32, gdim / gstr / box innermost first) of the two spectra a and b
+static int spectrum_maps(bs_ctx* ctx, const void* a, const void* b, const cuuint64_t gdim[3], const cuuint64_t gstr[2],
+                         const cuuint32_t box[3], CUtensorMap tm[2]) {
+    auto enc = bs_tensor_map_encoder();
+    if (!enc) return bs_set_error(ctx, BS_ERR_CUDA, "pcm: cuTensorMapEncodeTiled is not available");
+    const cuuint32_t estr[3] = {1, 1, 1};
+    for (int i = 0; i < 2; ++i) {
+        const CUresult r = enc(&tm[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(i ? b : a), gdim, gstr, box,
+                               estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                               CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (r != CUDA_SUCCESS) return bs_set_error(ctx, BS_ERR_CUDA, "pcm: cuTensorMapEncodeTiled failed (%d)", (int)r);
+    }
+    return BS_OK;
+}
+
 // n_img: 1 or 2 spectra through k_fft_col540 (y), 0 for the cross-power k_fft_xpower_col540 (z)
 static int launch_col540(bs_ctx* ctx, const StridedArgs& a, int tiles_x, int n_other, int n_img) {
     StridedPipeArgs pp;
@@ -2334,18 +2452,11 @@ static int launch_col540(bs_ctx* ctx, const StridedArgs& a, int tiles_x, int n_o
     // z pass: spectra [Pz = 540][Py = n_other][pitch] as floats, one 128 B x 1 x 180-row box per copy
     XpowerCol540Args xa;
     xa.p = pp;
-    auto enc = bs_tensor_map_encoder();
-    if (!enc) return bs_set_error(ctx, BS_ERR_CUDA, "pcm: cuTensorMapEncodeTiled is not available");
     const cuuint64_t gdim[3] = {(cuuint64_t)tiles_x * 2 * COL540_TC, (cuuint64_t)n_other, (cuuint64_t)Col540::N};
     const cuuint64_t gstr[2] = {(cuuint64_t)a.ostride * sizeof(float2), (cuuint64_t)a.estride * sizeof(float2)};
     const cuuint32_t box[3] = {2 * COL540_TC, 1, Col540::N / COL540_ZBOXES};
-    const cuuint32_t estr[3] = {1, 1, 1};
-    for (int i = 0; i < 2; ++i) {
-        const CUresult r = enc(&xa.tm[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, i ? (void*)a.b : (void*)a.a, gdim, gstr, box,
-                               estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                               CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return bs_set_error(ctx, BS_ERR_CUDA, "pcm: cuTensorMapEncodeTiled failed (%d)", (int)r);
-    }
+    int rc;
+    if ((rc = spectrum_maps(ctx, a.a, a.b, gdim, gstr, box, xa.tm))) return rc;
     // buffers, twiddles, one mbarrier per buffer
     const size_t smem = (3 * (size_t)Col540::XSIZE + Col540::N) * sizeof(float2) + 3 * sizeof(unsigned long long);
     k_fft_xpower_col540<<<nctas, COL540_NT, smem, ctx->stream>>>(xa);
@@ -2631,10 +2742,10 @@ static int xy_fuse(bs_ctx* ctx, const PcmGeometry& g, const void* fn, size_t sme
     return BS_OK;
 }
 
-// CTAs of k_fft_xy_col540's x role: 74 of 132 measured best (DESIGN.md), scaled to the SM count;
+// CTAs of k_fft_xy_col540's x role: 82 of 132 measured best (DESIGN.md), scaled to the SM count;
 // BS_FFT_XY_KX overrides it
 static int xy_split(bs_ctx* ctx) {
-    return std::max(1, std::min(ctx->sm_count - 1, env_int("BS_FFT_XY_KX", (74 * ctx->sm_count + 66) / 132)));
+    return std::max(1, std::min(ctx->sm_count - 1, env_int("BS_FFT_XY_KX", (82 * ctx->sm_count + 66) / 132)));
 }
 
 // counters in ws.sync; window: as many planes of plane_bytes as fill half of L2 (BS_FFT_XY_WINDOW overrides)
@@ -2682,9 +2793,9 @@ static int pcm_pass_xy(bs_ctx* ctx, const void* d1, const void* d2, int dtype, c
     size_t smem;
     bool fuse = false;
     int rc;
-    if (r2c_col540(ctx, r2c_args(ctx, d1, d2, dtype, g, t), dtype, g, &f.x, &smem) &&
-        (rc = xy_fuse(ctx, g, (const void*)k_fft_xy_col540, smem, &fuse)))
-        return rc;
+    const bool col540 = r2c_col540(ctx, r2c_args(ctx, d1, d2, dtype, g, t), dtype, g, &f.x, &smem);
+    smem = std::max(smem, XY_YSMEM);   // a CTA runs one role: the larger of the two
+    if (col540 && (rc = xy_fuse(ctx, g, (const void*)k_fft_xy_col540, smem, &fuse))) return rc;
     if (!fuse) {
         char i0[PCM_INFO_LEN] = "", i1[PCM_INFO_LEN] = "";
         if ((rc = pcm_pass_x_r2c(ctx, d1, d2, dtype, g, t, i0))) return rc;
@@ -2694,11 +2805,38 @@ static int pcm_pass_xy(bs_ctx* ctx, const void* d1, const void* d2, int dtype, c
     }
     f.tw_y = t->tw[1];
     f.kx = xy_split(ctx);
+    {   // the y role's tiles: 32 floats x 180 rows x 1 plane per box
+        const XR2CArgs& a = f.x.x;
+        const cuuint64_t gdim[3] = {2 * (cuuint64_t)a.pitch, (cuuint64_t)a.Py, (cuuint64_t)a.Pz};
+        const cuuint64_t gstr[2] = {(cuuint64_t)a.pitch * sizeof(float2), (cuuint64_t)a.Py * a.pitch * sizeof(float2)};
+        const cuuint32_t box[3] = {2 * COL540_TC, Col540X::N / XY_YBOXES, 1};
+        if ((rc = spectrum_maps(ctx, a.spec[0], a.spec[1], gdim, gstr, box, f.tm))) return rc;
+    }
     bs_launch_scope sc(ctx, "fft_xy");
     if ((rc = make_handoff(ctx, g, PCM_HANDOFF_XY, g.P[1], 2 * (g.pitch / COL540_TC),
                            2 * (size_t)g.P[1] * g.pitch * sizeof(float2), &f.h)) ||
         (rc = launch_fused(ctx, k_fft_xy_col540, f, smem)))
         return rc;
+#ifdef PCM_XY_PROBE
+    {   // one line per launch: per-role sums over the CTAs of thread 0's busy and hand-off wait time
+        static unsigned long long pr[2 * PCM_PROBE_CTAS];
+        const int n = std::min(ctx->sm_count, PCM_PROBE_CTAS);
+        BS_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        BS_CUDA(ctx, cudaMemcpyFromSymbol(pr, pcm_xy_probe, sizeof(pr)));
+        double busy[2] = {0, 0}, wait[2] = {0, 0};
+        for (int i = 0; i < n; ++i) {
+            busy[i >= f.kx] += 1e-3 * (double)(pr[2 * i + 1] - pr[2 * i]);
+            wait[i >= f.kx] += 1e-3 * (double)pr[2 * i];
+        }
+        memset(pr, 0, sizeof(pr));
+        BS_CUDA(ctx, cudaMemcpyToSymbol(pcm_xy_probe, pr, sizeof(pr)));
+        fprintf(stderr,
+                "pcm_xy_probe {\"kx\": %d, \"ctas\": %d, \"x_busy_us\": %.1f, \"x_wait_us\": %.1f, \"y_busy_us\": %.1f, "
+                "\"y_wait_us\": %.1f, \"line_pairs\": %lld, \"y_columns\": %lld}\n",
+                f.kx, n, busy[0], wait[0], busy[1], wait[1], (long long)g.P[1] * g.P[2],
+                (long long)g.P[2] * 2 * g.pitch);
+    }
+#endif
     pass_info(info, "k_fft_xy_col540", nullptr);
     return BS_OK;
 }
